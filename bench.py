@@ -3,10 +3,10 @@
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
                     [--workload dense|hybrid|rerank|bm25] [--batch B] [--inner R] [--n-docs N] [--dim D] [--top-k K]
-                    [--rerank-k K2] [--shard auto|corpus|queries] [--no-extras]
+                    [--rerank-k K2] [--shard auto|corpus|queries] [--no-extras] [--dump-outputs DIR]
 
 Headline (`value`, `e2e`, `roofline`, `cpu_baseline`) = BASELINE.json configs[1]: 1 M docs x 1024-d, dense-only cosine
-top_k=100 on 1 x B200.  A STEP = `--inner` R batches of `--batch` B queries per GPU through the hot path (defaults 64 x 256
+top_k=100 on 1 x H100.  A STEP = `--inner` R batches of `--batch` B queries per GPU through the hot path (defaults 64 x 256
 dense, 32 x 128 hybrid, 2 x 64 rerank): R is chosen so that the K timed steps hold >= 1 s of device work, and is stated in
 `config`.  The same JSON line carries, after the headline leg (unless --no-extras):
 
@@ -63,6 +63,10 @@ def parse_args():
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the headline leg returned for the last batch of its last timed step "
+                         "to DIR/<workload>_<name>.npy (float64, at most 64 MB: a seeded sample of query rows above "
+                         "that; inputs are seeded, so two builds can be compared output for output)")
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--workload", default="dense", choices=["dense", "hybrid", "rerank", "bm25"])
     ap.add_argument("--rerank-k", type=int, default=10, help="documents kept after the cross-encoder (config 4: 100 -> 10)")
@@ -84,17 +88,42 @@ def parse_args():
                          "(default): the smallest C whose shard fits --gpu-mem-budget-gb")
     ap.add_argument("--corpus-shards", type=int, default=0, help="explicit C (must divide N); overrides --shard")
     ap.add_argument("--gpu-mem-budget-gb", type=float, default=64.0,
-                    help="HBM one GPU may spend on index data under --shard auto (B200: 180 GB)")
+                    help="HBM one GPU may spend on index data under --shard auto (H100: 80 GB)")
     return ap.parse_args()
 
 
+# NVIDIA data-sheet peaks (HBM GB/s, dense bf16 TFLOP/s) by device name: the denominators when no measurement of the same
+# device model is available.  A figure from the data sheet is a bound, never a measurement.
+DATASHEET_PEAKS = {"NVIDIA H100 80GB HBM3": (3350.0, 989.0)}
+
+
 def peaks():
+    """(hbm GB/s, bf16 TFLOP/s, source) for the device bench.py runs on.  MEASURED_PEAKS.json is used only when its
+    `device` field names this device model and its figures do not exceed the device's data sheet; otherwise the data
+    sheet, and the source says why the file was not used.  Unknown device and no usable file: (None, None, source)."""
+    import torch
+
+    dev = torch.cuda.get_device_name()
+    sheet = DATASHEET_PEAKS.get(dev)
+    src_sheet = (f"{dev} data sheet ({sheet[0] / 1e3:.2f} TB/s HBM, {sheet[1]:.0f} TFLOP/s dense bf16), not a measurement"
+                 if sheet else f"no data-sheet peaks known for {dev}")
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(path):
         with open(path) as f:
             p = json.load(f)
-        return float(p["hbm_gbs"]), float(p.get("bf16_tflops_sustained", 1429.5)), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, 1400.0, "fallback (B200_PROFILING.md: 6.65 TB/s, 1.4 PF sustained bf16)"
+        hbm, tf = float(p["hbm_gbs"]), float(p.get("bf16_tflops_sustained", 0.0)) or None
+        if p.get("device") != dev:
+            why = f"MEASURED_PEAKS.json ignored: measured on {p.get('device', 'an unnamed device')}, not {dev}"
+        elif sheet and (hbm > 1.02 * sheet[0] or (tf or 0.0) > 1.02 * sheet[1]):
+            why = "MEASURED_PEAKS.json ignored: its figures exceed this device's data sheet"
+        else:
+            return hbm, tf if tf else (sheet[1] if sheet else None), f"measured on {dev} (MEASURED_PEAKS.json)"
+        src_sheet = f"{src_sheet}; {why}"
+    return (sheet[0], sheet[1], src_sheet) if sheet else (None, None, src_sheet)
+
+
+def _frac(x, peak):
+    return x / peak if peak else None
 
 
 class ClockSampler:
@@ -403,12 +432,15 @@ class Leg:
         ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         self.barrier()
         ev0.record()
+        out = None
         for s in range(steps):
             for r in range(self.inner):
-                self.run_dev(inputs[(s * self.inner + r) % self.ring])
+                out = self.run_dev(inputs[(s * self.inner + r) % self.ring])
         ev1.record()
         self.barrier()
         ms_total = ev0.elapsed_time(ev1)
+        # host copies of the last timed batch's results (the device tensors are buffers the next call reuses)
+        self.last_outputs = [t.detach().cpu().numpy().copy() for t in out] if out is not None else []
         clocks = sampler.stop() if (self.rank == 0 and sample_clocks) else None
         launches = eng.launch_count() - launches0
         prof = {name: eng.profile_read(name) for name in ("dense_scan", "dense_merge", "dense_sample", "bm25_score",
@@ -474,22 +506,14 @@ class Leg:
         avg = scan_ms / max(n_scan, 1)
         ach = alg / (avg * 1e-3) / 1e9 if n_scan else 0.0
         qpl = (self.B * res["n_batches"]) / max(n_scan, 1)
-        kern = ("dense_scan_mma2_kernel (tcgen05 cta_group::2 pair, 128 queries per pass)" if qpl > 64 else
-                "dense_scan_mma_kernel (tcgen05, <= 64 queries per pass)" if self.B >= 16 else "dense_scan_kernel (FFMA2)")
-        out = {"bound": "hbm", "kernel": kern, "achieved": ach, "peak": hbm, "unit": "GB/s", "frac": ach / hbm,
+        kern = "dense_scan_mma_kernel (wgmma, <= 64 queries per pass)" if self.B >= 16 else "dense_scan_kernel (FFMA)"
+        out = {"bound": "hbm", "kernel": kern, "achieved": ach, "peak": hbm, "unit": "GB/s", "frac": _frac(ach, hbm),
                "traffic": None, "traffic_source": None, "peak_source": src, "algorithmic_bytes_per_launch": alg,
                "avg_launch_ms": avg, "launches_timed": n_scan, "queries_per_launch": qpl,
                "share_of_step": scan_ms / res["ms_total"],
                "other_dense_stages_ms_per_batch": {
                    "sampling_passes+threshold_select": res["prof"]["dense_sample"][1] / max(res["n_batches"], 1),
                    "window_select+fp64_rescore": res["prof"]["dense_merge"][1] / max(res["n_batches"], 1)}}
-        prof = os.path.join(ROOT, "profiles", "r02_dense_scan_ncu.json")
-        if os.path.exists(prof) and self.C == 1:
-            try:
-                out["traffic"] = json.load(open(prof)).get("dram_bytes_per_launch")
-                out["traffic_source"] = "profiles/r02_dense_scan_ncu.json (ncu --set full of the same kernel, static)"
-            except Exception:
-                pass
         return out
 
     def roofline_bm25(self, res):
@@ -508,21 +532,19 @@ class Leg:
         return {"bound": "latency + l1tex", "kernel": "bm25_range_kernel (sample + collect)",
                 "postings_per_s": postings / (bm_ms * 1e-3), "postings_per_query": postings / (self.B * res["n_batches"]),
                 "algorithmic_bytes": postings * 12, "posting_GBps": postings * 12 / (bm_ms * 1e-3) / 1e9,
-                "frac_of_hbm_peak_if_every_posting_came_from_dram": postings * 12 / (bm_ms * 1e-3) / 1e9 / hbm,
+                "frac_of_hbm_peak_if_every_posting_came_from_dram": _frac(postings * 12 / (bm_ms * 1e-3) / 1e9, hbm),
                 "ms_total": bm_ms, "share_of_step": bm_ms / res["ms_total"],
-                "note": "the posting lists shared by a batch are served by L2 (ncu: DRAM traffic << posting bytes); ncu of the "
-                        "collect pass (profiles/r02_run13_bm25_range_ncu.md): issue slots 55 % busy, L1TEX 69 %, a third of "
-                        "the stalls on load latency -- no single limiter, so postings/s is the figure of merit, not GB/s"}
+                "note": "the posting lists shared by a batch are served by L2, so postings/s is the figure of merit, not GB/s"}
 
     def roofline_ce(self, res):
-        _, tpeak, _ = peaks()
+        _, tpeak, psrc = peaks()
         n_ce, ce_ms = res["prof"]["ce"]
         if not n_ce:
             return None
         ce_pairs, ce_rows, ce_sq = res["ce_stats"]
         flops = 6 * (24 * 384 * 384 * ce_rows + 4 * 384 * ce_sq)
         tf = flops / (ce_ms * 1e-3) / 1e12
-        return {"bound": "tensor", "achieved": tf, "peak": tpeak, "unit": "TFLOP/s", "frac": tf / tpeak, "ms_total": ce_ms,
+        return {"bound": "tensor", "achieved": tf, "peak": tpeak, "unit": "TFLOP/s", "frac": _frac(tf, tpeak), "peak_source": psrc, "ms_total": ce_ms,
                 "forward_calls": n_ce, "pairs": ce_pairs, "mean_pair_len": ce_rows / max(ce_pairs, 1),
                 "flops_counted": "L*(24*H^2*sum(len) + 4*H*sum(len^2)), padding excluded",
                 "share_of_step": ce_ms / res["ms_total"]}
@@ -601,6 +623,35 @@ def latency_b1(pipe, wl: Workload, idx, n_queries=200, top_k=100):
 _RESULT_OUT = sys.stdout
 
 
+# names of the arrays each device entry point returns, in order
+OUTPUT_NAMES = {"dense": ("ids", "scores", "counts"), "bm25": ("ids", "scores", "counts"),
+                "hybrid": ("ids", "scores", "sources", "counts"), "rerank": ("ids", "scores", "counts")}
+
+
+DUMP_LIMIT_BYTES = 64_000_000   # all files together, .npy headers included
+
+
+def dump_outputs(out_dir, kind, arrays, rank):
+    """DIR/<kind>_<name>.npy in float64 (ids and counts are far below 2**53, so they stay exact) for each array the timed
+    path returned for the LAST batch of its last step; with several ranks every rank writes its own rows under
+    rank<r>_<name>.  Above 64 MB in all, a fixed seeded sample of query rows is kept (the same rows of every array) and
+    their indices are written to DIR/<kind>_rows.npy."""
+    os.makedirs(out_dir, exist_ok=True)
+    names = OUTPUT_NAMES[kind]
+    if len(arrays) != len(names):
+        names = tuple(f"out{i}" for i in range(len(arrays)))
+    prefix = f"rank{rank}_" if int(os.environ.get("WORLD_SIZE", "1")) > 1 else ""
+    arrays = [np.asarray(a, dtype=np.float64) for a in arrays]
+    rows = arrays[0].shape[0] if arrays else 0
+    per_row = sum(a.nbytes for a in arrays) / max(rows, 1)
+    if rows and per_row * rows > DUMP_LIMIT_BYTES:
+        keep = np.sort(np.random.default_rng(0).choice(rows, int((DUMP_LIMIT_BYTES - 8 * rows - 4096) // per_row), replace=False))
+        arrays = [a[keep] for a in arrays]
+        np.save(os.path.join(out_dir, f"{prefix}{kind}_rows.npy"), keep.astype(np.float64))
+    for name, a in zip(names, arrays):
+        np.save(os.path.join(out_dir, f"{prefix}{kind}_{name}.npy"), a)
+
+
 def _emit(line):
     """The ONE JSON line of the contract, on the process's original stdout."""
     _RESULT_OUT.write(json.dumps(line) + "\n")
@@ -639,7 +690,7 @@ def main():
                                "corpus replicated, no collective")
                             + ("; queries split across groups" if n_groups > 1 else "")
                             + (f" [--corpus-shards {C}]" if args.corpus_shards else f" [--shard {args.shard}]")),
-              "l2_policy": "corpus (2.05 GB) is larger than L2 (126 MB); no flush needed",
+              "l2_policy": "corpus (2.05 GB) is larger than L2 (50 MB on the H100); no flush needed",
               "query_set": "1024 seeded unit vectors, cycled"}
 
     if args.impl == "reference":
@@ -737,6 +788,8 @@ def main():
     rr = need_rerank(pipe, C, lo, hi) if kind == "rerank" else None
     leg = Leg(kind, pipe, wl, args, world, rank, local_rank, C, my_group, lo, hi, idx, rr)
     res = leg.run(args.steps, args.warmup)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, kind, leg.last_outputs, rank)
     roofline = leg.roofline_dense(res) if kind != "bm25" else {}
     if kind in ("hybrid", "rerank", "bm25"):
         roofline["bm25"] = leg.roofline_bm25(res)

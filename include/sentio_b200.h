@@ -1,5 +1,5 @@
 /*
- * sentio_b200.h -- C ABI of libsentio_b200.so: the B200-native retrieve -> fuse -> rerank hot path.
+ * sentio_b200.h -- C ABI of libsentio_b200.so: the H100-native retrieve -> fuse -> rerank hot path.
  *
  * The reference (chernistry/sentio @ 68a63b1b) has no FFI: its "plugin API" is Python duck typing
  * (`retriever.retrieve(query, top_k)` src/core/graph/nodes.py:70, `reranker.rerank(query=, docs=, top_k=)`
@@ -96,8 +96,8 @@ int sb_profile_read(sb_ctx* ctx, int kernel_id, int64_t* n_out, double* ms_out);
 #define SB_MAX_DENSE_SLOTS 2
 int sb_dense_load(sb_ctx* ctx, int slot, const void* vecs, int64_t n, int32_t d, int32_t dtype, int64_t id_base);
 /*
- * Scan selection: 0 = auto (batches of >= 16 queries use the tcgen05 batched-query scan, smaller ones the CUDA-core
- * scan), 1 = CUDA-core scan only, 2 = tcgen05 scan whenever eligible.  Results are identical in every mode.
+ * Scan selection: 0 = auto (batches of >= 16 queries use the wgmma batched-query scan, smaller ones the CUDA-core
+ * scan), 1 = CUDA-core scan only, 2 = wgmma scan whenever eligible.  Results are identical in every mode.
  */
 int sb_dense_set_mode(sb_ctx* ctx, int mode);
 int64_t sb_dense_count(sb_ctx* ctx, int slot);
@@ -295,7 +295,7 @@ int sb_rerank_dev(sb_ctx* ctx, const int32_t* q_tok_dev, const int32_t* q_len_de
                   int32_t k_out, int64_t* out_ids_dev, float* out_scores_dev, int32_t* out_counts_dev, void* stream);
 
 /*
- * Test hook for the tcgen05 GEMM inside K5: out[M,N] = epilogue(A[M,K] * W[N,K]^T + bias (+ residual)), operands given as
+ * Test hook for the wgmma GEMM inside K5: out[M,N] = epilogue(A[M,K] * W[N,K]^T + bias (+ residual)), operands given as
  * host fp32 and rounded to fp16 on the device; epi 0 = bias (fp16 result), 1 = bias + erf-GELU (fp16 result),
  * 2 = bias + residual (fp32 result).  N % 128 == 0, K % 64 == 0.
  */

@@ -1,4 +1,4 @@
-"""sentio_b200 -- B200-native retrieve -> fuse -> rerank hot path behind chernistry/sentio's plugin surface.
+"""sentio_b200 -- H100-native retrieve -> fuse -> rerank hot path behind chernistry/sentio's plugin surface.
 
 Public surface (names match the reference's ``src/core/retrievers`` / ``src/core/rerankers`` modules):
 
@@ -12,8 +12,8 @@ Public surface (names match the reference's ``src/core/retrievers`` / ``src/core
     from sentio_b200.selector import create_document_selector_node # the node that follows the reranker
     from sentio_b200.pipeline import HybridPipeline, plan_layout   # batched / sharded arrays-in arrays-out path
 
-All arithmetic runs in libsentio_b200.so (hand-written sm_100a CUDA, C ABI in include/sentio_b200.h).  Importing this
-package does not touch the GPU; creating an engine without the built library or without a B200 raises.
+All arithmetic runs in libsentio_b200.so (hand-written sm_90a CUDA, C ABI in include/sentio_b200.h).  Importing this
+package does not touch the GPU; creating an engine without the built library or without an H100 raises.
 """
 from .document import Document
 

@@ -1,6 +1,6 @@
 """ctypes binding of libsentio_b200.so (C ABI declared in include/sentio_b200.h).
 
-There is deliberately NO fallback: if the shared library is missing or no B200 is visible, importing the engine
+There is deliberately NO fallback: if the shared library is missing or no H100 is visible, importing the engine
 raises.  The product never imports oracle/.
 """
 from __future__ import annotations
@@ -10,7 +10,7 @@ import os
 from pathlib import Path
 
 _PKG = Path(__file__).resolve().parent
-# SENTIO_B200_LIB: load another build of the same sources (A/B measurements of kernel variants: scripts/r02_gpu11.sh)
+# SENTIO_B200_LIB: load another build of the same sources (A/B measurements of kernel variants, python -m sentio_b200.build --variant)
 LIB_PATH = Path(os.environ.get("SENTIO_B200_LIB") or _PKG / "libsentio_b200.so")
 
 c_i64p = C.POINTER(C.c_int64)
@@ -120,7 +120,7 @@ def load_library(path: os.PathLike | None = None) -> C.CDLL:
     p = Path(path) if path else LIB_PATH
     if not p.exists():
         raise SentioB200Error(
-            f"{p} not found: build it with `python -m sentio_b200.build` (nvcc, sm_100a). "
+            f"{p} not found: build it with `python -m sentio_b200.build` (nvcc, sm_90a). "
             "sentio_b200 has no CPU fallback.")
     lib = C.CDLL(str(p))
     for name, (restype, argtypes) in SIGNATURES.items():

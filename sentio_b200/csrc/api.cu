@@ -37,17 +37,15 @@ int sb_create(int device, sb_ctx** out) {
   DeviceGuard g(device);
   cudaDeviceProp prop;
   SB_CUDA(cudaGetDeviceProperties(&prop, device));
-  SB_REQUIRE(prop.major == 10, SB_ERR_UNSUPPORTED,
-             "sb_create: device %d is sm_%d%d; this library is built for sm_100a (B200) only", device, prop.major,
+  SB_REQUIRE(prop.major == 9 && prop.minor == 0, SB_ERR_UNSUPPORTED,
+             "sb_create: device %d is sm_%d%d; this library is built for sm_90a (H100) only", device, prop.major,
              prop.minor);
   sb_ctx* ctx = new sb_ctx();
   ctx->device = device;
   ctx->num_sms = prop.multiProcessorCount;
   ctx->smem_optin = prop.sharedMemPerBlockOptin;
   // tuning knobs for experiments (bench / profiling); the defaults are the measured best
-  if (const char* v = getenv("SB_DENSE_PAIR")) ctx->dense_pair = atoi(v) != 0;
   if (const char* v = getenv("SB_DENSE_SAMPLE")) ctx->dense_sample_per_cta = atoi(v) > 0 ? atoi(v) : 2;
-  if (const char* v = getenv("SB_DENSE_MULTISAMPLE")) ctx->dense_multisample = atoi(v) != 0;
   if (const char* v = getenv("SB_DENSE_PREFETCH")) ctx->dense_prefetch = atoi(v) > 0 ? atoi(v) : 0;
   if (const char* v = getenv("SB_DENSE_STAGES")) ctx->dense_max_stages = atoi(v) >= 3 ? atoi(v) : 8;
   cudaError_t se = cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking);

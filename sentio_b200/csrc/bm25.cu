@@ -78,8 +78,7 @@ __global__ void bm25_dense_fill_kernel(const int64_t* __restrict__ indptr, const
 //    no cursor, no compare, no vote (8 instead of ~37 instructions per 32 postings).  Adding idf * 0.0 = +-0.0 to a doc
 //    without a posting leaves its accumulator bit-for-bit unchanged, exactly like rank_bm25's dense `score +=` does;
 //  * the posting-list walk addresses its shared-memory accumulators through 32-bit shared-space addresses and is
-//    branch-free (a posting beyond the sub-range reads a never-written per-warp dummy slot): the first version spent
-//    150 instructions per 128 postings on generic-address arithmetic and divergence bookkeeping (profiles/r02_run4_bm25*);
+//    branch-free (a posting beyond the sub-range reads a never-written per-warp dummy slot);
 //  * a finished sub-range is consumed by its warp according to MODE:
 //      kModeSample : (S ranges spread over the corpus, one per CTA) ceil(k/S)-th best positive score of the range, min
 //                    over the S ranges -> thr[q], a lower bound of the global k-th best score

@@ -1,4 +1,4 @@
-// ce_gemm.cuh -- interface of the tcgen05 GEMM used by the cross-encoder (ce_gemm.cu).
+// ce_gemm.cuh -- interface of the wgmma GEMM used by the cross-encoder (ce_gemm.cu).
 #pragma once
 #include <cuda.h>
 

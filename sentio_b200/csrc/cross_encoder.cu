@@ -1,10 +1,10 @@
 // cross_encoder.cu -- K5: BERT-style sequence classifier forward (MiniLM-L6 shape by default) for the reranker.
 //
 // Replaces the remote Jina rerank call behind JinaReranker.rerank (reference src/core/rerankers/jina_reranker.py:139-144).
-// Per layer:  QKV GEMM (tcgen05, bias)  ->  masked softmax attention  ->  out-proj GEMM (+bias +residual, fp32)
+// Per layer:  QKV GEMM (wgmma, bias)  ->  masked softmax attention  ->  out-proj GEMM (+bias +residual, fp32)
 //             -> LayerNorm -> FFN-up GEMM (+bias, erf-GELU) -> FFN-down GEMM (+bias +residual, fp32) -> LayerNorm.
 // The residual stream stays fp32 in HBM; every GEMM operand is an fp16 copy written by the producing kernel; all GEMM
-// accumulation is fp32 in tensor memory (ce_gemm.cu).
+// accumulation is fp32 in registers (wgmma, ce_gemm.cu).
 //
 // PACKED TOKENS: positions beyond a pair's length are padding -- never read as keys (masked) and never consumed, which is
 // what the additive -inf mask of the HuggingFace oracle yields for the [CLS] logit -- so they are not computed at all: the
@@ -361,9 +361,7 @@ __global__ void __launch_bounds__(128, S_MAX > 128 ? 2 : 4) ce_attention_mma_ker
   const int ld = 3 * H;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, t = lane & 3;
   // 16-row query tiles are dealt round-robin (tile j -> warp j & 3): a pair of ~90 tokens has 6 tiles, so every warp
-  // has work (the contiguous 32-rows-per-warp split left warp 3 idle for every pair shorter than 97 tokens).  Rotating
-  // the assignment per CTA to spread the two-tile warps over the SM's four schedulers was measured and changes nothing
-  // (2741 vs 2749 queries/s, profiles/r02_run12_ab_ce_{base,norot}.json).
+  // has work (the contiguous 32-rows-per-warp split left warp 3 idle for every pair shorter than 97 tokens).
   const int vwarp = warp;
   const int stage_rows = min(S_MAX, (len + 31) & ~31);  // 32-key groups beyond len are never touched
   // rows [len, stage_rows) are masked keys: zeros (finite products), written once -- len belongs to the pair, not the head
@@ -933,7 +931,7 @@ __global__ void ce_rank_kernel(const float* __restrict__ sig, const int64_t* __r
 
 extern "C" {
 
-// Test hook: run the tcgen05 GEMM of the cross-encoder on host fp32 operands (rounded to fp16 on the device).
+// Test hook: run the wgmma GEMM of the cross-encoder on host fp32 operands (rounded to fp16 on the device).
 int sb_ce_gemm_test(sb_ctx* ctx, const float* a, const float* w, const float* bias, const float* residual, int32_t M,
                     int32_t N, int32_t K, int32_t epi, float* out) {
   SB_REQUIRE(ctx && a && w && bias && out, SB_ERR_ARG, "sb_ce_gemm_test: NULL argument");

@@ -28,7 +28,7 @@ constexpr int kConsumerWarps = 8;
 constexpr int kConsumerThreads = kConsumerWarps * 32;
 constexpr int kScanThreads = kConsumerThreads + 64;  // + 1 TMA producer warp + 1 compaction warp
 constexpr int kMergeThreads = 512;
-constexpr int kRowPad = 128;  // n_pad granularity (tile rows of the tcgen05 scan; multiple of the CUDA-core tiles)
+constexpr int kRowPad = 128;  // n_pad granularity (tile rows of the wgmma scan; multiple of the CUDA-core tiles)
 
 // ------------------------------------------------------------------------------------------------ load kernels
 // One warp per row.  f32 input: x16 = fp16(x / ||x||) (division in fp64, single rounding); f16 input: verbatim.
@@ -205,12 +205,13 @@ __device__ __forceinline__ int compact_dispatch(int T, unsigned long long* best,
   return compact_into_best_smem(best, nbest, batch, nbatch, kprime, T, scratch, lane);
 }
 
-// two fp32 FMAs per instruction (SASS FFMA2): the 3-register FFMA issues at half rate on sm_100, FFMA2 restores
-// the full 128 FMA/clk/SM; operands are (lo, hi) float pairs packed in 64-bit registers.
+// a (lo, hi) pair of fp32 FMAs on floats packed in 64-bit registers: two FFMA on sm_90 (full rate there), each lane
+// rounded exactly as one fma.rn
 __device__ __forceinline__ unsigned long long ffma2(unsigned long long a, unsigned long long b, unsigned long long c) {
-  unsigned long long d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
+  const float lo = fmaf(__uint_as_float((uint32_t)a), __uint_as_float((uint32_t)b), __uint_as_float((uint32_t)c));
+  const float hi = fmaf(__uint_as_float((uint32_t)(a >> 32)), __uint_as_float((uint32_t)(b >> 32)),
+                        __uint_as_float((uint32_t)(c >> 32)));
+  return ((unsigned long long)__float_as_uint(hi) << 32) | (unsigned long long)__float_as_uint(lo);
 }
 __device__ __forceinline__ unsigned long long pack_f2(float lo, float hi) {
   return ((unsigned long long)__float_as_uint(hi) << 32) | (unsigned long long)__float_as_uint(lo);
@@ -558,7 +559,7 @@ __global__ void __launch_bounds__(kMergeThreads, 1) dense_merge_kernel(const Mer
 
 // ------------------------------------------------------------------------------------------------ query preparation
 // One CTA per operand row r (rows >= nq are padding): qn[r] = q[r] / ||q[r]|| in fp32 (the scans rank by cosine, so the
-// caller's scale must not reach the fp32 / fp16 arithmetic), optionally q16[r] = fp16(qn[r]) for the tcgen05 scan, and
+// caller's scale must not reach the fp32 / fp16 arithmetic), optionally q16[r] = fp16(qn[r]) for the wgmma scan, and
 // eps[r] = the bound on |approximate - exact cosine| the hand-off window uses (0 for an all-zero query).
 __global__ void __launch_bounds__(256) dense_prep_queries_kernel(const float* __restrict__ q_pad, int nq, int d_pad,
                                                                  float* __restrict__ qn, __half* __restrict__ q16,

@@ -1,4 +1,4 @@
-// dense_common.cuh -- pieces shared by the CUDA-core scan (dense.cu) and the tcgen05 batched scan (dense_mma.cu).
+// dense_common.cuh -- pieces shared by the CUDA-core scan (dense.cu) and the wgmma batched scan (dense_mma.cu).
 #pragma once
 #include "common.cuh"
 
@@ -15,7 +15,7 @@ struct RescoreArgs {
 };
 
 // ---- approximate -> exact hand-off (DESIGN.md "K1: exactness") --------------------------------------------------------
-// Both scans rank rows by an APPROXIMATE cosine a(x) (fp32 accumulation; the tcgen05 scan additionally rounds the
+// Both scans rank rows by an APPROXIMATE cosine a(x) (fp32 accumulation; the wgmma scan additionally rounds the
 // normalised query to fp16).  With |a(x) - cos(x)| <= eps for every row, the exact top-k is contained in
 //     W = { x : a(x) >= a_k - 2*eps },   a_k = the k-th largest approximate score
 // (the k best approximate rows have cos >= a_k - eps, so the k-th best exact cosine is >= a_k - eps, and a row with
@@ -27,7 +27,7 @@ struct RescoreArgs {
 // eps of the CUDA-core scan: fp32 FMA chains over d_pad products of |x||q| <= 1 (normalised operands): gamma_d <= d*2^-24;
 // doubled, plus 2^-19 for the fp32 normalisation of the query, the fp32 inverse row norm and the final product.
 __host__ __device__ __forceinline__ float dense_eps_fp32(int d_pad) { return (float)d_pad * 1.1920929e-7f + 1.9073486e-6f; }
-// accumulation part of the tcgen05 scan's eps: the tensor core's fp32 accumulator may truncate (<= 2 ulp per step)
+// accumulation part of the wgmma scan's eps: the tensor core's fp32 accumulator may truncate (<= 2 ulp per step)
 __host__ __device__ __forceinline__ float dense_eps_mma_acc(int d_pad) { return (float)d_pad * 2.3841858e-7f + 1.9073486e-6f; }
 
 // lower edge of the window as a composite key (keys >= it are members)

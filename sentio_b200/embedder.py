@@ -6,7 +6,7 @@ The step immediately before the dense search in ``DenseRetriever.retrieve`` is `
 (src/core/embeddings/base.py:146-420: ``embed_sync`` / ``embed_many_sync`` / ``embed_async_single`` /
 ``embed_async_many`` / ``dimension`` / ``stats`` / ``warm_up`` / ``close``, LFU-free dict cache) and computes the
 embedding locally: hashed word pieces ``[CLS] tokens [SEP]`` -> BERT-style encoder (the cross-encoder's kernels:
-tcgen05 GEMMs, packed tokens, [CLS]-only last layer) -> optional linear projection to ``dimension`` -> L2 normalise.
+wgmma GEMMs, packed tokens, [CLS]-only last layer) -> optional linear projection to ``dimension`` -> L2 normalise.
 
 There is no checkpoint offline, so the weights are random-init (MiniLM-L6 shape + a 384 -> 1024 projection by default,
 matching the 1024-d vectors of BASELINE.json); parity is against the HuggingFace ``BertModel`` forward of the same

@@ -1,4 +1,4 @@
-"""Reranker interfaces of the B200 path.
+"""Reranker interfaces of the GPU path.
 
 ``create_reranker_node`` (reference src/core/graph/nodes.py:124-127,179-183) calls ``reranker.rerank(query=, docs=,
 top_k=)`` and nothing else; ``rerank_async`` and the ``RerankingResult`` container complete the surface of the reference's

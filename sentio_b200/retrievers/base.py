@@ -1,4 +1,4 @@
-"""Retriever / scorer interfaces of the B200 path.
+"""Retriever / scorer interfaces of the GPU path.
 
 The LangGraph nodes of the reference only need two things from a retriever (src/core/graph/nodes.py:37-40,70):
 ``retrieve(query, top_k=...)`` returning documents best first, and -- for the async graph -- ``retrieve_async``.  Both are

@@ -201,7 +201,7 @@ class PyseriniBM25Retriever(BaseRetriever):
         if documents is None:
             if not os.path.isdir(self.index_dir):
                 raise RuntimeError(f"Pyserini index directory not found: {self.index_dir}")
-            raise RuntimeError("Pyserini is not installed - Lucene indexes cannot be read by the B200 path; pass "
+            raise RuntimeError("Pyserini is not installed - Lucene indexes cannot be read by the GPU path; pass "
                                "documents=... to score them with Pyserini's parameters on the GPU")
         self._inner = BM25Retriever(documents=documents, variant="okapi", device=device, k1=k1, b=b)
 

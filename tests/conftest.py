@@ -17,7 +17,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (run by the driver with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90a); skipped when no CUDA device is visible")
 
 
 def _cuda_device_visible() -> bool:
@@ -33,7 +33,7 @@ def pytest_collection_modifyitems(config, items):
     """Without a CUDA device the `gpu` tests are skipped (not errors), so a plain `pytest` run is green on a CPU box."""
     if _cuda_device_visible():
         return
-    skip = pytest.mark.skip(reason="needs a B200: no CUDA device visible")
+    skip = pytest.mark.skip(reason="needs an H100: no CUDA device visible")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)
@@ -53,7 +53,7 @@ def built_lib():
 
 @pytest.fixture(scope="session")
 def engine(built_lib):
-    """A real B200Engine; only requested by @pytest.mark.gpu tests."""
+    """A real engine on cuda:0; only requested by @pytest.mark.gpu tests."""
     from sentio_b200.engine import B200Engine
 
     eng = B200Engine(0)

@@ -373,12 +373,43 @@ def selector_cases(ns):
     return cases
 
 
+def reference_nodes_cases(ns):
+    """The reference's OWN LangGraph retriever / reranker node functions (src/core/graph/nodes.py), unmodified, driving
+    this repository's HybridRetriever / B200Reranker on the oracle-backed engine double (host logic)."""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    from test_reference_nodes import QUERIES, build_host_stack
+
+    hr, rr = build_host_stack()
+    retrieve_node = ns.create_retriever_node(hr, top_k=10)
+    rerank_node = ns.create_reranker_node(rr, top_k=4)
+    cases = []
+    for q in QUERIES:
+        state = retrieve_node(ns.create_initial_state(q))
+        got = state["retrieved_documents"]
+        assert all(type(d) is ns.Document for d in got) and "retriever_error" not in state["metadata"]
+        st5 = ns.create_initial_state(q)
+        st5["metadata"]["user_top_k"] = 5
+        top5 = [d.id for d in retrieve_node(st5)["retrieved_documents"]]
+        case = dict(query=q, retrieved=[[d.id, d.text, d.metadata["score"], d.metadata["hybrid_score"]] for d in got],
+                    retriever_type=state["metadata"]["retriever_type"], retrieved_count=state["metadata"]["retrieved_count"],
+                    top5=top5)
+        state = rerank_node(state)
+        case["reranked"] = [[d.id, d.metadata["rerank_score"], d.metadata["score"]] for d in state["reranked_documents"]]
+        case["reranker_type"] = state["metadata"].get("reranker_type")
+        cases.append(case)
+    return cases
+
+
 def main():
     ns = refload.load()
+    only = sys.argv[1:]   # fixture names to regenerate (default: all)
     fixtures = dict(fusion=fusion_cases(ns), bm25=bm25_cases(ns), scorers=scorer_cases(ns),
                     hybrid_e2e=hybrid_e2e_cases(ns), hybrid_cache=hybrid_cache_cases(ns),
-                    rerank_flow=rerank_flow_cases(ns), selector=selector_cases(ns))
+                    rerank_flow=rerank_flow_cases(ns), selector=selector_cases(ns),
+                    reference_nodes=reference_nodes_cases(ns))
     for name, data in fixtures.items():
+        if only and name not in only:
+            continue
         path = os.path.join(HERE, f"{name}.json")
         with open(path, "w") as f:
             json.dump(data, f)

@@ -1,4 +1,4 @@
-"""The C-ABI library builds for sm_100a, loads without a GPU and exports every symbol include/sentio_b200.h declares."""
+"""The C-ABI library builds for sm_90a, loads without a GPU and exports every symbol include/sentio_b200.h declares."""
 import ctypes
 import os
 import re

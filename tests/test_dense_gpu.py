@@ -34,7 +34,7 @@ def test_dense_topk_matches_oracle_f16_corpus(engine, n, d, k, B):
 @pytest.mark.parametrize("n,d,k,B", [(9000, 1024, 10, 16), (20000, 256, 100, 40), (30000, 768, 100, 70),
                                      (200000, 128, 228, 33), (12000, 64, 5, 130), (40000, 1024, 100, 260)])
 def test_dense_batched_tcgen05_path_matches_oracle(engine, n, d, k, B):
-    """B >= 16 queries take the tcgen05 batched-query scan (dense_mma.cu); results must equal the oracle AND be
+    """B >= 16 queries take the wgmma batched-query scan (dense_mma.cu); results must equal the oracle AND be
     bit-identical to the CUDA-core scan."""
     rng = np.random.default_rng(n + d + B)
     x = rng.standard_normal((n, d)).astype(np.float32)
@@ -54,7 +54,7 @@ def test_dense_batched_tcgen05_path_matches_oracle(engine, n, d, k, B):
 
 def _near_tie_corpus(rng, n, d, cluster, ulps=1):
     """Random unit corpus whose rows [200, 200+cluster) are 1-ulp (fp16) perturbations of one base row: their cosines
-    with any query differ by ~1e-6 .. 1e-5, far below the fp16-query rounding error of the tcgen05 scan."""
+    with any query differ by ~1e-6 .. 1e-5, far below the fp16-query rounding error of the wgmma scan."""
     x = rng.standard_normal((n, d)).astype(np.float32)
     x /= np.linalg.norm(x, axis=1, keepdims=True)
     x16 = x.astype(np.float16)
@@ -102,7 +102,7 @@ def test_dense_window_larger_than_the_winner_buffer_uses_the_exact_fallback(engi
 
 def test_dense_query_scale_does_not_change_the_result(engine):
     """ADVICE r01: cosine is scale invariant -- queries scaled by 1e6 / 1e-6 / 1e-30 / 1e30 must give the same ids on
-    the CUDA-core scan (B = 1) and on the tcgen05 scan (B = 64), whose fp16 operand would otherwise overflow / vanish."""
+    the CUDA-core scan (B = 1) and on the wgmma scan (B = 64), whose fp16 operand would otherwise overflow / vanish."""
     rng = np.random.default_rng(12)
     x = rng.standard_normal((20000, 256)).astype(np.float32)
     x /= np.linalg.norm(x, axis=1, keepdims=True)
@@ -201,7 +201,7 @@ def test_dense_full_size_1m_x_1024(engine):
     for b in range(2):
         wi, ws = dense_oracle.dense_topk(x16, q[b], k)
         assert_topk_matches(ids[b], sc[b], cnt[b], wi, ws, what=f"1M b={b}")
-    # (e) the bench configuration: a 256-query batch (two 128-query groups on the cta_group::2 pair kernel), compared
+    # (e) the bench configuration: a 256-query batch (four 64-query groups on the wgmma scan), compared
     #     with the oracle on 8 sampled queries and bit for bit with the CUDA-core scan on the first 64
     q256 = np.concatenate([synth.query_vectors(253, d, seed=99), x16[probe].astype(np.float32)])
     engine.dense_set_mode(0)

@@ -261,9 +261,13 @@ def test_library_path_override(monkeypatch, tmp_path):
 
     default = lib.LIB_PATH
     assert default.name == "libsentio_b200.so" and default.parent.name == "sentio_b200"
+    # reloading creates new ctypes classes (SbCeConfig) and drops the loaded library; engine.py keeps the old ones, so the
+    # module's original state is put back afterwards for the tests that run later in the same session
+    saved = dict(vars(lib))
     monkeypatch.setenv("SENTIO_B200_LIB", str(tmp_path / "libsentio_b200_x.so"))
     try:
         assert importlib.reload(lib).LIB_PATH == tmp_path / "libsentio_b200_x.so"
     finally:
         monkeypatch.delenv("SENTIO_B200_LIB")
         assert importlib.reload(lib).LIB_PATH == default
+        vars(lib).update(saved)

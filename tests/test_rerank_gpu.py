@@ -1,4 +1,4 @@
-"""K5 parity: tcgen05 GEMM unit test, cross-encoder forward vs the NumPy / HuggingFace oracles (rel 1e-3, abs floor 1e-4),
+"""K5 parity: wgmma GEMM unit test, cross-encoder forward vs the NumPy / HuggingFace oracles (rel 1e-3, abs floor 1e-4),
 and the reranker's control flow vs the reference JinaReranker (golden rerank_flow.json)."""
 import math
 
