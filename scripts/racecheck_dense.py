@@ -1,6 +1,7 @@
 #!/usr/bin/env python
-"""Small dense workload for `compute-sanitizer` (memcheck / racecheck): the wgmma scan (one and several 64-query groups),
-the CUDA-core scan, the window select + exact re-score and the brute-force fallback, checked against the oracle."""
+"""Small dense workload for `compute-sanitizer` (memcheck / racecheck): the wgmma scan (one group, a 256-query group plus
+a small one, two 256-query groups), the CUDA-core scan, the window select + exact re-score and the brute-force fallback,
+checked against the oracle."""
 import os
 import sys
 
@@ -21,7 +22,7 @@ def main():
     x16 = x.astype(np.float16)
     x16[3000:5600] = x16[11]                     # 2600 exact duplicates: window > winner buffer -> brute-force fallback
     eng.load_dense(x16)
-    for B in (3, 40, 130, 300):                       # CUDA-core scan / one wgmma group / several groups + a small one
+    for B in (3, 40, 130, 256, 300, 512):             # CUDA-core scan / one wgmma group / a full group (+ a small one) / two
         q = rng.standard_normal((B, d)).astype(np.float32)
         q[1] = x16[11].astype(np.float32)
         q[2] = 0.0

@@ -1,13 +1,16 @@
 // dense_mma.cu -- K1b: batched-query dense scan on the Hopper tensor cores (wgmma / TMA), sm_90a.
 //
-// One HBM pass over the fp16 corpus serves a whole GROUP of queries: the scores of a 128-row corpus tile against all
-// queries of the group are one accumulator  D[128, N] = A[128, D] * Q[N, D]^T  (A = corpus tile, K-major fp16, streamed
-// by TMA in 64-column SWIZZLE_128B boxes; B = the normalised fp16 query block, K-major, resident in shared memory for the
-// whole kernel; D in the registers of two consumer warpgroups, 64 corpus rows each).
-//   * dense_scan_mma_kernel<QBN>   one CTA per SM, N = QBN = 16 / 32 / 64 queries (m64nQBNk16).
-// 64 queries is the largest block whose resident operand (128 KB at d = 1024) leaves a useful TMA ring inside the 227 KB
-// of shared memory a block may use on the H100; larger batches take one pass per 64 queries.
-// The pass stays HBM bound: per 16 KB of corpus the tensor pipe needs 8 MMAs of 64 x QBN x 16.
+// One HBM pass over the fp16 corpus serves a whole GROUP of up to 256 queries: the scores of a 128-row corpus tile
+// against all queries of the group are one accumulator  D[128, N] = A[128, D] * Q[N, D]^T  (A = corpus tile, B = the
+// normalised fp16 query block, both K-major fp16 streamed by TMA in 64-column SWIZZLE_128B boxes; D in the registers of
+// two consumer warpgroups, 64 corpus rows each).
+//   * dense_scan_mma_kernel<QBN>   N = QBN = 16 / 32 / 64 / 128 / 256 queries (m64nQBNk16).
+// A ring stage holds one corpus box (16 KB) and the matching box of the query block (QBN x 128 B), so shared memory does
+// not grow with d: at QBN = 256 four 48 KB stages fit the 227 KB a block may use.
+// At QBN = 256 a 16 KB corpus box feeds 8 MMAs of 64 x 256 x 16: the pass is bound by the tensor pipe, not by HBM.
+//
+// Every CTA loads the query boxes itself (512 KB per tile from L2 at d = 1024): sharing them across a 2-CTA cluster by
+// TMA multicast was measured slower on the H100 (DESIGN.md K1b).
 //
 // Exactness (dense_common.cuh, DESIGN.md "K1: exactness"):
 //   * queries are L2-normalised before the fp16 rounding (cosine is scale invariant; the caller's scale never reaches
@@ -40,16 +43,19 @@ constexpr int kBK = 64;                       // fp16 elements per 128-byte swiz
 constexpr uint32_t kATileBytes = kTileRows * kBK * 2;   // 16 KB
 constexpr int kConsumerWarps = 8;
 constexpr int kMmaThreads = 32 * kConsumerWarps + 32;
+constexpr int kQbnMax = 256;                  // queries per group (m64n256k16)
 constexpr int kSampleRows = 16;               // corpus rows behind one sampling-pass key (one warp's accumulator rows)
 constexpr int kSampleKeys = kTileRows / kSampleRows;   // sampling-pass keys per (tile, query)
 constexpr int kSelectThreads = 512;
 constexpr int kSelStage = 8192;               // survivors staged in shared memory by dense_select_kernel (64 KB)
 constexpr int kSelTop = 2048;                 // window (winner) buffer; larger windows go to the exact fallback
 
-__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, int c0, int c1, uint32_t bar) {
+__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, int c0, int c1, uint32_t bar,
+                                            uint64_t policy) {
   asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(dst),
-      "l"(map), "r"(c0), "r"(c1), "r"(bar)
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%2, %3}], "
+      "[%4], %5;" ::"r"(dst),
+      "l"(map), "r"(c0), "r"(c1), "r"(bar), "l"(policy)
       : "memory");
 }
 // L2 prefetch of a tensor-map box (no shared-memory destination): keeps more HBM requests in flight than the ring holds
@@ -80,25 +86,23 @@ dense_scan_mma_kernel(const __grid_constant__ CUtensorMap tm_rows, const __grid_
   const uint32_t raw = smem_u32(msm_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;  // SWIZZLE_128B operands need 1024-byte alignment
   uint8_t* sm = msm_raw + (base - raw);
-  constexpr uint32_t kQBlockBytes = QBN * kBK * 2;      // one 64-column block of the query operand
-  const uint32_t q_bytes = (uint32_t)p.kb_count * kQBlockBytes;
-  const uint32_t a0 = base + q_bytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sm + q_bytes + (size_t)p.stages * kATileBytes);
+  constexpr uint32_t kQBoxBytes = QBN * kBK * 2;              // one 64-column box of the query block
+  constexpr uint32_t kStageBytes = kATileBytes + kQBoxBytes;  // corpus box, then query box
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sm + (size_t)p.stages * kStageBytes);
   const uint32_t bar_full = smem_u32(bars), bar_empty = smem_u32(bars + p.stages);
-  const uint32_t bar_q = smem_u32(bars + 2 * p.stages);
-  volatile float* thr = reinterpret_cast<volatile float*>(bars + 2 * p.stages + 2);   // [QBN]
-  int* cnt = reinterpret_cast<int*>(const_cast<float*>(thr) + QBN);                  // [QBN]
+  volatile float* thr = reinterpret_cast<volatile float*>(bars + 2 * p.stages);   // [QBN]
+  int* cnt = reinterpret_cast<int*>(const_cast<float*>(thr) + QBN);              // [QBN]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int grid = gridDim.x, cta = blockIdx.x;
   const int my_tiles = cta < p.num_tiles ? (p.num_tiles - 1 - cta) / grid + 1 : 0;
+  auto tile_row = [&](int t) { return (p.tile_first + (cta + t * grid) * p.tile_step) * kTileRows; };
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(bar_full + 8 * s, 1);
       mbar_init(bar_empty + 8 * s, kConsumerWarps);   // one arrival per consumer warp
     }
-    mbar_init(bar_q, 1);
     mbar_fence_init();
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_rows) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_q) : "memory");
@@ -112,23 +116,25 @@ dense_scan_mma_kernel(const __grid_constant__ CUtensorMap tm_rows, const __grid_
   if (warp == kConsumerWarps) {
     // ---------------------------------------------------------------- TMA producer
     if (lane == 0) {
-      mbar_expect_tx(bar_q, q_bytes);
-      for (int kb = 0; kb < p.kb_count; ++kb) tma_load_2d(base + (uint32_t)kb * kQBlockBytes, &tm_q, kb * kBK, 0, bar_q);
+      const uint64_t pol_corpus = policy_evict_first();   // 2 GB stream past the query block
+      const uint64_t pol_query = policy_evict_last();     // read again by every tile
       int it = 0;
       const int total_it = my_tiles * p.kb_count;
       for (int t = 0; t < my_tiles; ++t) {
-        const int tile = p.tile_first + (cta + t * grid) * p.tile_step;
+        const int row = tile_row(t);
         for (int kb = 0; kb < p.kb_count; ++kb, ++it) {
           const int s = it % p.stages;
           const uint32_t use = (uint32_t)(it / p.stages);
           const int pf = it + p.stages + p.prefetch;   // a box the ring will only reach later: pull it into L2 now
           if (p.prefetch > 0 && pf < total_it) {
             const int pt = pf / p.kb_count, pkb = pf - pt * p.kb_count;
-            tma_prefetch_l2_2d(&tm_rows, pkb * kBK, (p.tile_first + (cta + pt * grid) * p.tile_step) * kTileRows);
+            tma_prefetch_l2_2d(&tm_rows, pkb * kBK, tile_row(pt));
           }
           if (it >= p.stages) mbar_wait(bar_empty + 8 * s, (use & 1u) ^ 1u);
-          mbar_expect_tx(bar_full + 8 * s, kATileBytes);
-          tma_load_2d(a0 + (uint32_t)s * kATileBytes, &tm_rows, kb * kBK, tile * kTileRows, bar_full + 8 * s);
+          const uint32_t stage = base + (uint32_t)s * kStageBytes;
+          mbar_expect_tx(bar_full + 8 * s, kStageBytes);   // both boxes complete on the stage's one barrier
+          tma_load_2d(stage, &tm_rows, kb * kBK, row, bar_full + 8 * s, pol_corpus);
+          tma_load_2d(stage + kATileBytes, &tm_q, kb * kBK, 0, bar_full + 8 * s, pol_query);
         }
       }
     }
@@ -137,16 +143,15 @@ dense_scan_mma_kernel(const __grid_constant__ CUtensorMap tm_rows, const __grid_
     const int wg = warp >> 2;
     unsigned long long* my_cand = p.cand + (size_t)cta * p.capg;
     const size_t q_stride = (size_t)grid * p.capg;
-    mbar_wait(bar_q, 0);
     int it = 0;
     for (int t = 0; t < my_tiles; ++t) {
-      const int tile = p.tile_first + (cta + t * grid) * p.tile_step;
       float acc[QBN / 2];
       for (int kb = 0; kb < p.kb_count; ++kb, ++it) {
         const int s = it % p.stages;
         mbar_wait(bar_full + 8 * s, (uint32_t)(it / p.stages) & 1u);
-        const uint64_t da = wgmma_desc_sw128(a0 + (uint32_t)s * kATileBytes + (uint32_t)wg * (kATileBytes / 2));
-        const uint64_t db = wgmma_desc_sw128(base + (uint32_t)kb * kQBlockBytes);
+        const uint32_t stage = base + (uint32_t)s * kStageBytes;
+        const uint64_t da = wgmma_desc_sw128(stage + (uint32_t)wg * (kATileBytes / 2));
+        const uint64_t db = wgmma_desc_sw128(stage + kATileBytes);
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < kBK / 16; ++k)
@@ -161,7 +166,7 @@ dense_scan_mma_kernel(const __grid_constant__ CUtensorMap tm_rows, const __grid_
       __syncwarp();
       if (lane == 0) mbar_arrive(bar_empty + 8 * ((it - 1) % p.stages));
       // this thread's accumulator rows: row0 and row0 + 8; columns 8 j + 2 (lane % 4) + {0, 1}
-      const int64_t row0 = (int64_t)tile * kTileRows + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+      const int64_t row0 = (int64_t)tile_row(t) + wg * 64 + (warp & 3) * 16 + (lane >> 2);
       const bool live0 = row0 < p.n, live1 = row0 + 8 < p.n;
       const float invn0 = live0 ? __ldg(p.inv_norm + row0) : 0.f;
       const float invn1 = live1 ? __ldg(p.inv_norm + row0 + 8) : 0.f;
@@ -400,6 +405,16 @@ int encode_map(CUtensorMap* map, const void* ptr, int64_t rows, int64_t cols, in
   return SB_OK;
 }
 
+// ring stages of a QBN-query group: corpus box + query box each, capped by SB_DENSE_STAGES
+int mma_stages(const sb_ctx* ctx, int qbn) {
+  const size_t stage = kATileBytes + (size_t)qbn * kBK * 2 + 16;   // + its full / empty barriers
+  const size_t fixed = 1024 + (size_t)qbn * 8;                     // alignment slack + thresholds and counts
+  return std::min((int)((ctx->smem_optin - fixed) / stage), ctx->dense_max_stages);
+}
+size_t mma_smem(int qbn, int stages) {
+  return 1024 + (size_t)stages * (kATileBytes + (size_t)qbn * kBK * 2 + 16) + (size_t)qbn * 8;
+}
+
 template <int QBN>
 int launch_mma(const CUtensorMap& tm_rows, const CUtensorMap& tm_q, const MmaScanParams& mp, int grid, size_t smem,
                cudaStream_t st) {
@@ -416,6 +431,8 @@ int dispatch_mma(int qbn, const CUtensorMap& tm_rows, const CUtensorMap& tm_q, c
     case 16: return launch_mma<16>(tm_rows, tm_q, mp, grid, smem, st);
     case 32: return launch_mma<32>(tm_rows, tm_q, mp, grid, smem, st);
     case 64: return launch_mma<64>(tm_rows, tm_q, mp, grid, smem, st);
+    case 128: return launch_mma<128>(tm_rows, tm_q, mp, grid, smem, st);
+    case 256: return launch_mma<256>(tm_rows, tm_q, mp, grid, smem, st);
   }
   sb_set_error("dense_mma: unsupported query block %d", qbn);
   return SB_ERR_UNSUPPORTED;
@@ -427,18 +444,14 @@ bool dense_mma_eligible(const sb_ctx* ctx, const DenseIndex& ix, int B) {
   if (B < 16) return false;
   if (ix.d_pad % kBK != 0 || ix.n_pad % kTileRows != 0) return false;
   if (ix.n < 64 * kTileRows) return false;  // tiny corpora: the CUDA-core scan is already launch bound
-  const size_t need = (size_t)ix.d_pad * 16 * 2 + 3 * (size_t)kATileBytes + 4096;
-  return need <= ctx->smem_optin;
+  return mma_stages(ctx, kQbnMax) >= 3;     // shared memory does not depend on d
 }
 
 int dense_mma_topk_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int B, int k, int64_t* out_ids,
                            double* out_scores, int32_t* out_counts, cudaStream_t st) {
   const int kb_count = ix.d_pad / kBK;
   const int total_tiles = (int)(ix.n_pad / kTileRows);
-  // largest single-CTA query block whose resident operand leaves >= 3 pipeline stages
-  int qbn_max = 64;
-  while (qbn_max > 16 && (size_t)qbn_max * ix.d_pad * 2 + 3 * (size_t)kATileBytes + 4096 > ctx->smem_optin) qbn_max >>= 1;
-  const int gsz = qbn_max;                          // operand rows per group
+  const int gsz = kQbnMax;                          // operand rows per group
   const int grid = std::min(ctx->num_sms, total_tiles);
   // sampling pass geometry: a few tiles per CTA spread evenly over the corpus; every warp of a sampled tile reports the
   // best of its 16 rows, so a query gets n_s = kSampleKeys * sample_tiles keys -- aim for n_s >= 4 k
@@ -492,13 +505,12 @@ int dense_mma_topk_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int 
       Group& G = gs[(size_t)g];
       const int left = nq_chunk - g * gsz;
       __half* q16g = q16 + (size_t)(c0 + g * gsz) * ix.d_pad;
-      G.qbn = qbn_max;
+      G.qbn = gsz;
       while (G.qbn > 16 && G.qbn / 2 >= left) G.qbn >>= 1;
       G.nq = std::min(G.qbn, left);
       if ((rc = encode_map(&G.tm_q, q16g, G.qbn, ix.d_pad, G.qbn))) return rc;
-      const size_t q_bytes = (size_t)G.qbn * ix.d_pad * 2;
-      G.stages = std::max(3, std::min((int)((ctx->smem_optin - q_bytes - 3072) / kATileBytes), ctx->dense_max_stages));
-      G.smem = q_bytes + (size_t)G.stages * kATileBytes + 2048 + 1024;
+      G.stages = mma_stages(ctx, G.qbn);
+      G.smem = mma_smem(G.qbn, G.stages);
       rows_total = g * gsz + G.qbn;
     }
     MmaScanParams mp;

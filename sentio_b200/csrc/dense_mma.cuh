@@ -6,7 +6,7 @@
 bool dense_mma_eligible(const sb_ctx* ctx, const DenseIndex& ix, int B);
 
 // q_pad: [B][d_pad] fp32 device (zero padded).  Enqueues sampling passes + full passes + the exact stage for groups of
-// <= 64 queries (one HBM pass over the corpus per group).
+// <= 256 queries (one HBM pass over the corpus per group).
 int dense_mma_topk_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int B, int k, int64_t* out_ids,
                            double* out_scores, int32_t* out_counts, cudaStream_t st);
 

@@ -4,7 +4,7 @@ The LangGraph nodes of the reference only need two things from a retriever (src/
 ``retrieve(query, top_k=...)`` returning documents best first, and -- for the async graph -- ``retrieve_async``.  Both are
 kept with the reference's names and defaults (src/core/retrievers/base.py:13-42) so the classes here drop into
 ``create_retriever_node`` / ``GraphConfig(retriever=...)`` unchanged.  On top of that every GPU-backed retriever can answer
-MANY queries per call (``retrieve_batch``): one HBM pass of the dense scan serves 64 queries, so batching is where the
+MANY queries per call (``retrieve_batch``): one HBM pass of the dense scan serves 256 queries, so batching is where the
 throughput is.
 """
 from __future__ import annotations

@@ -110,7 +110,7 @@ class B200VectorStore:
 
     def search_batch(self, collection_name: str, query_vectors, limit: int = 10, with_payload: bool = True,
                      **_ignored) -> list[list[ScoredPoint]]:
-        """``search`` for many query vectors in ONE device batch (the wgmma scan serves 64 queries per HBM pass)."""
+        """``search`` for many query vectors in ONE device batch (the wgmma scan serves 256 queries per HBM pass)."""
         col = self._collections.get(collection_name)
         if col is None:
             raise ValueError(f"Collection {collection_name} not found")
