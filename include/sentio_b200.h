@@ -74,7 +74,7 @@ int64_t sb_launch_count(sb_ctx* ctx);
  * Optional per-kernel timing for the roofline leg of bench.py: when enabled every launch of the kernels below is
  * bracketed by a CUDA event pair on the launching stream; sb_profile_read drains the finished pairs of one kernel id
  * (0 dense_scan, 1 dense_merge, 2 bm25_score, 3 bm25_select+final, 4 fuse, 5 cross-encoder forward, 6 dense sampling
- * passes + threshold select) and returns the
+ * passes + threshold select, 7 filtered-search match mask, 8 filtered-search gather path) and returns the
  * launch count and the summed device time in milliseconds.
  */
 int sb_profile(sb_ctx* ctx, int enable);
@@ -116,6 +116,38 @@ int sb_dense_topk_dev(sb_ctx* ctx, int slot, const float* q_dev, int32_t B, int3
                       int64_t* out_ids_dev, double* out_scores_dev, int32_t* out_counts_dev, void* stream);
 /* copies stored (fp16 -> fp32) rows of the given ids back to the host: out[n_ids * d]; used by tests/tools */
 int sb_dense_fetch(sb_ctx* ctx, int slot, const int64_t* ids, int32_t n_ids, float* out);
+/*
+ * Filtered dense search -- the `query_filter=` argument of the Qdrant search (reference
+ * src/core/vector_store/qdrant_store.py:120-146, 351-381; filters built by _convert_filter, :456-471): a conjunction of
+ * "payload key == value" conditions.  The host side gives every distinct (key, value) a dictionary code; the library
+ * only compares int32 codes.
+ *
+ * sb_dense_tags_load: the payload index of dense slot `slot` for field `field` (< SB_MAX_TAG_FIELDS): codes[n] holds one
+ * code per row (>= 0), -1 = the row's payload lacks the key.  n must equal sb_dense_count.  sb_dense_load on the slot
+ * drops all of its tag columns.
+ * sb_dense_topk_filtered: as sb_dense_topk, over the rows that satisfy each query's conditions.  Query b's conditions
+ * are entries [f_off[b], f_off[b+1]) of f_field / f_code (CSR, like sb_bm25_topk's q_terms / q_off); a row matches iff
+ * tags[f_field[i]][row] == f_code[i] for every i.  f_code < 0 matches nothing; a query without conditions is
+ * unfiltered.  Every field named must have been loaded.  Results: the EXACT top-k of the matching rows, same order and
+ * scores as sb_dense_topk, out_counts[b] = min(k, matching rows); an all-zero query gives the first k matching rows
+ * with score 0.  A query with at most 2048 matching rows skips the scans (exact fp64 over its matching rows); the others
+ * are scanned with the match mask applied inside the scan (DESIGN.md K1c).
+ * sb_dense_topk_filtered_dev: the same on device buffers (q_dev, f_off_dev[B+1], f_field_dev / f_code_dev[n_conds]).
+ * Unlike the other `_dev` entry points it waits on `stream` twice: once to read the conditions, once to read the
+ * per-query match counts that choose between the scans and the exact gather, and size the scans.
+ * sb_dense_fallback_count: number of queries answered by the brute-force fallback kernel since the context was
+ * created (every dense search, filtered or not); synchronises the device.
+ */
+#define SB_MAX_TAG_FIELDS 16
+int sb_dense_tags_load(sb_ctx* ctx, int slot, int32_t field, const int32_t* codes, int64_t n);
+int sb_dense_topk_filtered(sb_ctx* ctx, int slot, const float* q, int32_t B, int32_t k, const int32_t* f_off,
+                           const int32_t* f_field, const int32_t* f_code, int64_t* out_ids, double* out_scores,
+                           int32_t* out_counts);
+int sb_dense_topk_filtered_dev(sb_ctx* ctx, int slot, const float* q_dev, int32_t B, int32_t k,
+                               const int32_t* f_off_dev, int32_t n_conds, const int32_t* f_field_dev,
+                               const int32_t* f_code_dev, int64_t* out_ids_dev, double* out_scores_dev,
+                               int32_t* out_counts_dev, void* stream);
+int64_t sb_dense_fallback_count(sb_ctx* ctx);
 
 /* ---------------------------------------------------------------- K2: BM25 ---------------------------------- */
 /*

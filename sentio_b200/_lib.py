@@ -48,6 +48,13 @@ SIGNATURES = {
     "sb_dense_topk_dev": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                                     C.c_void_p, C.c_void_p]),
     "sb_dense_fetch": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int32, C.c_void_p]),
+    "sb_dense_tags_load": (C.c_int, [C.c_void_p, C.c_int, C.c_int32, C.c_void_p, C.c_int64]),
+    "sb_dense_topk_filtered": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "sb_dense_topk_filtered_dev": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p,
+                                             C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                             C.c_void_p]),
+    "sb_dense_fallback_count": (C.c_int64, [C.c_void_p]),
     "sb_bm25_load": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p,
                                C.c_int64, C.c_double, C.c_void_p, C.c_int32, C.c_double, C.c_double, C.c_double,
                                C.c_int64]),

@@ -65,6 +65,8 @@ void sb_destroy(sb_ctx* ctx) {
   for (int s = 0; s < SB_MAX_DENSE_SLOTS; ++s) {
     if (ctx->dense[s].rows) cudaFree(ctx->dense[s].rows);
     if (ctx->dense[s].inv_norm) cudaFree(ctx->dense[s].inv_norm);
+    for (int f = 0; f < SB_MAX_TAG_FIELDS; ++f)
+      if (ctx->dense[s].tags[f]) cudaFree(ctx->dense[s].tags[f]);
   }
   Bm25Index& b = ctx->bm25;
   if (b.indptr) cudaFree(b.indptr);
@@ -89,6 +91,9 @@ void sb_destroy(sb_ctx* ctx) {
   ctx->acc_dev.release();
   ctx->qn_dev.release();
   ctx->qaux_dev.release();
+  ctx->fb_count_dev.release();
+  ctx->filt_dev.release();
+  ctx->filt_pin.release();
   ctx->doc_chars_dev.release();
   ctx->pin_in.release();
   ctx->pin_out.release();

@@ -96,6 +96,9 @@ struct DenseIndex {
   // cached CUtensorMap (128 bytes, 64-byte aligned) over rows[] for the wgmma batched scan; valid iff tm_rows_ptr == rows
   alignas(64) unsigned char tm_rows[128] = {0};
   const void* tm_rows_ptr = nullptr;
+  // payload index for filtered search (sb_dense_tags_load): tags[f][row] = dictionary code of field f, -1 = key absent;
+  // nullptr = field f not loaded.  Dropped by sb_dense_load.
+  int32_t* tags[SB_MAX_TAG_FIELDS] = {};
 };
 
 struct Bm25Index {
@@ -145,6 +148,9 @@ struct sb_ctx {
   DevBuf q_dev, cand_dev, out_ids_dev, out_sc_dev, out_cnt_dev, misc_dev, misc2_dev, misc3_dev, acc_dev;
   DevBuf qn_dev;     // dense: normalised fp32 queries [B][d_pad] fed to the scans
   DevBuf qaux_dev;   // dense: per-query eps [B] fp32 | fallback flags [B] i32
+  DevBuf fb_count_dev;   // dense: [1] u64, queries answered by the exact fallback kernel (sb_dense_fallback_count)
+  DevBuf filt_dev;       // filtered dense: match mask | per-query counts / state | conditions (CSR)
+  PinBuf filt_pin;       // filtered dense: host copies of the conditions and the per-query match counts
   DevBuf doc_chars_dev;  // K7: characters of every document's usable text (0 = blank), sb_doc_chars_load
   int64_t doc_chars_n = 0, doc_chars_base = 0;
   PinBuf pin_in, pin_out;
@@ -169,7 +175,8 @@ struct DeviceGuard {
 
 // kernel ids for sb_profile_read
 enum { SB_PROF_DENSE_SCAN = 0, SB_PROF_DENSE_MERGE = 1, SB_PROF_BM25_SCORE = 2, SB_PROF_BM25_SELECT = 3,
-       SB_PROF_FUSE = 4, SB_PROF_CE = 5, SB_PROF_DENSE_SAMPLE = 6, SB_PROF_COUNT = 7 };
+       SB_PROF_FUSE = 4, SB_PROF_CE = 5, SB_PROF_DENSE_SAMPLE = 6, SB_PROF_DENSE_FILTER = 7,
+       SB_PROF_DENSE_GATHER = 8, SB_PROF_COUNT = 9 };
 
 static inline cudaEvent_t prof_event(sb_ctx* ctx) {
   if (!ctx->prof_pool.empty()) {

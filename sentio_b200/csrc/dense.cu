@@ -81,6 +81,11 @@ struct ScanParams {
   int32_t bcap;              // capacity of each of the two append batches per query (kprime + bcap = sort size)
   int32_t stages;
   uint32_t tile_bytes;
+  // FILTER only: match bits of this pass's queries (bit r % 32 of mask[(r / 32) * mask_qs + query]) and the per-query
+  // state (1 = answered by the gather path: threshold +inf, nothing is appended)
+  const uint32_t* mask;
+  int32_t mask_qs;
+  const int32_t* state;
 };
 
 // Sum V per-lane partials across the warp: afterwards the lanes with (lane % (32/V)) == 0 hold value index lane/(32/V).
@@ -221,7 +226,7 @@ __device__ __forceinline__ unsigned long long h2_to_f2(uint32_t h2) {
   return pack_f2(f.x, f.y);
 }
 
-template <int NCHUNK, int QB, int RW, bool EXACT>
+template <int NCHUNK, int QB, int RW, bool EXACT, bool FILTER>
 __global__ void __launch_bounds__(kScanThreads, 1) dense_scan_kernel(const ScanParams p) {
   constexpr int R = kConsumerWarps * RW;  // rows per tile
   constexpr int V = RW * QB;              // partial sums per lane
@@ -255,7 +260,8 @@ __global__ void __launch_bounds__(kScanThreads, 1) dense_scan_kernel(const ScanP
   if (tid < QB) {
     cnt[2 * tid] = 0;
     cnt[2 * tid + 1] = 0;
-    thr[tid] = -INFINITY;
+    if constexpr (FILTER) thr[tid] = p.state[tid] ? INFINITY : -INFINITY;
+    else thr[tid] = -INFINITY;
     active[tid] = 0;
     pending[tid] = 0;
     frozen[tid] = 0;
@@ -361,6 +367,9 @@ __global__ void __launch_bounds__(kScanThreads, 1) dense_scan_kernel(const ScanP
     mbar_wait(bar_full0 + 8 * s, use & 1u);
     float invn = 0.f;
     if (leader) invn = __ldg(p.inv_norm + grow);  // consumed after the reduction: latency hides under the FMAs
+    uint32_t mword = 0u;
+    if constexpr (FILTER)
+      if (leader) mword = __ldg(p.mask + (size_t)(grow >> 5) * p.mask_qs + qi);
 
     unsigned long long acc[V];
 #pragma unroll
@@ -403,7 +412,9 @@ __global__ void __launch_bounds__(kScanThreads, 1) dense_scan_kernel(const ScanP
     const float dot = warp_reduce_multi<V>(part, lane);
     if (leader) {
       const float score = dot * invn;
-      if (grow < p.n && score > thr[qi]) {
+      bool match = true;
+      if constexpr (FILTER) match = (mword >> (grow & 31)) & 1u;
+      if (grow < p.n && score > thr[qi] && match) {
         const int a = active[qi];
         const int pos = atomicAdd(const_cast<int*>(&cnt[2 * qi + a]), 1);
         if (pos < p.bcap) cbuf[(size_t)qi * qstride + p.kprime + (size_t)a * p.bcap + pos] = make_key32(score, (uint32_t)grow);
@@ -462,6 +473,7 @@ struct MergeParams {
   int64_t* out_ids;          // [nq][k]
   double* out_scores;        // [nq][k]
   int32_t* out_counts;       // [nq]
+  const int32_t* state;      // FILTER only: [nq] 1 = answered by the gather path (nothing to merge)
 };
 
 __device__ __forceinline__ void block_sort_desc_u64(unsigned long long* a, int len, int tid, int nt) {
@@ -487,10 +499,13 @@ __device__ __forceinline__ void block_sort_desc_u64(unsigned long long* a, int l
 // R = ceil(K'/G) entries of every list (G*R >= K' >= k real keys); (2) every list contributes its prefix inside the
 // error window below that key; a FULL list whose last entry is still inside the window may have dropped members ->
 // fallback; (3) exact fp64 re-score of the whole window; (4) final order, emit k.
+template <bool FILTER>
 __global__ void __launch_bounds__(kMergeThreads, 1) dense_merge_kernel(const MergeParams p) {
   extern __shared__ __align__(16) uint8_t msmem[];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nt = blockDim.x, nw = nt >> 5;
   const int qi = blockIdx.x;
+  if constexpr (FILTER)
+    if (p.state[qi]) return;
   const int G = p.G, K = p.kprime;
   unsigned long long* sel = reinterpret_cast<unsigned long long*>(msmem);   // [kSelCap]
   unsigned long long* ek = sel + kSelCap;                                   // [kSelCap] exact score keys
@@ -629,8 +644,12 @@ struct FallbackParams {
   int64_t* out_ids;
   double* out_scores;
   int32_t* out_counts;
+  unsigned long long* counter;   // [1] queries answered here since the context was created
+  const uint32_t* mask;          // FILTER only: match bits, mask[(row / 32) * mask_qs + query]
+  int32_t mask_qs;
 };
 
+template <bool FILTER>
 __global__ void __launch_bounds__(kFbThreads, 1) dense_exact_fallback_kernel(const FallbackParams p) {
   const int qi = blockIdx.x;
   if (p.flag[qi] == 0) return;
@@ -639,8 +658,39 @@ __global__ void __launch_bounds__(kFbThreads, 1) dense_exact_fallback_kernel(con
   __shared__ double qq_s;
   __shared__ int s_beats;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nt = blockDim.x, nw = nt >> 5;
+  if (tid == 0) atomicAdd(p.counter, 1ull);
   const float* q = p.q + (size_t)qi * p.d_pad;
   const double qn = query_norm_cta(q, p.d_pad, &qq_s);
+  if (FILTER && !(qn > 0.0)) {
+    // all-zero query: every cosine is 0 -> the first k MATCHING rows in index order (one warp walks the mask words)
+    if (warp != 0) return;
+    const int64_t n_words = (p.n + 31) / 32;
+    int got = 0;
+    for (int64_t w0 = 0; w0 < n_words && got < p.k; w0 += 32) {
+      const int64_t w = w0 + lane;
+      uint32_t bits = w < n_words ? p.mask[(size_t)w * p.mask_qs + qi] : 0u;
+      const int c = __popc(bits);
+      int incl = c;
+      for (int o = 1; o < 32; o <<= 1) {
+        const int y = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += y;
+      }
+      for (int pos = got + incl - c; bits != 0u && pos < p.k; ++pos) {
+        const int b = __ffs(bits) - 1;
+        bits &= bits - 1u;
+        p.out_ids[(size_t)qi * p.k + pos] = p.id_base + w * 32 + b;
+        p.out_scores[(size_t)qi * p.k + pos] = 0.0;
+      }
+      got += __shfl_sync(0xffffffffu, incl, 31);
+    }
+    const int m = min(got, p.k);
+    for (int i = m + lane; i < p.k; i += 32) {
+      p.out_ids[(size_t)qi * p.k + i] = -1;
+      p.out_scores[(size_t)qi * p.k + i] = 0.0;
+    }
+    if (lane == 0) p.out_counts[qi] = m;
+    return;
+  }
   if (!(qn > 0.0)) {
     // all-zero query: every cosine is exactly 0 -> the first k rows in index order, no scan needed
     const int m = (int)min((int64_t)p.k, p.n);
@@ -664,7 +714,10 @@ __global__ void __launch_bounds__(kFbThreads, 1) dense_exact_fallback_kernel(con
     for (int c = warp; c < kFbBest; c += nw) {
       const int64_t row = r0 + c;
       unsigned long long okey = 0ull;
-      if (row < p.n) {
+      bool match = true;
+      if constexpr (FILTER)
+        if (row < p.n) match = (p.mask[(size_t)(row >> 5) * p.mask_qs + qi] >> (row & 31)) & 1u;
+      if (row < p.n && match) {
         okey = f64_orderable(exact_cosine_warp(p.rows, (uint32_t)row, q, p.d_pad, p.ch, qn, lane));
         if (okey == 0ull) okey = 1ull;
       }
@@ -690,6 +743,109 @@ __global__ void __launch_bounds__(kFbThreads, 1) dense_exact_fallback_kernel(con
   ra.out_scores = p.out_scores + (size_t)qi * p.k;
   ra.out_count = p.out_counts + qi;
   emit_exact_pairs(ek, ei, kFbBest, ra);
+}
+
+// ------------------------------------------------------------------------------------------------ filtered search
+// Match mask of a chunk of <= 256 queries: bit (row % 32) of mask[(row / 32) * qs + q] is set iff row < n satisfies
+// every condition of query q (no conditions: every row).  Each warp owns 32-row words (lane = row) and, per block of
+// 32 queries, ballots every query's predicate; lane j keeps query j's word, so a block of 32 query columns is one
+// 128-byte store.  counts[q] += popcount of its words.  Columns nq .. qs-1 are written as zero.
+constexpr int kGatherMax = 2048;   // queries with at most this many matching rows skip the scans (= winner buffer)
+
+struct MaskParams {
+  const int32_t* const* tags;   // [SB_MAX_TAG_FIELDS] device pointers of the slot's tag columns
+  const int32_t* f_off;         // [nq + 1] (absolute offsets into f_field / f_code)
+  const int32_t* f_field;
+  const int32_t* f_code;
+  int64_t n, n_words;
+  int32_t nq, qs;
+  uint32_t* mask;               // [n_words][qs]
+  int32_t* counts;              // [nq], zeroed by the caller
+};
+
+__global__ void __launch_bounds__(256) dense_filter_mask_kernel(const MaskParams p) {
+  const int lane = threadIdx.x & 31;
+  const int64_t warp0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+  int cnt[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // lane's query in block qb: qb * 32 + lane
+  for (int64_t w = warp0; w < p.n_words; w += nwarps) {
+    const int64_t row = w * 32 + lane;
+    const bool live = row < p.n;
+#pragma unroll
+    for (int qb = 0; qb < 8; ++qb) {
+      if (qb * 32 >= p.qs) break;
+      uint32_t mine = 0u;
+      for (int j = 0; j < 32; ++j) {
+        const int q = qb * 32 + j;
+        if (q >= p.nq) break;
+        bool m = live;
+        const int e = __ldg(p.f_off + q + 1);
+        for (int i = __ldg(p.f_off + q); i < e && m; ++i) {
+          const int32_t code = __ldg(p.f_code + i);
+          m = code >= 0 && __ldg(p.tags[__ldg(p.f_field + i)] + row) == code;
+        }
+        const uint32_t bits = __ballot_sync(0xffffffffu, m);
+        if (lane == j) mine = bits;
+      }
+      p.mask[(size_t)w * p.qs + qb * 32 + lane] = mine;
+      cnt[qb] += __popc(mine);
+    }
+  }
+#pragma unroll
+  for (int qb = 0; qb < 8; ++qb)
+    if (qb * 32 + lane < p.nq && cnt[qb] > 0) atomicAdd(p.counts + qb * 32 + lane, cnt[qb]);
+}
+
+// Exact path of a low-cardinality query (<= kGatherMax matching rows): one CTA compacts the query's matching rows out
+// of the mask and re-scores all of them in fp64 (rescore_and_emit, the same stage the scans end with).
+struct GatherParams {
+  const uint32_t* mask;
+  int32_t qs;
+  int64_t n_words;
+  const int32_t* qlist;      // [grid] chunk-local query index of each CTA
+  const __half* rows;
+  const float* q;            // [nq][d_pad] the caller's fp32 queries
+  int32_t d_pad, ch;
+  int64_t id_base;
+  int32_t k;
+  int64_t* out_ids;
+  double* out_scores;
+  int32_t* out_counts;
+};
+
+__global__ void __launch_bounds__(kMergeThreads, 1) dense_filter_gather_kernel(const GatherParams p) {
+  extern __shared__ __align__(16) uint8_t gsmem[];
+  unsigned long long* sel = reinterpret_cast<unsigned long long*>(gsmem);   // [kGatherMax] (key score field unused)
+  unsigned long long* ek = sel + kGatherMax;                               // [kGatherMax]
+  uint32_t* ei = reinterpret_cast<uint32_t*>(ek + kGatherMax);             // [kGatherMax]
+  float* q_s = reinterpret_cast<float*>(ei + kGatherMax);                  // [d_pad]
+  __shared__ double qq_s;
+  __shared__ int s_n;
+  const int qi = p.qlist[blockIdx.x];
+  if (threadIdx.x == 0) s_n = 0;
+  __syncthreads();
+  for (int64_t w = threadIdx.x; w < p.n_words; w += blockDim.x) {
+    uint32_t bits = p.mask[(size_t)w * p.qs + qi];
+    if (bits == 0u) continue;
+    int at = atomicAdd(&s_n, __popc(bits));
+    for (; bits != 0u; bits &= bits - 1u, ++at)
+      if (at < kGatherMax) sel[at] = make_key32(0.f, (uint32_t)(w * 32 + __ffs(bits) - 1));
+  }
+  __syncthreads();
+  const int nsel = min(s_n, kGatherMax);   // the host routes only queries with <= kGatherMax matches here
+  int P = 32;
+  while (P < nsel) P <<= 1;
+  RescoreArgs ra;
+  ra.rows = p.rows;
+  ra.q = p.q + (size_t)qi * p.d_pad;
+  ra.d_pad = p.d_pad;
+  ra.ch = p.ch;
+  ra.id_base = p.id_base;
+  ra.k = p.k;
+  ra.out_ids = p.out_ids + (size_t)qi * p.k;
+  ra.out_scores = p.out_scores + (size_t)qi * p.k;
+  ra.out_count = p.out_counts + qi;
+  rescore_and_emit(sel, nsel, P, ek, ei, &qq_s, q_s, ra);
 }
 
 // ------------------------------------------------------------------------------------------------ host side
@@ -756,14 +912,14 @@ int make_plan(sb_ctx* ctx, const DenseIndex& ix, int k, ScanPlan* pl) {
   return SB_OK;
 }
 
-template <int NCHUNK, int QB, int RW>
+template <int NCHUNK, int QB, int RW, bool FILTER>
 int launch_scan(const ScanParams& sp, const ScanPlan& pl, cudaStream_t st) {
   if (sp.ch == NCHUNK * 32) {
-    auto kern = dense_scan_kernel<NCHUNK, QB, RW, true>;
+    auto kern = dense_scan_kernel<NCHUNK, QB, RW, true, FILTER>;
     SB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.scan_smem));
     kern<<<pl.grid, kScanThreads, pl.scan_smem, st>>>(sp);
   } else {
-    auto kern = dense_scan_kernel<NCHUNK, QB, RW, false>;
+    auto kern = dense_scan_kernel<NCHUNK, QB, RW, false, FILTER>;
     SB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.scan_smem));
     kern<<<pl.grid, kScanThreads, pl.scan_smem, st>>>(sp);
   }
@@ -771,27 +927,28 @@ int launch_scan(const ScanParams& sp, const ScanPlan& pl, cudaStream_t st) {
   return SB_OK;
 }
 
-template <int NCHUNK, int RW>
+template <int NCHUNK, int RW, bool FILTER>
 int dispatch_qb(int qb, const ScanParams& sp, const ScanPlan& pl, cudaStream_t st) {
   if constexpr (NCHUNK <= 4) {
-    if (qb == 4) return launch_scan<NCHUNK, 4, RW>(sp, pl, st);
+    if (qb == 4) return launch_scan<NCHUNK, 4, RW, FILTER>(sp, pl, st);
   }
   if constexpr (NCHUNK <= 8) {
-    if (qb == 2) return launch_scan<NCHUNK, 2, RW>(sp, pl, st);
+    if (qb == 2) return launch_scan<NCHUNK, 2, RW, FILTER>(sp, pl, st);
   }
-  return launch_scan<NCHUNK, 1, RW>(sp, pl, st);
+  return launch_scan<NCHUNK, 1, RW, FILTER>(sp, pl, st);
 }
 
+template <bool FILTER>
 int dispatch_scan(int qb, const ScanParams& sp, const ScanPlan& pl, cudaStream_t st) {
   switch (pl.nchunk) {
-    case 1: return dispatch_qb<1, 4>(qb, sp, pl, st);
-    case 2: return dispatch_qb<2, 4>(qb, sp, pl, st);
-    case 3: return dispatch_qb<3, 4>(qb, sp, pl, st);
-    case 4: return dispatch_qb<4, 4>(qb, sp, pl, st);
-    case 6: return dispatch_qb<6, 2>(qb, sp, pl, st);
-    case 8: return dispatch_qb<8, 2>(qb, sp, pl, st);
-    case 12: return dispatch_qb<12, 1>(qb, sp, pl, st);
-    case 16: return dispatch_qb<16, 1>(qb, sp, pl, st);
+    case 1: return dispatch_qb<1, 4, FILTER>(qb, sp, pl, st);
+    case 2: return dispatch_qb<2, 4, FILTER>(qb, sp, pl, st);
+    case 3: return dispatch_qb<3, 4, FILTER>(qb, sp, pl, st);
+    case 4: return dispatch_qb<4, 4, FILTER>(qb, sp, pl, st);
+    case 6: return dispatch_qb<6, 2, FILTER>(qb, sp, pl, st);
+    case 8: return dispatch_qb<8, 2, FILTER>(qb, sp, pl, st);
+    case 12: return dispatch_qb<12, 1, FILTER>(qb, sp, pl, st);
+    case 16: return dispatch_qb<16, 1, FILTER>(qb, sp, pl, st);
   }
   sb_set_error("dense: unsupported chunk count %d", pl.nchunk);
   return SB_ERR_UNSUPPORTED;
@@ -802,13 +959,13 @@ int dispatch_scan(int qb, const ScanParams& sp, const ScanPlan& pl, cudaStream_t
 constexpr int kMergeChunk = 256;
 
 int dense_topk_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int B, int k, int64_t* out_ids,
-                       double* out_scores, int32_t* out_counts, cudaStream_t st) {
+                       double* out_scores, int32_t* out_counts, cudaStream_t st, const DenseFilter* flt = nullptr) {
   ScanPlan pl;
   int rc = make_plan(ctx, ix, k, &pl);
   if (rc) return rc;
   // batches of >= 16 queries ride the tensor cores: one HBM pass per 64 / 128 queries instead of one per 4
   if (ctx->dense_mode != 1 && dense_mma_eligible(ctx, ix, B))
-    return dense_mma_topk_enqueue(ctx, ix, q_pad, B, k, out_ids, out_scores, out_counts, st);
+    return dense_mma_topk_enqueue(ctx, ix, q_pad, B, k, out_ids, out_scores, out_counts, st, flt);
   const int chunk = B < kMergeChunk ? B : kMergeChunk;
   const size_t per_q = (size_t)pl.grid * pl.kprime;
   rc = ctx->cand_dev.reserve((size_t)chunk * per_q * 8);
@@ -817,13 +974,24 @@ int dense_topk_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int B, i
   float *qn = nullptr, *eps = nullptr;
   int32_t* fb = nullptr;
   if ((rc = dense_prep_queries(ctx, ix, q_pad, B, B, /*mma=*/false, &qn, nullptr, &eps, &fb, st))) return rc;
-  SB_CUDA(cudaFuncSetAttribute(dense_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.merge_smem));
+  if (flt) SB_CUDA(cudaFuncSetAttribute(dense_merge_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        (int)pl.merge_smem));
+  else SB_CUDA(cudaFuncSetAttribute(dense_merge_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                    (int)pl.merge_smem));
   for (int c0 = 0; c0 < B; c0 += chunk) {
     const int nq = std::min(chunk, B - c0);
     int b0 = 0;
     while (b0 < nq) {
       int qb = pl.qb_max;
       while (qb > nq - b0) qb >>= 1;
+      if (flt) {   // a pass whose queries are all answered by the gather path is not launched
+        bool any = false;
+        for (int i = 0; i < qb; ++i) any |= flt->state_host[c0 + b0 + i] == 0;
+        if (!any) {
+          b0 += qb;
+          continue;
+        }
+      }
       ScanParams sp;
       sp.rows = ix.rows;
       sp.inv_norm = ix.inv_norm;
@@ -837,9 +1005,12 @@ int dense_topk_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int B, i
       sp.bcap = pl.bcap;
       sp.stages = pl.stages;
       sp.tile_bytes = pl.tile_bytes;
+      sp.mask = flt ? flt->mask + (c0 + b0) : nullptr;
+      sp.mask_qs = flt ? flt->qs : 0;
+      sp.state = flt ? flt->state + (c0 + b0) : nullptr;
       {
         ProfScope ps(ctx, SB_PROF_DENSE_SCAN, st);
-        rc = dispatch_scan(qb, sp, pl, st);
+        rc = flt ? dispatch_scan<true>(qb, sp, pl, st) : dispatch_scan<false>(qb, sp, pl, st);
       }
       if (rc) return rc;
       b0 += qb;
@@ -861,13 +1032,15 @@ int dense_topk_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int B, i
     mp.out_ids = out_ids + (size_t)c0 * k;
     mp.out_scores = out_scores + (size_t)c0 * k;
     mp.out_counts = out_counts + c0;
+    mp.state = flt ? flt->state + c0 : nullptr;
     {
       ProfScope ps(ctx, SB_PROF_DENSE_MERGE, st);
-      dense_merge_kernel<<<nq, kMergeThreads, pl.merge_smem, st>>>(mp);
+      if (flt) dense_merge_kernel<true><<<nq, kMergeThreads, pl.merge_smem, st>>>(mp);
+      else dense_merge_kernel<false><<<nq, kMergeThreads, pl.merge_smem, st>>>(mp);
     }
     SB_CUDA(cudaGetLastError());
   }
-  return dense_fallback_enqueue(ctx, ix, q_pad, B, k, fb, out_ids, out_scores, out_counts, st);
+  return dense_fallback_enqueue(ctx, ix, q_pad, B, k, fb, out_ids, out_scores, out_counts, st, flt);
 }
 
 __global__ void fill_empty_topk_kernel(int64_t* ids, double* sc, int32_t* cnt, int B, int k) {
@@ -914,8 +1087,17 @@ int dense_prep_queries(sb_ctx* ctx, const DenseIndex& ix, const float* q_pad, in
 }
 
 int dense_fallback_enqueue(sb_ctx* ctx, const DenseIndex& ix, const float* q_pad, int B, int k, const int32_t* fb,
-                           int64_t* out_ids, double* out_scores, int32_t* out_counts, cudaStream_t st) {
+                           int64_t* out_ids, double* out_scores, int32_t* out_counts, cudaStream_t st,
+                           const DenseFilter* flt) {
+  if (ctx->fb_count_dev.cap == 0) {
+    int rc = ctx->fb_count_dev.reserve(8);
+    if (rc) return rc;
+    SB_CUDA(cudaMemsetAsync(ctx->fb_count_dev.p, 0, 8, st));
+  }
   FallbackParams fp;
+  fp.counter = ctx->fb_count_dev.as<unsigned long long>();
+  fp.mask = flt ? flt->mask : nullptr;
+  fp.mask_qs = flt ? flt->qs : 0;
   fp.flag = fb;
   fp.rows = ix.rows;
   fp.q = q_pad;
@@ -928,10 +1110,136 @@ int dense_fallback_enqueue(sb_ctx* ctx, const DenseIndex& ix, const float* q_pad
   fp.out_scores = out_scores;
   fp.out_counts = out_counts;
   ctx->launches += 1;
-  dense_exact_fallback_kernel<<<B, kFbThreads, 0, st>>>(fp);
+  if (flt) dense_exact_fallback_kernel<true><<<B, kFbThreads, 0, st>>>(fp);
+  else dense_exact_fallback_kernel<false><<<B, kFbThreads, 0, st>>>(fp);
   SB_CUDA(cudaGetLastError());
   return SB_OK;
 }
+
+namespace {
+
+// Filtered top-k of B queries (q_pad on the device; conditions as host CSR arrays) in chunks of <= 256 queries: per
+// chunk the match mask + match counts, one wait for the counts, then the gather path for low-cardinality queries and
+// the masked scans for the rest.
+int dense_topk_filtered_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int B, int k, const int32_t* f_off,
+                                const int32_t* f_field, const int32_t* f_code, int64_t* out_ids, double* out_scores,
+                                int32_t* out_counts, cudaStream_t st) {
+  SB_REQUIRE(k <= kDenseMaxK, SB_ERR_UNSUPPORTED, "dense: top_k %d too large (max %d per call)", k, kDenseMaxK);
+  SB_REQUIRE(f_off[0] == 0, SB_ERR_ARG, "sb_dense_topk_filtered: f_off[0] must be 0");
+  for (int b = 0; b < B; ++b)
+    SB_REQUIRE(f_off[b + 1] >= f_off[b], SB_ERR_ARG, "sb_dense_topk_filtered: f_off is not non-decreasing at %d", b);
+  const int n_conds = f_off[B];
+  for (int i = 0; i < n_conds; ++i) {
+    const int f = f_field[i];
+    SB_REQUIRE(f >= 0 && f < SB_MAX_TAG_FIELDS, SB_ERR_ARG, "sb_dense_topk_filtered: field %d out of range", f);
+    SB_REQUIRE(ix.tags[f] != nullptr, SB_ERR_STATE, "sb_dense_topk_filtered: field %d has no tag column loaded", f);
+  }
+  if (n_conds == 0)   // no query has a condition: exactly the unfiltered search
+    return dense_topk_enqueue(ctx, ix, q_pad, B, k, out_ids, out_scores, out_counts, st);
+
+  const int64_t n_words = ix.n_pad / 32;
+  int qchunk = 256;   // queries per mask; the mask (n_pad * qchunk / 8 bytes) is kept under 1 GB
+  while (qchunk > 32 && (size_t)n_words * 4 * qchunk > (1ull << 30)) qchunk >>= 1;
+  // device: tag pointers | f_off | f_field | f_code | counts [qchunk] | state [qchunk] | qlist [qchunk] | mask
+  const size_t o_off = 128, o_field = o_off + ((size_t)(B + 1) * 4 + 15) / 16 * 16;
+  const size_t o_code = o_field + ((size_t)n_conds * 4 + 15) / 16 * 16;
+  const size_t o_cnt = o_code + ((size_t)n_conds * 4 + 15) / 16 * 16;
+  const size_t o_state = o_cnt + (size_t)qchunk * 4, o_qlist = o_state + (size_t)qchunk * 4;
+  const size_t o_mask = (o_qlist + (size_t)qchunk * 4 + 255) / 256 * 256;
+  const size_t dev_bytes = o_mask + (size_t)n_words * qchunk * 4;
+  int rc;
+  if ((rc = ctx->filt_dev.reserve(dev_bytes))) return rc;
+  if ((rc = ctx->filt_pin.reserve(o_mask))) return rc;
+  uint8_t* dv = ctx->filt_dev.as<uint8_t>();
+  uint8_t* hp = ctx->filt_pin.as<uint8_t>();
+  SB_CUDA(cudaStreamSynchronize(st));   // the pinned staging may still feed an earlier call's copies
+  memcpy(hp, ix.tags, sizeof(ix.tags));
+  memcpy(hp + o_off, f_off, (size_t)(B + 1) * 4);
+  memcpy(hp + o_field, f_field, (size_t)n_conds * 4);
+  memcpy(hp + o_code, f_code, (size_t)n_conds * 4);
+  SB_CUDA(cudaMemcpyAsync(dv, hp, o_cnt, cudaMemcpyHostToDevice, st));
+  int32_t* cnt_h = reinterpret_cast<int32_t*>(hp + o_cnt);
+  int32_t* state_h = reinterpret_cast<int32_t*>(hp + o_state);
+  int32_t* qlist_h = reinterpret_cast<int32_t*>(hp + o_qlist);
+  int32_t* cnt_d = reinterpret_cast<int32_t*>(dv + o_cnt);
+  int32_t* state_d = reinterpret_cast<int32_t*>(dv + o_state);
+  int32_t* qlist_d = reinterpret_cast<int32_t*>(dv + o_qlist);
+  uint32_t* mask = reinterpret_cast<uint32_t*>(dv + o_mask);
+  const size_t gather_smem = (size_t)kGatherMax * 20 + (size_t)ix.d_pad * 4 + 64;
+  SB_CUDA(cudaFuncSetAttribute(dense_filter_gather_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                               (int)gather_smem));
+  for (int c0 = 0; c0 < B; c0 += qchunk) {
+    const int nq = std::min(qchunk, B - c0);
+    const int qs = std::max(32, next_pow2(nq));   // >= the widest wgmma group of the chunk
+    SB_CUDA(cudaMemsetAsync(cnt_d, 0, (size_t)nq * 4, st));
+    MaskParams mk;
+    mk.tags = reinterpret_cast<const int32_t* const*>(dv);
+    mk.f_off = reinterpret_cast<const int32_t*>(dv + o_off) + c0;
+    mk.f_field = reinterpret_cast<const int32_t*>(dv + o_field);
+    mk.f_code = reinterpret_cast<const int32_t*>(dv + o_code);
+    mk.n = ix.n;
+    mk.n_words = n_words;
+    mk.nq = nq;
+    mk.qs = qs;
+    mk.mask = mask;
+    mk.counts = cnt_d;
+    const int64_t blocks = std::min<int64_t>((n_words + 7) / 8, (int64_t)ctx->num_sms * 8);
+    {
+      ProfScope ps(ctx, SB_PROF_DENSE_FILTER, st);
+      dense_filter_mask_kernel<<<(unsigned)blocks, 256, 0, st>>>(mk);
+    }
+    SB_CUDA(cudaGetLastError());
+    SB_CUDA(cudaMemcpyAsync(cnt_h, cnt_d, (size_t)nq * 4, cudaMemcpyDeviceToHost, st));
+    SB_CUDA(cudaStreamSynchronize(st));
+    // route: a filtered query with <= kGatherMax matching rows is answered exactly from its matches; the others are
+    // scanned with the mask (a query without conditions matches every row)
+    int n_gather = 0;
+    int64_t c_min = ix.n;
+    for (int q = 0; q < nq; ++q) {
+      const bool filtered = f_off[c0 + q + 1] > f_off[c0 + q];
+      const bool gather = filtered && cnt_h[q] <= kGatherMax;
+      state_h[q] = gather ? 1 : 0;
+      if (gather) qlist_h[n_gather++] = q;
+      else c_min = std::min<int64_t>(c_min, cnt_h[q]);
+    }
+    SB_CUDA(cudaMemcpyAsync(state_d, state_h, (size_t)qchunk * 8, cudaMemcpyHostToDevice, st));  // state + qlist
+    const float* qc = q_pad + (size_t)c0 * ix.d_pad;
+    int64_t* oi = out_ids + (size_t)c0 * k;
+    double* os = out_scores + (size_t)c0 * k;
+    int32_t* oc = out_counts + c0;
+    if (n_gather > 0) {
+      GatherParams gp;
+      gp.mask = mask;
+      gp.qs = qs;
+      gp.n_words = n_words;
+      gp.qlist = qlist_d;
+      gp.rows = ix.rows;
+      gp.q = qc;
+      gp.d_pad = ix.d_pad;
+      gp.ch = ix.d_pad / 8;
+      gp.id_base = ix.id_base;
+      gp.k = k;
+      gp.out_ids = oi;
+      gp.out_scores = os;
+      gp.out_counts = oc;
+      ProfScope ps(ctx, SB_PROF_DENSE_GATHER, st);
+      dense_filter_gather_kernel<<<n_gather, kMergeThreads, gather_smem, st>>>(gp);
+    }
+    SB_CUDA(cudaGetLastError());
+    if (n_gather < nq) {
+      DenseFilter flt;
+      flt.mask = mask;
+      flt.qs = qs;
+      flt.state = state_d;
+      flt.state_host = state_h;
+      flt.c_min = c_min;
+      if ((rc = dense_topk_enqueue(ctx, ix, qc, nq, k, oi, os, oc, st, &flt))) return rc;
+    }
+  }
+  return SB_OK;
+}
+
+}  // namespace
 
 // Shared with other translation units (hybrid batch path, scorers).
 int sb_dense_pad_queries(sb_ctx* ctx, const DenseIndex& ix, const float* q, int B, bool q_on_device, float** q_pad_out,
@@ -962,6 +1270,8 @@ int sb_dense_load(sb_ctx* ctx, int slot, const void* vecs, int64_t n, int32_t d,
   SB_CUDA(cudaStreamSynchronize(ctx->stream));
   if (ix.rows) cudaFree(ix.rows);
   if (ix.inv_norm) cudaFree(ix.inv_norm);
+  for (int f = 0; f < SB_MAX_TAG_FIELDS; ++f)
+    if (ix.tags[f]) cudaFree(ix.tags[f]);
   ix = DenseIndex();
   ix.n = n;
   ix.d = d;
@@ -1110,6 +1420,117 @@ int sb_dense_fetch(sb_ctx* ctx, int slot, const int64_t* ids, int32_t n_ids, flo
   SB_CUDA(cudaMemcpyAsync(out, ctx->misc3_dev.p, (size_t)n_ids * ix.d * 4, cudaMemcpyDeviceToHost, ctx->stream));
   SB_CUDA(cudaStreamSynchronize(ctx->stream));
   return SB_OK;
+}
+
+int sb_dense_tags_load(sb_ctx* ctx, int slot, int32_t field, const int32_t* codes, int64_t n) {
+  SB_REQUIRE(ctx != nullptr, SB_ERR_ARG, "sb_dense_tags_load: ctx is NULL");
+  SB_REQUIRE(slot >= 0 && slot < SB_MAX_DENSE_SLOTS, SB_ERR_ARG, "sb_dense_tags_load: bad slot %d", slot);
+  SB_REQUIRE(field >= 0 && field < SB_MAX_TAG_FIELDS, SB_ERR_ARG, "sb_dense_tags_load: field %d out of range [0,%d)",
+             field, SB_MAX_TAG_FIELDS);
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  DeviceGuard g(ctx->device);
+  DenseIndex& ix = ctx->dense[slot];
+  SB_REQUIRE(ix.d > 0, SB_ERR_STATE, "sb_dense_tags_load: dense slot %d has no index loaded", slot);
+  SB_REQUIRE(n == ix.n, SB_ERR_ARG, "sb_dense_tags_load: %lld codes for %lld rows", (long long)n, (long long)ix.n);
+  SB_REQUIRE(n == 0 || codes != nullptr, SB_ERR_ARG, "sb_dense_tags_load: codes is NULL");
+  for (int64_t i = 0; i < n; ++i)
+    SB_REQUIRE(codes[i] >= -1, SB_ERR_ARG, "sb_dense_tags_load: code %d at row %lld (must be >= -1)", codes[i],
+               (long long)i);
+  SB_CUDA(cudaStreamSynchronize(ctx->stream));
+  if (ix.tags[field]) cudaFree(ix.tags[field]);
+  ix.tags[field] = nullptr;
+  SB_CUDA(cudaMalloc(&ix.tags[field], (size_t)std::max<int64_t>(n, 1) * 4));
+  if (n) SB_CUDA(cudaMemcpy(ix.tags[field], codes, (size_t)n * 4, cudaMemcpyHostToDevice));
+  return SB_OK;
+}
+
+int sb_dense_topk_filtered_dev(sb_ctx* ctx, int slot, const float* q_dev, int32_t B, int32_t k,
+                               const int32_t* f_off_dev, int32_t n_conds, const int32_t* f_field_dev,
+                               const int32_t* f_code_dev, int64_t* out_ids_dev, double* out_scores_dev,
+                               int32_t* out_counts_dev, void* stream) {
+  SB_REQUIRE(ctx != nullptr, SB_ERR_ARG, "sb_dense_topk_filtered_dev: ctx is NULL");
+  SB_REQUIRE(slot >= 0 && slot < SB_MAX_DENSE_SLOTS, SB_ERR_ARG, "sb_dense_topk_filtered_dev: bad slot %d", slot);
+  SB_REQUIRE(B >= 0 && k > 0 && n_conds >= 0, SB_ERR_ARG, "sb_dense_topk_filtered_dev: bad B=%d k=%d n_conds=%d", B, k,
+             n_conds);
+  if (B == 0) return SB_OK;
+  SB_REQUIRE(q_dev && f_off_dev && out_ids_dev && out_scores_dev && out_counts_dev, SB_ERR_ARG,
+             "sb_dense_topk_filtered_dev: NULL buffer");
+  SB_REQUIRE(n_conds == 0 || (f_field_dev && f_code_dev), SB_ERR_ARG, "sb_dense_topk_filtered_dev: NULL conditions");
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  DeviceGuard g(ctx->device);
+  cudaStream_t st = pick_stream(ctx, stream);
+  DenseIndex& ix = ctx->dense[slot];
+  SB_REQUIRE(ix.d > 0, SB_ERR_STATE, "sb_dense_topk_filtered_dev: dense slot %d has no index loaded", slot);
+  // the conditions decide which kernels run: read them once
+  std::vector<int32_t> h((size_t)B + 1 + 2 * (size_t)n_conds);
+  SB_CUDA(cudaMemcpyAsync(h.data(), f_off_dev, (size_t)(B + 1) * 4, cudaMemcpyDeviceToHost, st));
+  if (n_conds) {
+    SB_CUDA(cudaMemcpyAsync(h.data() + B + 1, f_field_dev, (size_t)n_conds * 4, cudaMemcpyDeviceToHost, st));
+    SB_CUDA(cudaMemcpyAsync(h.data() + B + 1 + n_conds, f_code_dev, (size_t)n_conds * 4, cudaMemcpyDeviceToHost, st));
+  }
+  SB_CUDA(cudaStreamSynchronize(st));
+  SB_REQUIRE(h[B] == n_conds, SB_ERR_ARG, "sb_dense_topk_filtered_dev: f_off[B] = %d != n_conds = %d", h[B], n_conds);
+  if (ix.n == 0) {
+    fill_empty_topk_kernel<<<(B * k + 255) / 256, 256, 0, st>>>(out_ids_dev, out_scores_dev, out_counts_dev, B, k);
+    SB_CUDA(cudaGetLastError());
+    return SB_OK;
+  }
+  float* q_pad = nullptr;
+  int rc = sb_dense_pad_queries(ctx, ix, q_dev, B, true, &q_pad, st);
+  if (rc) return rc;
+  return dense_topk_filtered_enqueue(ctx, ix, q_pad, B, k, h.data(), h.data() + B + 1, h.data() + B + 1 + n_conds,
+                                     out_ids_dev, out_scores_dev, out_counts_dev, st);
+}
+
+int sb_dense_topk_filtered(sb_ctx* ctx, int slot, const float* q, int32_t B, int32_t k, const int32_t* f_off,
+                           const int32_t* f_field, const int32_t* f_code, int64_t* out_ids, double* out_scores,
+                           int32_t* out_counts) {
+  SB_REQUIRE(ctx != nullptr, SB_ERR_ARG, "sb_dense_topk_filtered: ctx is NULL");
+  SB_REQUIRE(slot >= 0 && slot < SB_MAX_DENSE_SLOTS, SB_ERR_ARG, "sb_dense_topk_filtered: bad slot %d", slot);
+  SB_REQUIRE(B >= 0 && k > 0, SB_ERR_ARG, "sb_dense_topk_filtered: bad B=%d k=%d", B, k);
+  if (B == 0) return SB_OK;
+  SB_REQUIRE(q && f_off && out_ids && out_scores && out_counts, SB_ERR_ARG, "sb_dense_topk_filtered: NULL buffer");
+  SB_REQUIRE(f_off[B] == 0 || (f_field && f_code), SB_ERR_ARG, "sb_dense_topk_filtered: NULL conditions");
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  DeviceGuard g(ctx->device);
+  cudaStream_t st = ctx->stream;
+  DenseIndex& ix = ctx->dense[slot];
+  SB_REQUIRE(ix.d > 0, SB_ERR_STATE, "sb_dense_topk_filtered: dense slot %d has no index loaded", slot);
+  if (ix.n == 0) {
+    for (int i = 0; i < B * k; ++i) { out_ids[i] = -1; out_scores[i] = 0.0; }
+    for (int i = 0; i < B; ++i) out_counts[i] = 0;
+    return SB_OK;
+  }
+  int rc;
+  const size_t qbytes = (size_t)B * ix.d * sizeof(float);
+  const size_t nid = (size_t)B * k;
+  if ((rc = ctx->pin_in.reserve(qbytes))) return rc;
+  SB_CUDA(cudaStreamSynchronize(st));
+  memcpy(ctx->pin_in.p, q, qbytes);
+  float* q_pad = nullptr;
+  if ((rc = sb_dense_pad_queries(ctx, ix, ctx->pin_in.as<float>(), B, false, &q_pad, st))) return rc;
+  if ((rc = ctx->out_ids_dev.reserve(nid * 8))) return rc;
+  if ((rc = ctx->out_sc_dev.reserve(nid * 8))) return rc;
+  if ((rc = ctx->out_cnt_dev.reserve((size_t)B * 4))) return rc;
+  if ((rc = dense_topk_filtered_enqueue(ctx, ix, q_pad, B, k, f_off, f_field, f_code, ctx->out_ids_dev.as<int64_t>(),
+                                        ctx->out_sc_dev.as<double>(), ctx->out_cnt_dev.as<int32_t>(), st)))
+    return rc;
+  SB_CUDA(cudaMemcpyAsync(out_ids, ctx->out_ids_dev.p, nid * 8, cudaMemcpyDeviceToHost, st));
+  SB_CUDA(cudaMemcpyAsync(out_scores, ctx->out_sc_dev.p, nid * 8, cudaMemcpyDeviceToHost, st));
+  SB_CUDA(cudaMemcpyAsync(out_counts, ctx->out_cnt_dev.p, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
+  SB_CUDA(cudaStreamSynchronize(st));
+  return SB_OK;
+}
+
+int64_t sb_dense_fallback_count(sb_ctx* ctx) {
+  if (!ctx) return -1;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  DeviceGuard g(ctx->device);
+  if (ctx->fb_count_dev.cap == 0) return 0;
+  unsigned long long v = 0;
+  if (cudaDeviceSynchronize() != cudaSuccess) return -1;
+  if (cudaMemcpy(&v, ctx->fb_count_dev.p, 8, cudaMemcpyDeviceToHost) != cudaSuccess) return -1;
+  return (int64_t)v;
 }
 
 }  // extern "C"

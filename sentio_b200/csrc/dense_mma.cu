@@ -76,9 +76,11 @@ struct MmaScanParams {
   int32_t capg;
   int32_t stages;
   int32_t prefetch;             // boxes (16 KB) prefetched into L2 beyond the shared-memory ring (0 = off)
+  const uint32_t* mask;         // FILTER only: match bits of the group's queries, mask[(row / 32) * mask_qs + column]
+  int32_t mask_qs;
 };
 
-template <int QBN>
+template <int QBN, bool FILTER>
 __global__ void __launch_bounds__(kMmaThreads, 1)
 dense_scan_mma_kernel(const __grid_constant__ CUtensorMap tm_rows, const __grid_constant__ CUtensorMap tm_q,
                       const MmaScanParams p) {
@@ -170,18 +172,31 @@ dense_scan_mma_kernel(const __grid_constant__ CUtensorMap tm_rows, const __grid_
       const bool live0 = row0 < p.n, live1 = row0 + 8 < p.n;
       const float invn0 = live0 ? __ldg(p.inv_norm + row0) : 0.f;
       const float invn1 = live1 ? __ldg(p.inv_norm + row0 + 8) : 0.f;
+      // FILTER: row0 and row0 + 8 lie in one 32-row mask word; columns 4 j + 2 (lane % 4) + {0, 1} are one 8-byte load
+      const uint32_t* mrow = nullptr;
+      if constexpr (FILTER) mrow = p.mask + (size_t)(row0 >> 5) * p.mask_qs + 2 * (lane & 3);
+      const int sh0 = (int)(row0 & 31), sh1 = sh0 + 8;
       if (p.thr_init == nullptr) {
         // Sampling pass.  The threshold only needs a LOWER bound of the k-th best score, and the k-th largest of ANY set
         // of distinct rows' scores is one: each warp contributes the best score among its 16 rows per query (two
         // registers, then a max over the 8 lanes that share a column), one 8-byte store per (warp, query) at slot
-        // t * kSampleKeys + warp of the CTA's list.
+        // t * kSampleKeys + warp of the CTA's list.  FILTER: the best among its MATCHING rows; a warp without one
+        // reports -inf, which can only lower the threshold.
         const int slot = t * kSampleKeys + warp;
 #pragma unroll
         for (int j = 0; j < QBN / 4; j += 2) {   // acc[2 j .. 2 j + 3]: columns 4 j .. 4 j + 7
+          uint2 mw = make_uint2(0u, 0u);
+          if constexpr (FILTER) mw = __ldg(reinterpret_cast<const uint2*>(mrow + 4 * j));
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
-            const float s0 = live0 ? acc[2 * j + e] * invn0 : -INFINITY;
-            const float s1 = live1 ? acc[2 * j + 2 + e] * invn1 : -INFINITY;
+            bool m0 = live0, m1 = live1;
+            if constexpr (FILTER) {
+              const uint32_t w = e ? mw.y : mw.x;
+              m0 = m0 && ((w >> sh0) & 1u);
+              m1 = m1 && ((w >> sh1) & 1u);
+            }
+            const float s0 = m0 ? acc[2 * j + e] * invn0 : -INFINITY;
+            const float s1 = m1 ? acc[2 * j + 2 + e] * invn1 : -INFINITY;
             uint32_t best = max(f32_orderable(s0), f32_orderable(s1));
             best = max(best, __shfl_xor_sync(0xffffffffu, best, 4));
             best = max(best, __shfl_xor_sync(0xffffffffu, best, 8));
@@ -193,6 +208,8 @@ dense_scan_mma_kernel(const __grid_constant__ CUtensorMap tm_rows, const __grid_
       } else {
 #pragma unroll
         for (int j = 0; j < QBN / 4; j += 2) {   // acc[2 j .. 2 j + 3]: columns 4 j .. 4 j + 7
+          uint2 mw = make_uint2(0u, 0u);
+          if constexpr (FILTER) mw = __ldg(reinterpret_cast<const uint2*>(mrow + 4 * j));
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             if (!(h ? live1 : live0)) continue;
@@ -202,7 +219,9 @@ dense_scan_mma_kernel(const __grid_constant__ CUtensorMap tm_rows, const __grid_
             for (int e = 0; e < 2; ++e) {
               const int col = 4 * j + 2 * (lane & 3) + e;
               const float score = acc[2 * j + 2 * h + e] * invn;
-              if (score >= thr[col]) {
+              bool match = true;
+              if constexpr (FILTER) match = ((e ? mw.y : mw.x) >> (h ? sh1 : sh0)) & 1u;
+              if (score >= thr[col] && match) {
                 const int pos = atomicAdd(&cnt[col], 1);
                 if (pos < p.capg) my_cand[(size_t)col * q_stride + pos] = make_key32(score, (uint32_t)row);
               }
@@ -238,6 +257,7 @@ struct SelectParams {
   int64_t* out_ids;
   double* out_scores;
   int32_t* out_counts;
+  const int32_t* state;             // FILTER only: [nq] 1 = answered by the gather path (threshold +inf, no emit)
 };
 
 // One CTA per query.  A lower bound of the k-th best approximate key among the survivors of all CTAs by an MSB-first
@@ -247,6 +267,7 @@ struct SelectParams {
 //   mode 1: gather every survivor inside the window below it, exact fp64 re-score of all of them, emit k.
 // Survivors are staged in shared memory when they fit (the normal case: ~0.3 % of the corpus); otherwise every pass
 // streams them from HBM/L2 -- slower, still exact.
+template <bool FILTER>
 __global__ void __launch_bounds__(kSelectThreads, 2) dense_select_kernel(const SelectParams p) {
   extern __shared__ __align__(16) uint8_t ssm[];
   unsigned long long* keys = reinterpret_cast<unsigned long long*>(ssm);  // [kSelStage] staged survivors
@@ -263,6 +284,12 @@ __global__ void __launch_bounds__(kSelectThreads, 2) dense_select_kernel(const S
   if (p.mode == 0 && qi >= p.nq) {   // padded operand row: nothing may survive
     if (tid == 0) p.thr_out[qi] = INFINITY;
     return;
+  }
+  if constexpr (FILTER) {
+    if (p.state[qi]) {   // answered by the gather path: nothing may survive, nothing to emit
+      if (p.mode == 0 && tid == 0) p.thr_out[qi] = INFINITY;
+      return;
+    }
   }
   if (p.mode == 1 && p.fallback[qi] != 0) return;   // a list overflowed: the brute-force kernel answers this query
   const int32_t* counts = p.counts + (size_t)qi * G;
@@ -415,24 +442,25 @@ size_t mma_smem(int qbn, int stages) {
   return 1024 + (size_t)stages * (kATileBytes + (size_t)qbn * kBK * 2 + 16) + (size_t)qbn * 8;
 }
 
-template <int QBN>
+template <int QBN, bool FILTER>
 int launch_mma(const CUtensorMap& tm_rows, const CUtensorMap& tm_q, const MmaScanParams& mp, int grid, size_t smem,
                cudaStream_t st) {
-  auto kern = dense_scan_mma_kernel<QBN>;
+  auto kern = dense_scan_mma_kernel<QBN, FILTER>;
   SB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   kern<<<grid, kMmaThreads, smem, st>>>(tm_rows, tm_q, mp);
   SB_CUDA(cudaGetLastError());
   return SB_OK;
 }
 
+template <bool FILTER>
 int dispatch_mma(int qbn, const CUtensorMap& tm_rows, const CUtensorMap& tm_q, const MmaScanParams& mp, int grid,
                  size_t smem, cudaStream_t st) {
   switch (qbn) {
-    case 16: return launch_mma<16>(tm_rows, tm_q, mp, grid, smem, st);
-    case 32: return launch_mma<32>(tm_rows, tm_q, mp, grid, smem, st);
-    case 64: return launch_mma<64>(tm_rows, tm_q, mp, grid, smem, st);
-    case 128: return launch_mma<128>(tm_rows, tm_q, mp, grid, smem, st);
-    case 256: return launch_mma<256>(tm_rows, tm_q, mp, grid, smem, st);
+    case 16: return launch_mma<16, FILTER>(tm_rows, tm_q, mp, grid, smem, st);
+    case 32: return launch_mma<32, FILTER>(tm_rows, tm_q, mp, grid, smem, st);
+    case 64: return launch_mma<64, FILTER>(tm_rows, tm_q, mp, grid, smem, st);
+    case 128: return launch_mma<128, FILTER>(tm_rows, tm_q, mp, grid, smem, st);
+    case 256: return launch_mma<256, FILTER>(tm_rows, tm_q, mp, grid, smem, st);
   }
   sb_set_error("dense_mma: unsupported query block %d", qbn);
   return SB_ERR_UNSUPPORTED;
@@ -448,26 +476,36 @@ bool dense_mma_eligible(const sb_ctx* ctx, const DenseIndex& ix, int B) {
 }
 
 int dense_mma_topk_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int B, int k, int64_t* out_ids,
-                           double* out_scores, int32_t* out_counts, cudaStream_t st) {
+                           double* out_scores, int32_t* out_counts, cudaStream_t st, const DenseFilter* flt) {
   const int kb_count = ix.d_pad / kBK;
   const int total_tiles = (int)(ix.n_pad / kTileRows);
   const int gsz = kQbnMax;                          // operand rows per group
   const int grid = std::min(ctx->num_sms, total_tiles);
+  // filtered: a fraction phi of the rows matches the group's sparsest scanned query; a 16-row warp holds a matching row
+  // with probability hit = 1 - (1 - phi)^16, and then ~ m_eff = 16 phi / hit of them
+  const double phi = flt ? std::min(1.0, (double)std::max<int64_t>(flt->c_min, 1) / (double)ix.n) : 1.0;
+  const double hit = flt ? 1.0 - pow(1.0 - phi, (double)kSampleRows) : 1.0;
+  const double m_eff = flt ? (double)kSampleRows * phi / hit : (double)kSampleRows;
   // sampling pass geometry: a few tiles per CTA spread evenly over the corpus; every warp of a sampled tile reports the
-  // best of its 16 rows, so a query gets n_s = kSampleKeys * sample_tiles keys -- aim for n_s >= 4 k
-  const int per_cta = std::max(ctx->dense_sample_per_cta, std::min(8, (4 * k / kSampleKeys + grid - 1) / grid));
-  const int sample_tiles = std::min(per_cta * grid, total_tiles);
+  // best of its 16 rows, so a query gets n_s = kSampleKeys * sample_tiles keys -- aim for n_s >= 4 k (filtered: 4 k
+  // keys that come from a matching row, up to a sampling pass over the whole corpus)
+  const int per_cta = flt ? std::max(ctx->dense_sample_per_cta,
+                                     (int)ceil(4.0 * k / ((double)kSampleKeys * hit * grid)))
+                          : std::max(ctx->dense_sample_per_cta, std::min(8, (4 * k / kSampleKeys + grid - 1) / grid));
+  const int sample_tiles = (int)std::min<int64_t>((int64_t)per_cta * grid, total_tiles);
   const int sample_step = total_tiles / sample_tiles;
   const int sgrid = std::min(grid, sample_tiles);
   // per-(CTA, query) list capacity.  Sampling pass: kSampleKeys keys per sampled tile of the CTA.  Full pass: the
   // threshold is the k-th best of n_s maxima of 16 rows, passed by a fraction p of the rows with (1 - p)^16 = 1 - k / n_s;
   // 8x the expected rows_per_cta * p plus slack.  An overflowing list raises the query's fallback flag, so the capacity
   // only trades memory against the odds of a brute-force answer; no threshold at all (k >= n_s) means every row survives.
+  // Filtered: n_s * hit real keys over groups of m_eff matching rows, passed by a fraction p of the phi * rows_per_cta
+  // matching rows; for every scanned query (phi >= the smallest) the expected survivors are at most this many.
   const int64_t worst = (int64_t)((total_tiles + grid - 1) / grid + 1) * kTileRows;
   const int64_t samp_keys = (int64_t)((sample_tiles + sgrid - 1) / sgrid + 1) * kSampleKeys;
-  const double f = (double)k / ((double)kSampleKeys * sample_tiles);
-  const double pass = f >= 0.95 ? 1.0 : -log(1.0 - f) / (double)kSampleRows;
-  const int64_t expect = (int64_t)((double)worst * pass) + 1;
+  const double f = (double)k / ((double)kSampleKeys * sample_tiles * hit);
+  const double pass = f >= 0.95 ? 1.0 : -log(1.0 - f) / m_eff;
+  const int64_t expect = (int64_t)((double)worst * phi * pass) + 1;
   const int capg = (int)std::min<int64_t>(worst, std::max<int64_t>(8 * expect + 256, samp_keys));
   int rc;
   SB_REQUIRE(grid <= kSelectThreads, SB_ERR_UNSUPPORTED, "dense_mma: %d CTAs exceed the select kernel's prefix width", grid);
@@ -489,7 +527,17 @@ int dense_mma_topk_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int 
   }
   const CUtensorMap& tm_rows = *reinterpret_cast<const CUtensorMap*>(ix.tm_rows);
   const size_t sel_smem = (size_t)kSelStage * 8 + (size_t)kSelTop * 20 + 64;
-  SB_CUDA(cudaFuncSetAttribute(dense_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sel_smem));
+  if (flt) SB_CUDA(cudaFuncSetAttribute(dense_select_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        (int)sel_smem));
+  else SB_CUDA(cudaFuncSetAttribute(dense_select_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                    (int)sel_smem));
+  auto launch_select = [&](int nblocks, const SelectParams& s) {
+    if (flt) dense_select_kernel<true><<<nblocks, kSelectThreads, sel_smem, st>>>(s);
+    else dense_select_kernel<false><<<nblocks, kSelectThreads, sel_smem, st>>>(s);
+  };
+  auto run_mma = [&](int qbn, const CUtensorMap& tm_q, const MmaScanParams& m, int g, size_t smem) {
+    return flt ? dispatch_mma<true>(qbn, tm_rows, tm_q, m, g, smem, st) : dispatch_mma<false>(qbn, tm_rows, tm_q, m, g, smem, st);
+  };
   // normalised fp16 operand rows of the whole batch (rows beyond B are zero), eps, cleared fallback flags
   float* eps = nullptr;
   int32_t* fb = nullptr;
@@ -519,6 +567,7 @@ int dense_mma_topk_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int 
     mp.kb_count = kb_count;
     mp.capg = capg;
     mp.prefetch = ctx->dense_prefetch;
+    mp.mask_qs = flt ? flt->qs : 0;
     SelectParams sp;
     sp.cand = cand;
     sp.counts = counts;
@@ -536,6 +585,7 @@ int dense_mma_topk_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int 
     sp.out_ids = out_ids + (size_t)c0 * k;
     sp.out_scores = out_scores + (size_t)c0 * k;
     sp.out_counts = out_counts + c0;
+    sp.state = flt ? flt->state + c0 : nullptr;
     // (1) sampling passes -> safe thresholds for every query of the chunk (one select launch).  The kernel writes list
     // slot `cta` of [row][launch grid][capg], so every group is launched with exactly sgrid CTAs.
     mp.thr_init = nullptr;
@@ -550,11 +600,12 @@ int dense_mma_topk_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int 
         mp.cand = cand + (size_t)g * gsz * sgrid * capg;
         mp.counts = counts + (size_t)g * gsz * sgrid;
         mp.stages = G.stages;
-        if ((rc = dispatch_mma(G.qbn, tm_rows, G.tm_q, mp, sgrid, G.smem, st))) return rc;
+        mp.mask = flt ? flt->mask + c0 + (size_t)g * gsz : nullptr;
+        if ((rc = run_mma(G.qbn, G.tm_q, mp, sgrid, G.smem))) return rc;
       }
       sp.grid = sgrid;
       sp.mode = 0;
-      dense_select_kernel<<<rows_total, kSelectThreads, sel_smem, st>>>(sp);
+      launch_select(rows_total, sp);
     }
     SB_CUDA(cudaGetLastError());
     // (2) the full passes, then one select + exact re-score launch for the chunk
@@ -568,16 +619,17 @@ int dense_mma_topk_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int 
       mp.cand = cand + (size_t)g * gsz * grid * capg;
       mp.counts = counts + (size_t)g * gsz * grid;
       mp.stages = G.stages;
+      mp.mask = flt ? flt->mask + c0 + (size_t)g * gsz : nullptr;
       ProfScope ps(ctx, SB_PROF_DENSE_SCAN, st);
-      if ((rc = dispatch_mma(G.qbn, tm_rows, G.tm_q, mp, grid, G.smem, st))) return rc;
+      if ((rc = run_mma(G.qbn, G.tm_q, mp, grid, G.smem))) return rc;
     }
     sp.grid = grid;
     sp.mode = 1;
     {
       ProfScope ps(ctx, SB_PROF_DENSE_MERGE, st);
-      dense_select_kernel<<<nq_chunk, kSelectThreads, sel_smem, st>>>(sp);
+      launch_select(nq_chunk, sp);
     }
     SB_CUDA(cudaGetLastError());
   }
-  return dense_fallback_enqueue(ctx, ix, q_pad, B, k, fb, out_ids, out_scores, out_counts, st);
+  return dense_fallback_enqueue(ctx, ix, q_pad, B, k, fb, out_ids, out_scores, out_counts, st, flt);
 }

@@ -67,7 +67,8 @@ class B200Engine:
     def launch_count(self) -> int:
         return int(self._lib.sb_launch_count(self._h))
 
-    PROF_IDS = {"dense_scan": 0, "dense_merge": 1, "bm25_score": 2, "bm25_select": 3, "fuse": 4, "ce": 5, "dense_sample": 6}
+    PROF_IDS = {"dense_scan": 0, "dense_merge": 1, "bm25_score": 2, "bm25_select": 3, "fuse": 4, "ce": 5, "dense_sample": 6,
+                "dense_filter_mask": 7, "dense_filter_gather": 8}
 
     def profile(self, enable: bool) -> None:
         check(self._lib.sb_profile(self._h, 1 if enable else 0), "sb_profile")
@@ -117,9 +118,25 @@ class B200Engine:
         buf = (C.c_uint8 * nbytes).from_address(p)
         return np.frombuffer(buf, dtype=dt, count=int(np.prod(shape))).reshape(shape)
 
-    def dense_topk(self, q: np.ndarray, k: int, slot: int = 0, out=None):
+    def load_dense_tags(self, field: int, codes: np.ndarray, slot: int = 0) -> None:
+        """Payload index column ``field`` (< 16) of dense slot ``slot``: one int32 code per row, -1 = key absent."""
+        c = np.ascontiguousarray(codes, dtype=np.int32).reshape(-1)
+        check(self._lib.sb_dense_tags_load(self._h, slot, int(field), _ptr(c), len(c)), "sb_dense_tags_load")
+
+    def fallback_count(self) -> int:
+        """Queries answered by the brute-force fallback kernel since the engine was created (synchronises)."""
+        v = int(self._lib.sb_dense_fallback_count(self._h))
+        if v < 0:
+            raise SentioB200Error("sb_dense_fallback_count failed")
+        return v
+
+    def dense_topk(self, q: np.ndarray, k: int, slot: int = 0, out=None, filters=None):
         """``out`` = (ids [B,k] int64, scores [B,k] float64, counts [B] int32) to be filled in place (e.g. page-locked
-        arrays from ``pinned_empty``); fresh arrays otherwise."""
+        arrays from ``pinned_empty``); fresh arrays otherwise.  ``filters`` = CSR conditions (f_off int32 [B+1],
+        f_field int32, f_code int32): the exact top-k of the rows matching each query's conditions
+        (``sb_dense_topk_filtered``); None = unfiltered."""
+        if filters is not None:
+            return self._dense_topk_filtered(q, k, slot, filters)
         q = np.ascontiguousarray(np.atleast_2d(q), dtype=np.float32)
         B, d = q.shape
         if slot not in self.dense_dim:
@@ -135,7 +152,25 @@ class B200Engine:
         check(self._lib.sb_dense_topk(self._h, slot, _ptr(q), B, k, _ptr(ids), _ptr(sc), _ptr(cnt)), "sb_dense_topk")
         return ids, sc, cnt
 
-    def dense_topk_dev(self, q_t, k: int, slot: int = 0, out=None):
+    def _dense_topk_filtered(self, q, k, slot, filters):
+        q = np.ascontiguousarray(np.atleast_2d(q), dtype=np.float32)
+        B, d = q.shape
+        if slot not in self.dense_dim:
+            raise SentioB200Error(f"dense slot {slot} has no index loaded")
+        if d != self.dense_dim[slot]:
+            raise ValueError(f"query dimension {d} != index dimension {self.dense_dim[slot]}")
+        off, fld, code = (np.ascontiguousarray(a, dtype=np.int32).reshape(-1) for a in filters)
+        if len(off) != B + 1 or len(fld) != len(code) or int(off[-1]) != len(fld):
+            raise ValueError("filters must be CSR (f_off [B+1], f_field [n], f_code [n]) with f_off[B] == n")
+        ids = np.empty((B, k), dtype=np.int64)
+        sc = np.empty((B, k), dtype=np.float64)
+        cnt = np.empty(B, dtype=np.int32)
+        check(self._lib.sb_dense_topk_filtered(self._h, slot, _ptr(q), B, k, _ptr(off), _ptr(fld), _ptr(code), _ptr(ids),
+                                               _ptr(sc), _ptr(cnt)), "sb_dense_topk_filtered")
+        return ids, sc, cnt
+
+    def dense_topk_dev(self, q_t, k: int, slot: int = 0, out=None, filters=None):
+        """``filters`` = (f_off [B+1], f_field, f_code) int32 CUDA tensors, or None (unfiltered)."""
         import torch
 
         B, d = q_t.shape
@@ -145,8 +180,18 @@ class B200Engine:
             out = (torch.empty((B, k), dtype=torch.int64, device=dev), torch.empty((B, k), dtype=torch.float64, device=dev),
                    torch.empty((B,), dtype=torch.int32, device=dev))
         ids, sc, cnt = out
-        check(self._lib.sb_dense_topk_dev(self._h, slot, _tptr(q_t), B, k, _tptr(ids), _tptr(sc), _tptr(cnt),
-                                          self._stream()), "sb_dense_topk_dev")
+        if filters is None:
+            check(self._lib.sb_dense_topk_dev(self._h, slot, _tptr(q_t), B, k, _tptr(ids), _tptr(sc), _tptr(cnt),
+                                              self._stream()), "sb_dense_topk_dev")
+            return ids, sc, cnt
+        off, fld, code = filters
+        for t in (off, fld, code):
+            assert t.is_cuda and t.dtype == torch.int32 and t.is_contiguous()
+        if off.numel() != B + 1 or fld.numel() != code.numel():
+            raise ValueError("filters must be CSR (f_off [B+1], f_field [n], f_code [n])")
+        check(self._lib.sb_dense_topk_filtered_dev(self._h, slot, _tptr(q_t), B, k, _tptr(off), int(fld.numel()),
+                                                   _tptr(fld), _tptr(code), _tptr(ids), _tptr(sc), _tptr(cnt),
+                                                   self._stream()), "sb_dense_topk_filtered_dev")
         return ids, sc, cnt
 
     def dense_fetch(self, ids: Sequence[int], slot: int = 0) -> np.ndarray:

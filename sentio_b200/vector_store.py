@@ -18,6 +18,7 @@ from typing import Any, Sequence
 import numpy as np
 
 from .engine import B200Engine
+from .payload_filter import PayloadIndex
 
 __all__ = ["B200VectorStore", "ScoredPoint", "Record"]
 
@@ -46,6 +47,14 @@ class _Collection:
         self.payloads: list[dict] = []
         self.row_of: dict[Any, int] = {}
         self.dim = 0
+        self._payload_index: PayloadIndex | None = None
+
+    def payload_index(self) -> PayloadIndex:
+        # built lazily: a tag column per payload key, on the first filter that names the key
+        if self._payload_index is None:
+            self._payload_index = PayloadIndex(self.payloads,
+                                               lambda f, codes: self.engine.load_dense_tags(f, codes, slot=0))
+        return self._payload_index
 
 
 class B200VectorStore:
@@ -92,7 +101,10 @@ class B200VectorStore:
 
     # ------------------------------------------------------------------ the calls the hot path makes
     def search(self, collection_name: str, query_vector, limit: int = 10, with_payload: bool = True,
-               with_vectors: bool = False, **_ignored) -> list[ScoredPoint]:
+               with_vectors: bool = False, query_filter=None, **_ignored) -> list[ScoredPoint]:
+        """``query_filter``: a Qdrant ``Filter(must=[FieldCondition(key, match=MatchValue(value))...])`` or a bare
+        ``FieldCondition`` (what the reference's ``_convert_filter`` emits): the exact top-``limit`` of the points whose
+        payload satisfies every condition.  Other filter shapes raise ``ValueError`` (sentio_b200/payload_filter.py)."""
         col = self._collections.get(collection_name)
         if col is None:
             raise ValueError(f"Collection {collection_name} not found")
@@ -100,7 +112,9 @@ class B200VectorStore:
             query_vector = query_vector[1]
         q = np.asarray(query_vector, dtype=np.float32).reshape(1, -1)
         limit = max(1, min(int(limit), max(len(col.ids), 1)))   # Qdrant never returns more points than the collection holds
-        ids, scores, counts = col.engine.dense_topk(q, int(limit))
+        filters = self._compile_filters(col, [query_filter]) if query_filter is not None else None
+        ids, scores, counts = col.engine.dense_topk(q, int(limit), filters=filters) if filters is not None \
+            else col.engine.dense_topk(q, int(limit))
         out = []
         for j in range(int(counts[0])):
             row = int(ids[0, j])
@@ -109,8 +123,9 @@ class B200VectorStore:
         return out
 
     def search_batch(self, collection_name: str, query_vectors, limit: int = 10, with_payload: bool = True,
-                     **_ignored) -> list[list[ScoredPoint]]:
-        """``search`` for many query vectors in ONE device batch (the wgmma scan serves 256 queries per HBM pass)."""
+                     query_filter=None, **_ignored) -> list[list[ScoredPoint]]:
+        """``search`` for many query vectors in ONE device batch (the wgmma scan serves 256 queries per HBM pass).
+        ``query_filter``: one filter for the whole batch, or a list / tuple with one filter (or None) per query."""
         col = self._collections.get(collection_name)
         if col is None:
             raise ValueError(f"Collection {collection_name} not found")
@@ -119,10 +134,24 @@ class B200VectorStore:
             raise ValueError("query_vectors must be [B, d]")
         if q.shape[0] == 0:
             return []
-        ids, scores, counts = col.engine.dense_topk(q, int(limit))
+        filters = None
+        if query_filter is not None:
+            per_query = list(query_filter) if isinstance(query_filter, (list, tuple)) else [query_filter] * q.shape[0]
+            if len(per_query) != q.shape[0]:
+                raise ValueError(f"query_filter: {len(per_query)} filters for {q.shape[0]} queries")
+            if any(f is not None for f in per_query):
+                filters = self._compile_filters(col, per_query)
+        ids, scores, counts = col.engine.dense_topk(q, int(limit), filters=filters) if filters is not None \
+            else col.engine.dense_topk(q, int(limit))
         return [[ScoredPoint(id=col.ids[int(ids[b, j])], score=float(scores[b, j]),
                              payload=col.payloads[int(ids[b, j])] if with_payload else None)
                  for j in range(int(counts[b]))] for b in range(q.shape[0])]
+
+    @staticmethod
+    def _compile_filters(col: _Collection, filters):
+        """CSR conditions for the engine, or None when no query has a condition (the unfiltered search)."""
+        off, fld, code = col.payload_index().compile(filters)
+        return (off, fld, code) if len(fld) else None
 
     def search_batch_arrays(self, collection_name: str, query_vectors: np.ndarray, limit: int):
         """Batched extension: (rows [B,k] int64, scores [B,k] float64, counts [B]) without Python objects."""
