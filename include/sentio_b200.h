@@ -148,6 +148,33 @@ int sb_dense_topk_filtered_dev(sb_ctx* ctx, int slot, const float* q_dev, int32_
                                const int32_t* f_code_dev, int64_t* out_ids_dev, double* out_scores_dev,
                                int32_t* out_counts_dev, void* stream);
 int64_t sb_dense_fallback_count(sb_ctx* ctx);
+/*
+ * Point upsert / delete in place -- the write half of the Qdrant client (`client.upsert(collection, points=...)`,
+ * `client.delete(collection, points_selector=PointIdsList(...))`, reference src/core/vector_store/qdrant_store.py:196-206,
+ * 298-349).  A slot holds rows [0, count) densely; capacity past that is zero (tag code -1).  A mutated slot is
+ * indistinguishable from one freshly loaded with the same rows in the same order: the same fp16 rows, inverse norms and
+ * tag codes, so the same search results bit for bit (DESIGN.md K1d).  Every call below validates all of its input
+ * before it modifies anything (a rejected call leaves the slot unchanged), synchronises the context's device first (a
+ * search enqueued earlier on any stream finishes against the old contents) and returns after its own work is done.
+ * An empty slot is sb_dense_load(slot, NULL, 0, d, ...).
+ *
+ * sb_dense_reserve: grow the slot's capacity to at least n_cap rows (never shrinks).  Without it, an upsert that
+ * outgrows the capacity reallocates to max(needed, 1.5 x capacity) rows, with old and new buffers alive during the copy.
+ * sb_dense_upsert: stores vecs[i] (n rows of sb_dense_dim values, dtype as sb_dense_load, same conversion) at row
+ * rows[i].  rows[i] < count overwrites; rows >= count must be exactly count .. count+m-1 (any order); no row twice; the
+ * count stays under 2^31.  Every loaded tag column is set to -1 on the written rows (sb_dense_tags_write sets codes).
+ * sb_dense_tags_write: codes[i] (>= -1) -> tag column `field` (loaded) at rows[i] (distinct, < count).
+ * sb_dense_delete: removes rows[0..n) (distinct, < count) by swap-compaction: the surviving rows among the last n rows,
+ * in ascending order, move into the deleted rows below count - n, also in ascending order, carrying their inverse norm
+ * and tag codes; the vacated tail is zeroed.  The moves are returned as moved_from[i] -> moved_to[i], i < *n_moved
+ * (moved_from / moved_to: capacity n), so the caller can update its row -> id map.  Exact score ties still break by
+ * ascending row, but after a delete row order is no longer insertion order.
+ */
+int sb_dense_reserve(sb_ctx* ctx, int slot, int64_t n_cap);
+int sb_dense_upsert(sb_ctx* ctx, int slot, const int64_t* rows, const void* vecs, int64_t n, int32_t dtype);
+int sb_dense_tags_write(sb_ctx* ctx, int slot, int32_t field, const int64_t* rows, const int32_t* codes, int64_t n);
+int sb_dense_delete(sb_ctx* ctx, int slot, const int64_t* rows, int64_t n, int64_t* moved_from, int64_t* moved_to,
+                    int64_t* n_moved);
 
 /* ---------------------------------------------------------------- K2: BM25 ---------------------------------- */
 /*

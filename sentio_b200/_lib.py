@@ -55,6 +55,11 @@ SIGNATURES = {
                                              C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                              C.c_void_p]),
     "sb_dense_fallback_count": (C.c_int64, [C.c_void_p]),
+    "sb_dense_reserve": (C.c_int, [C.c_void_p, C.c_int, C.c_int64]),
+    "sb_dense_upsert": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32]),
+    "sb_dense_tags_write": (C.c_int, [C.c_void_p, C.c_int, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64]),
+    "sb_dense_delete": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
+                                  C.POINTER(C.c_int64)]),
     "sb_bm25_load": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p,
                                C.c_int64, C.c_double, C.c_void_p, C.c_int32, C.c_double, C.c_double, C.c_double,
                                C.c_int64]),

@@ -87,15 +87,19 @@ struct PinBuf {
 // ------------------------------------------------------------------ index state
 struct DenseIndex {
   int64_t n = 0;        // valid rows
-  int64_t n_pad = 0;    // rows allocated (multiple of 32, zero filled)
+  int64_t n_pad = 0;    // rows the scans cover: round_up(n, 128)
+  int64_t n_cap = 0;    // rows allocated in rows / inv_norm / every tag column (>= n_pad, multiple of 128); rows in
+                        // [n, n_cap) are zero with inv_norm 0 and tag code -1
   int32_t d = 0;        // logical dimension
   int32_t d_pad = 0;    // stored row length in halves (multiple of 8 -> 16 B aligned rows)
   int64_t id_base = 0;
-  __half* rows = nullptr;    // [n_pad][d_pad]
-  float* inv_norm = nullptr; // [n_pad], 1/||row|| of the STORED fp16 row (0 for zero rows)
-  // cached CUtensorMap (128 bytes, 64-byte aligned) over rows[] for the wgmma batched scan; valid iff tm_rows_ptr == rows
+  __half* rows = nullptr;    // [n_cap][d_pad]
+  float* inv_norm = nullptr; // [n_cap], 1/||row|| of the STORED fp16 row (0 for zero rows)
+  // cached CUtensorMap (128 bytes, 64-byte aligned) over rows[0, n_pad) for the wgmma batched scan; valid iff
+  // tm_rows_ptr == rows and tm_n_pad == n_pad (an append within capacity keeps `rows` but widens n_pad)
   alignas(64) unsigned char tm_rows[128] = {0};
   const void* tm_rows_ptr = nullptr;
+  int64_t tm_n_pad = 0;
   // payload index for filtered search (sb_dense_tags_load): tags[f][row] = dictionary code of field f, -1 = key absent;
   // nullptr = field f not loaded.  Dropped by sb_dense_load.
   int32_t* tags[SB_MAX_TAG_FIELDS] = {};

@@ -32,16 +32,18 @@ constexpr int kRowPad = 128;  // n_pad granularity (tile rows of the wgmma scan;
 
 // ------------------------------------------------------------------------------------------------ load kernels
 // One warp per row.  f32 input: x16 = fp16(x / ||x||) (division in fp64, single rounding); f16 input: verbatim.
-// inv_norm = 1/||x16|| of the stored values (fp64 accumulate), 0 for all-zero rows.
+// inv_norm = 1/||x16|| of the stored values (fp64 accumulate), 0 for all-zero rows.  Input row r goes to row row0 + r,
+// or to dst_rows[r] when a destination list is given (sb_dense_upsert).
 template <typename TIn>
 __global__ void dense_store_rows_kernel(const TIn* __restrict__ in, int64_t n_rows, int32_t d, int32_t d_pad,
                                         __half* __restrict__ rows, float* __restrict__ inv_norm, int64_t row0,
-                                        bool normalise) {
+                                        const int64_t* __restrict__ dst_rows, bool normalise) {
   int64_t r = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   int lane = threadIdx.x & 31;
   if (r >= n_rows) return;
+  const int64_t out_row = dst_rows ? dst_rows[r] : row0 + r;
   const TIn* src = in + r * (int64_t)d;
-  __half* dst = rows + (row0 + r) * (int64_t)d_pad;
+  __half* dst = rows + out_row * (int64_t)d_pad;
   double scale = 1.0;
   if (normalise) {
     double ss = 0.0;
@@ -64,7 +66,42 @@ __global__ void dense_store_rows_kernel(const TIn* __restrict__ in, int64_t n_ro
     ss16 += hv * hv;
   }
   for (int o = 16; o; o >>= 1) ss16 += __shfl_xor_sync(0xffffffffu, ss16, o);
-  if (lane == 0) inv_norm[row0 + r] = ss16 > 0.0 ? (float)(1.0 / sqrt(ss16)) : 0.f;
+  if (lane == 0) inv_norm[out_row] = ss16 > 0.0 ? (float)(1.0 / sqrt(ss16)) : 0.f;
+}
+
+// ------------------------------------------------------------------------------------------------ mutation kernels
+// sb_dense_delete's compaction: one warp per move from[m] -> to[m] (sources >= n - |D| > destinations, so one launch
+// has no read/write hazard): the fp16 row in 16-byte copies, its inverse norm and its code in every loaded tag column.
+struct MoveParams {
+  __half* rows;
+  float* inv_norm;
+  int32_t* tags[SB_MAX_TAG_FIELDS];   // nullptr = field not loaded
+  const int64_t* from;
+  const int64_t* to;
+  int64_t n_moves;
+  int32_t ch;                         // 16-byte chunks per row = d_pad / 8
+};
+
+__global__ void __launch_bounds__(256) dense_move_rows_kernel(const MoveParams p) {
+  const int64_t m = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (m >= p.n_moves) return;
+  const int64_t s = p.from[m], t = p.to[m];
+  const uint4* src = reinterpret_cast<const uint4*>(p.rows) + s * p.ch;
+  uint4* dst = reinterpret_cast<uint4*>(p.rows) + t * p.ch;
+  for (int c = lane; c < p.ch; c += 32) dst[c] = src[c];
+  if (lane == 0) p.inv_norm[t] = p.inv_norm[s];
+#pragma unroll
+  for (int f = 0; f < SB_MAX_TAG_FIELDS; ++f)
+    if (lane == f + 1 && p.tags[f] != nullptr) p.tags[f][t] = p.tags[f][s];
+}
+
+// codes[i] -> col[rows[i]]; codes == nullptr writes -1 (an upserted row's payload is unknown until its codes arrive)
+__global__ void __launch_bounds__(256) dense_tags_scatter_kernel(int32_t* __restrict__ col,
+                                                                 const int64_t* __restrict__ rows,
+                                                                 const int32_t* __restrict__ codes, int64_t n) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) col[rows[i]] = codes ? codes[i] : -1;
 }
 
 // ------------------------------------------------------------------------------------------------ scan kernel
@@ -1239,6 +1276,94 @@ int dense_topk_filtered_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad,
   return SB_OK;
 }
 
+int64_t round_rows(int64_t n) { return (n + kRowPad - 1) / kRowPad * kRowPad; }
+
+// The one store-rows path of sb_dense_load and sb_dense_upsert: n host rows (SB_F32 / SB_F16) through a device staging
+// buffer in chunks, converted by dense_store_rows_kernel into rows row0 + i, or dst_dev[i] (a device list) when given.
+// Returns after the last chunk has been stored.
+int dense_store_staged(sb_ctx* ctx, DenseIndex& ix, const void* vecs, int64_t n, int32_t dtype, const int64_t* dst_dev,
+                       int64_t row0) {
+  const int d = ix.d;
+  const size_t esz = dtype == SB_F32 ? 4 : 2;
+  const int64_t chunk_rows = std::max<int64_t>(1, (int64_t)((256ull << 20) / ((size_t)d * esz)));
+  int rc = ctx->misc_dev.reserve((size_t)std::min<int64_t>(chunk_rows, n) * d * esz);
+  if (rc) return rc;
+  for (int64_t r0 = 0; r0 < n; r0 += chunk_rows) {
+    const int64_t nr = std::min<int64_t>(chunk_rows, n - r0);
+    const uint8_t* src = reinterpret_cast<const uint8_t*>(vecs) + (size_t)r0 * d * esz;
+    SB_CUDA(cudaMemcpyAsync(ctx->misc_dev.p, src, (size_t)nr * d * esz, cudaMemcpyHostToDevice, ctx->stream));
+    const int wpb = 8;
+    const unsigned blocks = (unsigned)((nr + wpb - 1) / wpb);
+    const int64_t* dst = dst_dev ? dst_dev + r0 : nullptr;
+    if (dtype == SB_F32)
+      dense_store_rows_kernel<float><<<blocks, wpb * 32, 0, ctx->stream>>>(ctx->misc_dev.as<float>(), nr, d, ix.d_pad,
+                                                                           ix.rows, ix.inv_norm, row0 + r0, dst, true);
+    else
+      dense_store_rows_kernel<__half><<<blocks, wpb * 32, 0, ctx->stream>>>(ctx->misc_dev.as<__half>(), nr, d, ix.d_pad,
+                                                                            ix.rows, ix.inv_norm, row0 + r0, dst, false);
+    SB_CUDA(cudaGetLastError());
+    SB_CUDA(cudaStreamSynchronize(ctx->stream));  // staging buffer is reused by the next chunk
+  }
+  return SB_OK;
+}
+
+// Reallocate rows / inv_norm / every loaded tag column to n_cap rows (> ix.n_cap): the [0, n_pad) prefix is copied
+// device to device, the rest is zero (tags -1).  Old and new buffers coexist during the copy.
+int dense_grow(sb_ctx* ctx, DenseIndex& ix, int64_t n_cap) {
+  const size_t rb = (size_t)ix.d_pad * sizeof(__half);
+  __half* rows = nullptr;
+  float* inv = nullptr;
+  int32_t* tags[SB_MAX_TAG_FIELDS] = {};
+  cudaError_t e = cudaMalloc(&rows, (size_t)n_cap * rb);
+  if (e == cudaSuccess) e = cudaMalloc(&inv, (size_t)n_cap * sizeof(float));
+  for (int f = 0; f < SB_MAX_TAG_FIELDS && e == cudaSuccess; ++f)
+    if (ix.tags[f]) e = cudaMalloc(&tags[f], (size_t)n_cap * 4);
+  const int64_t keep = ix.n_pad;
+  cudaStream_t st = ctx->stream;
+  if (e == cudaSuccess && keep) e = cudaMemcpyAsync(rows, ix.rows, (size_t)keep * rb, cudaMemcpyDeviceToDevice, st);
+  if (e == cudaSuccess && keep)
+    e = cudaMemcpyAsync(inv, ix.inv_norm, (size_t)keep * sizeof(float), cudaMemcpyDeviceToDevice, st);
+  if (e == cudaSuccess) e = cudaMemsetAsync(rows + (size_t)keep * ix.d_pad, 0, (size_t)(n_cap - keep) * rb, st);
+  if (e == cudaSuccess) e = cudaMemsetAsync(inv + keep, 0, (size_t)(n_cap - keep) * sizeof(float), st);
+  for (int f = 0; f < SB_MAX_TAG_FIELDS && e == cudaSuccess; ++f) {
+    if (!tags[f]) continue;
+    if (keep) e = cudaMemcpyAsync(tags[f], ix.tags[f], (size_t)keep * 4, cudaMemcpyDeviceToDevice, st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(tags[f] + keep, 0xff, (size_t)(n_cap - keep) * 4, st);
+  }
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  if (e != cudaSuccess) {   // the slot keeps its old buffers; the new ones are released on every failure
+    cudaStreamSynchronize(st);
+    cudaFree(rows);
+    cudaFree(inv);
+    for (int f = 0; f < SB_MAX_TAG_FIELDS; ++f) cudaFree(tags[f]);
+    sb_set_error("dense: growing slot to %lld rows failed: %s", (long long)n_cap, cudaGetErrorString(e));
+    return SB_ERR_CUDA;
+  }
+  cudaFree(ix.rows);
+  cudaFree(ix.inv_norm);
+  ix.rows = rows;
+  ix.inv_norm = inv;
+  for (int f = 0; f < SB_MAX_TAG_FIELDS; ++f)
+    if (ix.tags[f]) {
+      cudaFree(ix.tags[f]);
+      ix.tags[f] = tags[f];
+    }
+  ix.n_cap = n_cap;
+  return SB_OK;
+}
+
+// rows[0..n) all in [0, limit) and pairwise distinct; `sorted` receives them in ascending order
+int check_rows(const char* who, const int64_t* rows, int64_t n, int64_t limit, std::vector<int64_t>& sorted) {
+  sorted.assign(rows, rows + n);
+  std::sort(sorted.begin(), sorted.end());
+  for (int64_t i = 0; i < n; ++i) {
+    SB_REQUIRE(sorted[i] >= 0 && sorted[i] < limit, SB_ERR_ARG, "%s: row %lld out of range [0, %lld)", who,
+               (long long)sorted[i], (long long)limit);
+    SB_REQUIRE(i == 0 || sorted[i] != sorted[i - 1], SB_ERR_ARG, "%s: row %lld given twice", who, (long long)sorted[i]);
+  }
+  return SB_OK;
+}
+
 }  // namespace
 
 // Shared with other translation units (hybrid batch path, scorers).
@@ -1276,33 +1401,151 @@ int sb_dense_load(sb_ctx* ctx, int slot, const void* vecs, int64_t n, int32_t d,
   ix.n = n;
   ix.d = d;
   ix.d_pad = (d + 7) / 8 * 8;
-  ix.n_pad = (n + kRowPad - 1) / kRowPad * kRowPad;
+  ix.n_pad = round_rows(n);
   ix.id_base = id_base;
   if (n == 0) return SB_OK;
-  SB_CUDA(cudaMalloc(&ix.rows, (size_t)ix.n_pad * ix.d_pad * sizeof(__half)));
-  SB_CUDA(cudaMalloc(&ix.inv_norm, (size_t)ix.n_pad * sizeof(float)));
-  SB_CUDA(cudaMemsetAsync(ix.rows, 0, (size_t)ix.n_pad * ix.d_pad * sizeof(__half), ctx->stream));
-  SB_CUDA(cudaMemsetAsync(ix.inv_norm, 0, (size_t)ix.n_pad * sizeof(float), ctx->stream));
-  // staged upload: chunks of rows through a device staging buffer
-  const size_t esz = dtype == SB_F32 ? 4 : 2;
-  const int64_t chunk_rows = std::max<int64_t>(1, (int64_t)((256ull << 20) / ((size_t)d * esz)));
-  int rc = ctx->misc_dev.reserve((size_t)std::min<int64_t>(chunk_rows, n) * d * esz);
+  ix.n_cap = ix.n_pad;
+  SB_CUDA(cudaMalloc(&ix.rows, (size_t)ix.n_cap * ix.d_pad * sizeof(__half)));
+  SB_CUDA(cudaMalloc(&ix.inv_norm, (size_t)ix.n_cap * sizeof(float)));
+  SB_CUDA(cudaMemsetAsync(ix.rows, 0, (size_t)ix.n_cap * ix.d_pad * sizeof(__half), ctx->stream));
+  SB_CUDA(cudaMemsetAsync(ix.inv_norm, 0, (size_t)ix.n_cap * sizeof(float), ctx->stream));
+  return dense_store_staged(ctx, ix, vecs, n, dtype, nullptr, 0);
+}
+
+int sb_dense_reserve(sb_ctx* ctx, int slot, int64_t n_cap) {
+  SB_REQUIRE(ctx != nullptr, SB_ERR_ARG, "sb_dense_reserve: ctx is NULL");
+  SB_REQUIRE(slot >= 0 && slot < SB_MAX_DENSE_SLOTS, SB_ERR_ARG, "sb_dense_reserve: bad slot %d", slot);
+  SB_REQUIRE(n_cap >= 0 && n_cap < (1ll << 31), SB_ERR_ARG, "sb_dense_reserve: bad capacity %lld", (long long)n_cap);
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  DeviceGuard g(ctx->device);
+  DenseIndex& ix = ctx->dense[slot];
+  SB_REQUIRE(ix.d > 0, SB_ERR_STATE, "sb_dense_reserve: dense slot %d has no index loaded", slot);
+  const int64_t want = round_rows(n_cap);
+  if (want <= ix.n_cap) return SB_OK;
+  SB_CUDA(cudaDeviceSynchronize());   // searches enqueued on other streams may still read the old buffers
+  return dense_grow(ctx, ix, want);
+}
+
+int sb_dense_upsert(sb_ctx* ctx, int slot, const int64_t* rows, const void* vecs, int64_t n, int32_t dtype) {
+  SB_REQUIRE(ctx != nullptr, SB_ERR_ARG, "sb_dense_upsert: ctx is NULL");
+  SB_REQUIRE(slot >= 0 && slot < SB_MAX_DENSE_SLOTS, SB_ERR_ARG, "sb_dense_upsert: bad slot %d", slot);
+  SB_REQUIRE(n >= 0, SB_ERR_ARG, "sb_dense_upsert: bad n=%lld", (long long)n);
+  SB_REQUIRE(dtype == SB_F32 || dtype == SB_F16, SB_ERR_ARG, "sb_dense_upsert: dtype must be SB_F32 or SB_F16");
+  SB_REQUIRE(n == 0 || (rows != nullptr && vecs != nullptr), SB_ERR_ARG, "sb_dense_upsert: NULL buffer");
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  DeviceGuard g(ctx->device);
+  DenseIndex& ix = ctx->dense[slot];
+  SB_REQUIRE(ix.d > 0, SB_ERR_STATE, "sb_dense_upsert: dense slot %d has no index loaded", slot);
+  if (n == 0) return SB_OK;
+  // rows < count overwrite; the others must be exactly count .. count + m - 1
+  SB_REQUIRE(n < (1ll << 31) && ix.n + n < (1ll << 31), SB_ERR_ARG, "sb_dense_upsert: a shard holds at most 2^31-1 rows");
+  std::vector<int64_t> sorted;
+  int rc = check_rows("sb_dense_upsert", rows, n, ix.n + n, sorted);
   if (rc) return rc;
-  for (int64_t r0 = 0; r0 < n; r0 += chunk_rows) {
-    const int64_t nr = std::min<int64_t>(chunk_rows, n - r0);
-    const uint8_t* src = reinterpret_cast<const uint8_t*>(vecs) + (size_t)r0 * d * esz;
-    SB_CUDA(cudaMemcpyAsync(ctx->misc_dev.p, src, (size_t)nr * d * esz, cudaMemcpyHostToDevice, ctx->stream));
-    const int wpb = 8;
-    const unsigned blocks = (unsigned)((nr + wpb - 1) / wpb);
-    if (dtype == SB_F32)
-      dense_store_rows_kernel<float><<<blocks, wpb * 32, 0, ctx->stream>>>(ctx->misc_dev.as<float>(), nr, d, ix.d_pad,
-                                                                           ix.rows, ix.inv_norm, r0, true);
-    else
-      dense_store_rows_kernel<__half><<<blocks, wpb * 32, 0, ctx->stream>>>(ctx->misc_dev.as<__half>(), nr, d,
-                                                                            ix.d_pad, ix.rows, ix.inv_norm, r0, false);
-    SB_CUDA(cudaGetLastError());
-    SB_CUDA(cudaStreamSynchronize(ctx->stream));  // staging buffer is reused by the next chunk
+  const int64_t m = sorted.end() - std::lower_bound(sorted.begin(), sorted.end(), ix.n);
+  SB_REQUIRE(m == 0 || (sorted[n - m] == ix.n && sorted[n - 1] == ix.n + m - 1), SB_ERR_ARG,
+             "sb_dense_upsert: appended rows must be exactly %lld .. %lld", (long long)ix.n, (long long)(ix.n + m - 1));
+  SB_CUDA(cudaDeviceSynchronize());   // searches enqueued on other streams may still read the slot
+  const int64_t n_new = ix.n + m;
+  if (round_rows(n_new) > ix.n_cap)
+    if ((rc = dense_grow(ctx, ix, std::max(round_rows(n_new), round_rows(ix.n_cap + ix.n_cap / 2))))) return rc;
+  if ((rc = ctx->misc2_dev.reserve((size_t)n * 8))) return rc;
+  int64_t* dst = ctx->misc2_dev.as<int64_t>();
+  SB_CUDA(cudaMemcpyAsync(dst, rows, (size_t)n * 8, cudaMemcpyHostToDevice, ctx->stream));
+  if ((rc = dense_store_staged(ctx, ix, vecs, n, dtype, dst, 0))) return rc;
+  for (int f = 0; f < SB_MAX_TAG_FIELDS; ++f)
+    if (ix.tags[f])
+      dense_tags_scatter_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(ix.tags[f], dst, nullptr, n);
+  SB_CUDA(cudaGetLastError());
+  SB_CUDA(cudaStreamSynchronize(ctx->stream));
+  ix.n = n_new;
+  ix.n_pad = round_rows(n_new);
+  return SB_OK;
+}
+
+int sb_dense_tags_write(sb_ctx* ctx, int slot, int32_t field, const int64_t* rows, const int32_t* codes, int64_t n) {
+  SB_REQUIRE(ctx != nullptr, SB_ERR_ARG, "sb_dense_tags_write: ctx is NULL");
+  SB_REQUIRE(slot >= 0 && slot < SB_MAX_DENSE_SLOTS, SB_ERR_ARG, "sb_dense_tags_write: bad slot %d", slot);
+  SB_REQUIRE(field >= 0 && field < SB_MAX_TAG_FIELDS, SB_ERR_ARG, "sb_dense_tags_write: field %d out of range [0,%d)",
+             field, SB_MAX_TAG_FIELDS);
+  SB_REQUIRE(n >= 0, SB_ERR_ARG, "sb_dense_tags_write: bad n=%lld", (long long)n);
+  SB_REQUIRE(n == 0 || (rows != nullptr && codes != nullptr), SB_ERR_ARG, "sb_dense_tags_write: NULL buffer");
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  DeviceGuard g(ctx->device);
+  DenseIndex& ix = ctx->dense[slot];
+  SB_REQUIRE(ix.d > 0, SB_ERR_STATE, "sb_dense_tags_write: dense slot %d has no index loaded", slot);
+  SB_REQUIRE(ix.tags[field] != nullptr, SB_ERR_STATE, "sb_dense_tags_write: field %d has no tag column loaded", field);
+  std::vector<int64_t> sorted;
+  int rc = check_rows("sb_dense_tags_write", rows, n, ix.n, sorted);
+  if (rc) return rc;
+  for (int64_t i = 0; i < n; ++i)
+    SB_REQUIRE(codes[i] >= -1, SB_ERR_ARG, "sb_dense_tags_write: code %d at entry %lld (must be >= -1)", codes[i],
+               (long long)i);
+  if (n == 0) return SB_OK;
+  SB_CUDA(cudaDeviceSynchronize());
+  if ((rc = ctx->misc2_dev.reserve((size_t)n * 12))) return rc;
+  int64_t* r_dev = ctx->misc2_dev.as<int64_t>();
+  int32_t* c_dev = reinterpret_cast<int32_t*>(r_dev + n);
+  SB_CUDA(cudaMemcpyAsync(r_dev, rows, (size_t)n * 8, cudaMemcpyHostToDevice, ctx->stream));
+  SB_CUDA(cudaMemcpyAsync(c_dev, codes, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
+  dense_tags_scatter_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(ix.tags[field], r_dev, c_dev, n);
+  SB_CUDA(cudaGetLastError());
+  SB_CUDA(cudaStreamSynchronize(ctx->stream));
+  return SB_OK;
+}
+
+int sb_dense_delete(sb_ctx* ctx, int slot, const int64_t* rows, int64_t n, int64_t* moved_from, int64_t* moved_to,
+                    int64_t* n_moved) {
+  SB_REQUIRE(ctx != nullptr, SB_ERR_ARG, "sb_dense_delete: ctx is NULL");
+  SB_REQUIRE(slot >= 0 && slot < SB_MAX_DENSE_SLOTS, SB_ERR_ARG, "sb_dense_delete: bad slot %d", slot);
+  SB_REQUIRE(n >= 0 && n_moved != nullptr, SB_ERR_ARG, "sb_dense_delete: bad arguments");
+  SB_REQUIRE(n == 0 || (rows != nullptr && moved_from != nullptr && moved_to != nullptr), SB_ERR_ARG,
+             "sb_dense_delete: NULL buffer");
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  DeviceGuard g(ctx->device);
+  DenseIndex& ix = ctx->dense[slot];
+  SB_REQUIRE(ix.d > 0, SB_ERR_STATE, "sb_dense_delete: dense slot %d has no index loaded", slot);
+  std::vector<int64_t> del;
+  int rc = check_rows("sb_dense_delete", rows, n, ix.n, del);
+  if (rc) return rc;
+  *n_moved = 0;
+  if (n == 0) return SB_OK;
+  // the plan: the surviving rows of the tail [keep, n), ascending, fill the deleted rows below `keep`, ascending
+  const int64_t keep = ix.n - n;
+  const int64_t n_holes = std::lower_bound(del.begin(), del.end(), keep) - del.begin();
+  int64_t j = n_holes, src = keep, mv = 0;
+  for (int64_t i = 0; i < n_holes; ++i, ++src) {
+    while (j < n && del[j] == src) { ++j; ++src; }
+    moved_from[mv] = src;
+    moved_to[mv] = del[i];
+    ++mv;
   }
+  *n_moved = mv;
+  SB_CUDA(cudaDeviceSynchronize());   // searches enqueued on other streams may still read the rows that move
+  if (mv) {
+    if ((rc = ctx->misc2_dev.reserve((size_t)mv * 16))) return rc;
+    int64_t* f_dev = ctx->misc2_dev.as<int64_t>();
+    SB_CUDA(cudaMemcpyAsync(f_dev, moved_from, (size_t)mv * 8, cudaMemcpyHostToDevice, ctx->stream));
+    SB_CUDA(cudaMemcpyAsync(f_dev + mv, moved_to, (size_t)mv * 8, cudaMemcpyHostToDevice, ctx->stream));
+    MoveParams mp;
+    mp.rows = ix.rows;
+    mp.inv_norm = ix.inv_norm;
+    memcpy(mp.tags, ix.tags, sizeof(mp.tags));
+    mp.from = f_dev;
+    mp.to = f_dev + mv;
+    mp.n_moves = mv;
+    mp.ch = ix.d_pad / 8;
+    dense_move_rows_kernel<<<(unsigned)((mv + 7) / 8), 256, 0, ctx->stream>>>(mp);
+    SB_CUDA(cudaGetLastError());
+  }
+  // the vacated tail [keep, n) returns to the zero state of unused capacity
+  SB_CUDA(cudaMemsetAsync(ix.rows + (size_t)keep * ix.d_pad, 0, (size_t)n * ix.d_pad * sizeof(__half), ctx->stream));
+  SB_CUDA(cudaMemsetAsync(ix.inv_norm + keep, 0, (size_t)n * sizeof(float), ctx->stream));
+  for (int f = 0; f < SB_MAX_TAG_FIELDS; ++f)
+    if (ix.tags[f]) SB_CUDA(cudaMemsetAsync(ix.tags[f] + keep, 0xff, (size_t)n * 4, ctx->stream));
+  SB_CUDA(cudaStreamSynchronize(ctx->stream));
+  ix.n = keep;
+  ix.n_pad = round_rows(keep);
   return SB_OK;
 }
 
@@ -1439,7 +1682,10 @@ int sb_dense_tags_load(sb_ctx* ctx, int slot, int32_t field, const int32_t* code
   SB_CUDA(cudaStreamSynchronize(ctx->stream));
   if (ix.tags[field]) cudaFree(ix.tags[field]);
   ix.tags[field] = nullptr;
-  SB_CUDA(cudaMalloc(&ix.tags[field], (size_t)std::max<int64_t>(n, 1) * 4));
+  // a column spans the slot's capacity: -1 on the rows past n, so upserts and deletes never reallocate it alone
+  const int64_t cap = std::max<int64_t>(ix.n_cap, 1);
+  SB_CUDA(cudaMalloc(&ix.tags[field], (size_t)cap * 4));
+  SB_CUDA(cudaMemset(ix.tags[field], 0xff, (size_t)cap * 4));
   if (n) SB_CUDA(cudaMemcpy(ix.tags[field], codes, (size_t)n * 4, cudaMemcpyHostToDevice));
   return SB_OK;
 }

@@ -521,9 +521,10 @@ int dense_mma_topk_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int 
   float* thr = ctx->misc3_dev.as<float>();
   int32_t* counts = reinterpret_cast<int32_t*>(thr + (size_t)gsz * gmax);
   unsigned long long* cand = ctx->cand_dev.as<unsigned long long>();
-  if (ix.tm_rows_ptr != ix.rows) {  // (re)build the corpus tensor map once per loaded index
+  if (ix.tm_rows_ptr != ix.rows || ix.tm_n_pad != ix.n_pad) {  // (re)build the corpus map when rows or n_pad change
     if ((rc = encode_map(reinterpret_cast<CUtensorMap*>(ix.tm_rows), ix.rows, ix.n_pad, ix.d_pad, kTileRows))) return rc;
     ix.tm_rows_ptr = ix.rows;
+    ix.tm_n_pad = ix.n_pad;
   }
   const CUtensorMap& tm_rows = *reinterpret_cast<const CUtensorMap*>(ix.tm_rows);
   const size_t sel_smem = (size_t)kSelStage * 8 + (size_t)kSelTop * 20 + 64;

@@ -123,6 +123,44 @@ class B200Engine:
         c = np.ascontiguousarray(codes, dtype=np.int32).reshape(-1)
         check(self._lib.sb_dense_tags_load(self._h, slot, int(field), _ptr(c), len(c)), "sb_dense_tags_load")
 
+    # ------------------------------------------------------------------ K1d dense mutation (upsert / delete in place)
+    def dense_reserve(self, n_cap: int, slot: int = 0) -> None:
+        """Grow slot ``slot``'s row capacity to at least ``n_cap`` (never shrinks), so later appends do not reallocate."""
+        check(self._lib.sb_dense_reserve(self._h, slot, int(n_cap)), "sb_dense_reserve")
+
+    def dense_upsert(self, rows, vecs, slot: int = 0) -> None:
+        """Store ``vecs[i]`` at row ``rows[i]``: rows below the count overwrite, the others must be exactly count ..
+        count + m - 1 (appends, any order).  Loaded tag columns read -1 on the written rows until ``dense_tags_write``."""
+        r = np.ascontiguousarray(rows, dtype=np.int64).reshape(-1)
+        v = np.ascontiguousarray(vecs)
+        dt = 1 if v.dtype == np.float16 else 0
+        if dt == 0:
+            v = np.ascontiguousarray(v, dtype=np.float32)
+        if v.ndim != 2 or v.shape[0] != len(r) or v.shape[1] != self.dense_dim.get(slot):
+            raise ValueError(f"vecs must be [{len(r)}, {self.dense_dim.get(slot)}]")
+        check(self._lib.sb_dense_upsert(self._h, slot, _ptr(r), _ptr(v), len(r), dt), "sb_dense_upsert")
+        self.dense_count[slot] = int(self._lib.sb_dense_count(self._h, slot))
+
+    def dense_tags_write(self, field: int, rows, codes, slot: int = 0) -> None:
+        """``codes[i]`` -> tag column ``field`` at row ``rows[i]``."""
+        r = np.ascontiguousarray(rows, dtype=np.int64).reshape(-1)
+        c = np.ascontiguousarray(codes, dtype=np.int32).reshape(-1)
+        if len(r) != len(c):
+            raise ValueError("rows and codes must have the same length")
+        check(self._lib.sb_dense_tags_write(self._h, slot, int(field), _ptr(r), _ptr(c), len(r)), "sb_dense_tags_write")
+
+    def dense_delete(self, rows, slot: int = 0):
+        """Delete rows by swap-compaction; returns the moves (moved_from, moved_to) int64 arrays: the row that held
+        ``moved_from[i]`` is now row ``moved_to[i]`` (include/sentio_b200.h, sb_dense_delete)."""
+        r = np.ascontiguousarray(rows, dtype=np.int64).reshape(-1)
+        mf = np.empty(len(r), dtype=np.int64)
+        mt = np.empty(len(r), dtype=np.int64)
+        nm = C.c_int64(0)
+        check(self._lib.sb_dense_delete(self._h, slot, _ptr(r), len(r), _ptr(mf), _ptr(mt), C.byref(nm)),
+              "sb_dense_delete")
+        self.dense_count[slot] = int(self._lib.sb_dense_count(self._h, slot))
+        return mf[:nm.value].copy(), mt[:nm.value].copy()
+
     def fallback_count(self) -> int:
         """Queries answered by the brute-force fallback kernel since the engine was created (synchronises)."""
         v = int(self._lib.sb_dense_fallback_count(self._h))

@@ -91,10 +91,12 @@ def payload_value(payload, key: str):
     return cur
 
 
-def build_tag_column(payloads: Sequence[dict], key: str):
+def build_tag_column(payloads: Sequence[dict], key: str, known: dict | None = None):
     """(codes int32 [n], {value_key: code}) for one payload key; -1 where the key is absent (or null).  List- and
-    dict-valued fields raise: a multi-valued field cannot be one code per row."""
+    dict-valued fields raise: a multi-valued field cannot be one code per row.  With ``known`` (an existing table, left
+    unchanged), its codes are reused and only the values it lacks are returned, numbered after it."""
     codes = np.full(len(payloads), -1, dtype=np.int32)
+    base = known or {}
     table: dict = {}
     for i, p in enumerate(payloads):
         v = payload_value(p, key)
@@ -103,17 +105,43 @@ def build_tag_column(payloads: Sequence[dict], key: str):
         if isinstance(v, (list, tuple, dict, set)):
             raise ValueError(f"query_filter: payload key {key!r} holds a {type(v).__name__} on row {i}; "
                              "filters on list-valued or nested payload fields are not supported")
-        codes[i] = table.setdefault(value_key(v), len(table))
+        vk = value_key(v)
+        codes[i] = base[vk] if vk in base else table.setdefault(vk, len(base) + len(table))
     return codes, table
 
 
 class PayloadIndex:
-    """Per-collection payload index: tag columns built lazily, one per key, on the first filter that names the key."""
+    """Per-collection payload index: tag columns built lazily, one per key, on the first filter that names the key.
+    ``payloads`` is the collection's live list: keys indexed later are built from its current contents."""
 
-    def __init__(self, payloads: Sequence[dict], load_column):
+    def __init__(self, payloads: Sequence[dict], load_column, write_codes=None):
         self._payloads = payloads
         self._load = load_column          # load_column(field, codes)
+        self._write = write_codes         # write_codes(field, rows, codes): codes of some rows of a loaded column
         self.fields: dict[str, tuple[int, dict]] = {}
+
+    def encode(self, payloads: Sequence[dict]):
+        """Codes of new payloads for every indexed key, without changing the index: {key: (codes, new table entries)}.
+        Raises ``ValueError`` (list- or dict-valued field) before anything is modified."""
+        out = {}
+        for key, (_f, table) in self.fields.items():
+            codes, added = build_tag_column(payloads, key, table)
+            out[key] = (codes, added)
+        return out
+
+    def apply(self, rows, encoded) -> None:
+        """Commit ``encode``'s result for the payloads now stored at ``rows``: new values join their key's table and the
+        codes are written to the device column."""
+        rows = np.asarray(rows, dtype=np.int64)
+        for key, (codes, added) in encoded.items():
+            f, table = self.fields[key]
+            table.update(added)
+            if len(rows):
+                self._write(f, rows, codes)
+
+    def update(self, rows, payloads: Sequence[dict]) -> None:
+        """The payloads at ``rows`` changed: codes for every already-indexed key, new values added to its table."""
+        self.apply(rows, self.encode(payloads))
 
     def field(self, key: str):
         if key not in self.fields:

@@ -80,16 +80,20 @@ class _GpuEmbeddingScorer:
         self._vector_source = vector_source  # (B200VectorStore, collection_name) or None
         self._device = device
 
-    def _resolve(self, query: str, docs: list[Document]):
-        """-> (engine, query_vec, cand matrix or None, cand rows or None)."""
+    def _semantic_mmr(self, query: str, docs: list[Document], **kw):
+        """``semantic_mmr`` of the query against the docs: their stored rows when every doc id is in the vector source,
+        else their re-embedded texts."""
         q = np.asarray(self.embedder.embed_sync(query), dtype=np.float32)
         if self._vector_source is not None:
             store, collection = self._vector_source
-            rows = store.rows_of(collection, [d.id for d in docs])
-            if (rows >= 0).all():
-                return store.engine_of(collection), q, None, rows
+            # the id -> row lookup and the device call under one hold of the collection's lock: an upsert / delete in
+            # between moves rows, and a row looked up before it would score another point's vector
+            with store.locked(collection):
+                rows = store.rows_of(collection, [d.id for d in docs])
+                if (rows >= 0).all():
+                    return store.engine_of(collection).semantic_mmr(q, cand_ids=rows, **kw)
         cand = np.asarray(self.embedder.embed_many_sync([d.text for d in docs]), dtype=np.float32)
-        return (self._engine or _engine(self._device)), q, cand, None
+        return (self._engine or _engine(self._device)).semantic_mmr(q, cand=cand, **kw)
 
 
 class SemanticSimilarityScorer(_GpuEmbeddingScorer):
@@ -104,8 +108,7 @@ class SemanticSimilarityScorer(_GpuEmbeddingScorer):
         try:
             if not docs:
                 return []
-            eng, q, cand, rows = self._resolve(query, docs)
-            sem, _ = eng.semantic_mmr(q, cand=cand, cand_ids=rows, w_sem=self.weight, want_sem=True, want_mmr=False)
+            sem, _ = self._semantic_mmr(query, docs, w_sem=self.weight, want_sem=True, want_mmr=False)
             return [float(x) for x in sem]
         except Exception as exc:
             logger.warning("Error in semantic scoring: %s", exc)
@@ -127,9 +130,8 @@ class MMRScorer(_GpuEmbeddingScorer):
         if not docs:
             return []
         try:
-            eng, q, cand, rows = self._resolve(query, docs)
-            _, mmr = eng.semantic_mmr(q, cand=cand, cand_ids=rows, lambda_=self.lambda_, w_mmr=self.weight,
-                                      want_sem=False, want_mmr=True)
+            _, mmr = self._semantic_mmr(query, docs, lambda_=self.lambda_, w_mmr=self.weight, want_sem=False,
+                                        want_mmr=True)
             return [float(x) for x in mmr]
         except Exception as exc:
             logger.warning("MMR scorer failed: %s", exc)

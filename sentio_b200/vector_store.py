@@ -1,18 +1,26 @@
-"""B200VectorStore -- an HBM-resident stand-in for the slice of ``qdrant_client.QdrantClient`` the hot path uses.
+"""B200VectorStore -- an HBM-resident stand-in for the slice of ``qdrant_client.QdrantClient`` the reference uses.
 
 The reference's dense path is ``client.search(collection_name=, query_vector=, limit=, with_payload=True)``
 (src/core/retrievers/dense.py:46-64), its cache probe ``client.collection_exists(collection_name=)``
 (src/core/retrievers/hybrid.py:101-105) and its BM25 corpus load ``client.scroll(...)``
-(src/core/retrievers/factory.py:95-101).  This class answers exactly those calls from a ``B200Engine``: vectors live in
-HBM as fp16 rows (one engine per collection), payloads / ids stay on the host.  Because it is call-compatible, the
-reference's OWN ``DenseRetriever`` runs unchanged on top of it (INTEGRATION.md), and so does ours.
+(src/core/retrievers/factory.py:95-101).  Its store writes with ``client.upsert`` / ``client.delete`` and bootstraps and
+inspects collections with ``create_collection(vectors_config=)`` / ``get_collection`` / ``get_collections``
+(src/core/vector_store/qdrant_store.py:196-263, 298-349).  This class answers exactly those calls from a ``B200Engine``:
+vectors live in HBM as fp16 rows (one engine per collection), payloads / ids stay on the host.  Because it is
+call-compatible, the reference's OWN ``DenseRetriever`` runs unchanged on top of it (INTEGRATION.md), and so does ours.
 
 Payload / id schema follows what the reference's ingest writes: ``payload = {"content": text, "metadata": {...}}``,
 point id = string (src/core/vector_store/qdrant_store.py:333-340).
+
+Threads: searches may come from a thread pool (the reference's ``retrieve_async``).  Every search (device call plus
+its row -> id mapping) and every mutation holds the collection's lock, so a search never maps rows through a
+half-updated id / payload mirror.
 """
 from __future__ import annotations
 
-from dataclasses import dataclass
+import enum
+import threading
+from dataclasses import dataclass, field
 from typing import Any, Sequence
 
 import numpy as np
@@ -20,7 +28,7 @@ import numpy as np
 from .engine import B200Engine
 from .payload_filter import PayloadIndex
 
-__all__ = ["B200VectorStore", "ScoredPoint", "Record"]
+__all__ = ["B200VectorStore", "ScoredPoint", "Record", "UpdateResult", "CollectionInfo", "Distance"]
 
 
 @dataclass
@@ -39,6 +47,52 @@ class Record:
     vector: Any = None
 
 
+@dataclass
+class UpdateResult:
+    status: str = "completed"
+
+
+class Distance(enum.Enum):
+    COSINE = "Cosine"
+
+
+@dataclass
+class VectorParams:
+    size: int
+    distance: Distance = Distance.COSINE
+
+
+@dataclass
+class CollectionParams:
+    vectors: VectorParams
+
+
+@dataclass
+class CollectionConfig:
+    params: CollectionParams
+
+
+@dataclass
+class CollectionInfo:
+    points_count: int
+    config: CollectionConfig
+    status: str = "green"
+
+
+@dataclass
+class CollectionDescription:
+    name: str
+
+
+@dataclass
+class CollectionsResponse:
+    collections: list = field(default_factory=list)
+
+
+def _distance_name(dist) -> str:
+    return str(getattr(dist, "name", dist))
+
+
 class _Collection:
     def __init__(self, name: str, device: int):
         self.name = name
@@ -47,14 +101,37 @@ class _Collection:
         self.payloads: list[dict] = []
         self.row_of: dict[Any, int] = {}
         self.dim = 0
+        self.lock = threading.RLock()
         self._payload_index: PayloadIndex | None = None
 
     def payload_index(self) -> PayloadIndex:
         # built lazily: a tag column per payload key, on the first filter that names the key
         if self._payload_index is None:
             self._payload_index = PayloadIndex(self.payloads,
-                                               lambda f, codes: self.engine.load_dense_tags(f, codes, slot=0))
+                                               lambda f, codes: self.engine.load_dense_tags(f, codes, slot=0),
+                                               lambda f, rows, codes: self.engine.dense_tags_write(f, rows, codes, slot=0))
         return self._payload_index
+
+
+def _points_columns(points):
+    """(ids, vectors, payloads) of a list of ``PointStruct``-shaped objects or a ``Batch``-shaped object."""
+    if hasattr(points, "ids") and hasattr(points, "vectors"):
+        ids, vecs = list(points.ids), points.vectors
+        pls = getattr(points, "payloads", None)
+        pls = [None] * len(ids) if pls is None else list(pls)
+        if isinstance(vecs, dict):
+            raise ValueError("upsert: named vectors are not supported (one unnamed vector per point)")
+        vecs = list(vecs)
+    else:
+        pts = list(points)
+        ids = [p.id for p in pts]
+        vecs = [p.vector for p in pts]
+        pls = [getattr(p, "payload", None) for p in pts]
+    if len(vecs) != len(ids) or len(pls) != len(ids):
+        raise ValueError("upsert: ids, vectors and payloads must have the same length")
+    if any(isinstance(v, dict) for v in vecs):
+        raise ValueError("upsert: named vectors are not supported (one unnamed vector per point)")
+    return ids, vecs, pls
 
 
 class B200VectorStore:
@@ -66,9 +143,22 @@ class B200VectorStore:
     def collection_exists(self, collection_name: str) -> bool:
         return collection_name in self._collections
 
-    def create_collection(self, collection_name: str, vectors: np.ndarray, ids: Sequence[Any] | None = None,
-                          payloads: Sequence[dict] | None = None) -> None:
-        """Upload a whole collection (brute-force search needs no incremental index)."""
+    def create_collection(self, collection_name: str, vectors: np.ndarray | None = None,
+                          ids: Sequence[Any] | None = None, payloads: Sequence[dict] | None = None,
+                          vectors_config=None, **_ignored) -> None:
+        """Upload a whole collection (brute-force search needs no incremental index), or, with Qdrant's
+        ``vectors_config=VectorParams(size, distance)`` and no vectors, create an empty one that ``upsert`` fills.
+        Only the Cosine distance exists here; any other raises ``ValueError``."""
+        if vectors_config is not None:
+            if isinstance(vectors_config, dict):
+                raise ValueError("create_collection: named vectors are not supported (one unnamed vector per point)")
+            dist = _distance_name(getattr(vectors_config, "distance", "Cosine"))
+            if dist.lower() != "cosine":
+                raise ValueError(f"create_collection: distance {dist} is not supported (only Cosine)")
+        if vectors is None:
+            if vectors_config is None:
+                raise ValueError("create_collection: give vectors or vectors_config")
+            vectors = np.zeros((0, int(vectors_config.size)), dtype=np.float32)
         vecs = np.asarray(vectors)
         n = vecs.shape[0]
         col = _Collection(collection_name, self._device)
@@ -89,15 +179,125 @@ class B200VectorStore:
         if col is not None:
             col.engine.close()
 
+    def get_collection(self, collection_name: str) -> CollectionInfo:
+        col = self._get(collection_name)
+        with col.lock:
+            return CollectionInfo(points_count=len(col.ids),
+                                  config=CollectionConfig(CollectionParams(VectorParams(col.dim, Distance.COSINE))))
+
+    def get_collections(self) -> CollectionsResponse:
+        return CollectionsResponse([CollectionDescription(name) for name in list(self._collections)])
+
     def engine_of(self, collection_name: str) -> B200Engine:
         return self._collections[collection_name].engine
 
+    def locked(self, collection_name: str):
+        """The collection's lock (reentrant), for a caller that maps ids to rows (``rows_of``) and then reads those rows
+        on the device: held across both, no upsert / delete can move the rows in between."""
+        return self._get(collection_name).lock
+
     def rows_of(self, collection_name: str, ids: Sequence[Any]) -> np.ndarray:
         col = self._collections[collection_name]
-        return np.asarray([col.row_of.get(i, -1) for i in ids], dtype=np.int64)
+        with col.lock:
+            return np.asarray([col.row_of.get(i, -1) for i in ids], dtype=np.int64)
 
     def count(self, collection_name: str) -> int:
         return len(self._collections[collection_name].ids)
+
+    def _get(self, collection_name: str) -> _Collection:
+        col = self._collections.get(collection_name)
+        if col is None:
+            raise ValueError(f"Collection {collection_name} not found")
+        return col
+
+    # ------------------------------------------------------------------ writes
+    def upsert(self, collection_name: str, points, wait: bool = True, **_ignored) -> UpdateResult:
+        """Qdrant ``upsert``: ``points`` is a list of ``PointStruct``-shaped objects (``.id`` / ``.vector`` /
+        ``.payload``) or a ``Batch`` (``.ids`` / ``.vectors`` / ``.payloads``).  An existing id overwrites its row
+        (vector and payload), a new id appends; within one call the last occurrence of an id wins.  Everything is
+        validated before the device is touched, so a ``ValueError`` leaves the collection unchanged.  Always
+        synchronous (``wait`` is accepted and ignored)."""
+        col = self._get(collection_name)
+        ids, vecs, pls = _points_columns(points)
+        last = {}
+        for i, pid in enumerate(ids):   # first-appearance order, last occurrence's values
+            last[pid] = i
+        pick = list(last.values())
+        uids = list(last)
+        if not uids:
+            return UpdateResult(status="completed")
+        try:
+            v = np.asarray([vecs[i] for i in pick], dtype=np.float32)
+        except (TypeError, ValueError) as e:
+            raise ValueError(f"upsert: vectors must be equal-length numeric sequences ({e})") from None
+        if v.ndim != 2 or v.shape[1] != col.dim:
+            raise ValueError(f"upsert: vectors must have dimension {col.dim}, got shape {v.shape}")
+        if not np.isfinite(v).all():
+            raise ValueError("upsert: vectors contain NaN or infinite values")
+        new_payloads = []
+        for i in pick:
+            p = pls[i]
+            if p is not None and not isinstance(p, dict):
+                raise ValueError(f"upsert: payload must be a dict, got {type(p).__name__}")
+            new_payloads.append(dict(p) if p is not None else {})
+        with col.lock:
+            pi = col._payload_index
+            encoded = pi.encode(new_payloads) if pi is not None else None
+            n0 = len(col.ids)
+            rows, appended = [], 0
+            for pid in uids:
+                r = col.row_of.get(pid)
+                if r is None:
+                    r = n0 + appended
+                    appended += 1
+                rows.append(r)
+            rows = np.asarray(rows, dtype=np.int64)
+            col.engine.dense_upsert(rows, v, slot=0)
+            col.ids.extend([None] * appended)
+            col.payloads.extend([None] * appended)
+            for pid, r, p in zip(uids, rows.tolist(), new_payloads):
+                col.ids[r] = pid
+                col.payloads[r] = p
+                col.row_of[pid] = r
+            if pi is not None:
+                pi.apply(rows, encoded)
+        return UpdateResult(status="completed")
+
+    def delete(self, collection_name: str, points_selector, wait: bool = True, **_ignored) -> UpdateResult:
+        """Qdrant ``delete`` by ids: ``points_selector`` is a ``PointIdsList``-shaped object (``.points``) or a plain
+        list of ids.  Unknown ids are ignored.  Deleting by filter (``FilterSelector``) raises ``ValueError``."""
+        col = self._get(collection_name)
+        if hasattr(points_selector, "points"):
+            ids = list(points_selector.points)
+        elif isinstance(points_selector, (list, tuple)):
+            ids = list(points_selector)
+        else:   # FilterSelector, a bare Filter, or anything else: never read as a list of ids
+            raise ValueError(f"delete: points_selector of type {type(points_selector).__name__} is not supported; "
+                             "give PointIdsList(points=[...]) or a list of ids (deleting by filter is not supported)")
+        with col.lock:
+            rows = sorted({col.row_of[i] for i in ids if i in col.row_of})
+            if rows:
+                moved_from, moved_to = col.engine.dense_delete(rows, slot=0)
+                for r in rows:
+                    del col.row_of[col.ids[r]]
+                for f, t in zip(moved_from.tolist(), moved_to.tolist()):
+                    col.ids[t] = col.ids[f]
+                    col.payloads[t] = col.payloads[f]
+                    col.row_of[col.ids[t]] = t
+                keep = len(col.ids) - len(rows)
+                del col.ids[keep:]
+                del col.payloads[keep:]   # in place: the payload index reads this list
+        return UpdateResult(status="completed")
+
+    def retrieve(self, collection_name: str, ids: Sequence[Any], with_payload: bool = True, with_vectors: bool = False,
+                 **_ignored) -> list[Record]:
+        """Points by id (unknown ids are skipped, as in Qdrant); vectors are the stored fp16 values, widened."""
+        col = self._get(collection_name)
+        with col.lock:
+            rows = [col.row_of[i] for i in ids if i in col.row_of]
+            vecs = col.engine.dense_fetch(rows, slot=0) if with_vectors and rows else None
+            return [Record(id=col.ids[r], payload=col.payloads[r] if with_payload else None,
+                           vector=vecs[j].tolist() if vecs is not None else None) for j, r in enumerate(rows)]
 
     # ------------------------------------------------------------------ the calls the hot path makes
     def search(self, collection_name: str, query_vector, limit: int = 10, with_payload: bool = True,
@@ -105,47 +305,45 @@ class B200VectorStore:
         """``query_filter``: a Qdrant ``Filter(must=[FieldCondition(key, match=MatchValue(value))...])`` or a bare
         ``FieldCondition`` (what the reference's ``_convert_filter`` emits): the exact top-``limit`` of the points whose
         payload satisfies every condition.  Other filter shapes raise ``ValueError`` (sentio_b200/payload_filter.py)."""
-        col = self._collections.get(collection_name)
-        if col is None:
-            raise ValueError(f"Collection {collection_name} not found")
+        col = self._get(collection_name)
         if isinstance(query_vector, tuple):  # ("name", vector) form of the named-vector API
             query_vector = query_vector[1]
         q = np.asarray(query_vector, dtype=np.float32).reshape(1, -1)
-        limit = max(1, min(int(limit), max(len(col.ids), 1)))   # Qdrant never returns more points than the collection holds
-        filters = self._compile_filters(col, [query_filter]) if query_filter is not None else None
-        ids, scores, counts = col.engine.dense_topk(q, int(limit), filters=filters) if filters is not None \
-            else col.engine.dense_topk(q, int(limit))
-        out = []
-        for j in range(int(counts[0])):
-            row = int(ids[0, j])
-            out.append(ScoredPoint(id=col.ids[row], score=float(scores[0, j]),
-                                   payload=col.payloads[row] if with_payload else None))
-        return out
+        with col.lock:
+            limit = max(1, min(int(limit), max(len(col.ids), 1)))   # Qdrant never returns more points than it holds
+            filters = self._compile_filters(col, [query_filter]) if query_filter is not None else None
+            ids, scores, counts = col.engine.dense_topk(q, int(limit), filters=filters) if filters is not None \
+                else col.engine.dense_topk(q, int(limit))
+            out = []
+            for j in range(int(counts[0])):
+                row = int(ids[0, j])
+                out.append(ScoredPoint(id=col.ids[row], score=float(scores[0, j]),
+                                       payload=col.payloads[row] if with_payload else None))
+            return out
 
     def search_batch(self, collection_name: str, query_vectors, limit: int = 10, with_payload: bool = True,
                      query_filter=None, **_ignored) -> list[list[ScoredPoint]]:
         """``search`` for many query vectors in ONE device batch (the wgmma scan serves 256 queries per HBM pass).
         ``query_filter``: one filter for the whole batch, or a list / tuple with one filter (or None) per query."""
-        col = self._collections.get(collection_name)
-        if col is None:
-            raise ValueError(f"Collection {collection_name} not found")
+        col = self._get(collection_name)
         q = np.asarray(query_vectors, dtype=np.float32)
         if q.ndim != 2:
             raise ValueError("query_vectors must be [B, d]")
         if q.shape[0] == 0:
             return []
-        filters = None
-        if query_filter is not None:
-            per_query = list(query_filter) if isinstance(query_filter, (list, tuple)) else [query_filter] * q.shape[0]
-            if len(per_query) != q.shape[0]:
-                raise ValueError(f"query_filter: {len(per_query)} filters for {q.shape[0]} queries")
-            if any(f is not None for f in per_query):
-                filters = self._compile_filters(col, per_query)
-        ids, scores, counts = col.engine.dense_topk(q, int(limit), filters=filters) if filters is not None \
-            else col.engine.dense_topk(q, int(limit))
-        return [[ScoredPoint(id=col.ids[int(ids[b, j])], score=float(scores[b, j]),
-                             payload=col.payloads[int(ids[b, j])] if with_payload else None)
-                 for j in range(int(counts[b]))] for b in range(q.shape[0])]
+        with col.lock:
+            filters = None
+            if query_filter is not None:
+                per_query = list(query_filter) if isinstance(query_filter, (list, tuple)) else [query_filter] * q.shape[0]
+                if len(per_query) != q.shape[0]:
+                    raise ValueError(f"query_filter: {len(per_query)} filters for {q.shape[0]} queries")
+                if any(f is not None for f in per_query):
+                    filters = self._compile_filters(col, per_query)
+            ids, scores, counts = col.engine.dense_topk(q, int(limit), filters=filters) if filters is not None \
+                else col.engine.dense_topk(q, int(limit))
+            return [[ScoredPoint(id=col.ids[int(ids[b, j])], score=float(scores[b, j]),
+                                 payload=col.payloads[int(ids[b, j])] if with_payload else None)
+                     for j in range(int(counts[b]))] for b in range(q.shape[0])]
 
     @staticmethod
     def _compile_filters(col: _Collection, filters):
@@ -156,17 +354,17 @@ class B200VectorStore:
     def search_batch_arrays(self, collection_name: str, query_vectors: np.ndarray, limit: int):
         """Batched extension: (rows [B,k] int64, scores [B,k] float64, counts [B]) without Python objects."""
         col = self._collections[collection_name]
-        return col.engine.dense_topk(np.asarray(query_vectors, dtype=np.float32), int(limit))
+        with col.lock:
+            return col.engine.dense_topk(np.asarray(query_vectors, dtype=np.float32), int(limit))
 
     def scroll(self, collection_name: str, limit: int = 100, offset: int | None = None, with_payload: bool = True,
                with_vectors: bool = False, **_ignored):
-        col = self._collections.get(collection_name)
-        if col is None:
-            raise ValueError(f"Collection {collection_name} not found")
-        start = int(offset or 0)
-        stop = min(len(col.ids), start + int(limit))
-        recs = [Record(id=col.ids[i], payload=col.payloads[i] if with_payload else None) for i in range(start, stop)]
-        return recs, (stop if stop < len(col.ids) else None)
+        col = self._get(collection_name)
+        with col.lock:
+            start = int(offset or 0)
+            stop = min(len(col.ids), start + int(limit))
+            recs = [Record(id=col.ids[i], payload=col.payloads[i] if with_payload else None) for i in range(start, stop)]
+            return recs, (stop if stop < len(col.ids) else None)
 
     def close(self) -> None:
         for col in self._collections.values():
