@@ -96,6 +96,25 @@ int sb_profile_read(sb_ctx* ctx, int kernel_id, int64_t* n_out, double* ms_out);
 #define SB_MAX_DENSE_SLOTS 2
 int sb_dense_load(sb_ctx* ctx, int slot, const void* vecs, int64_t n, int32_t d, int32_t dtype, int64_t id_base);
 /*
+ * Distance metric of a slot -- Qdrant's `Distance` of the collection (reference QdrantStore.distance,
+ * src/core/vector_store/qdrant_store.py:52; create_collection passes rest.Distance[distance.upper()], :224-237).
+ * sb_dense_load_metric: sb_dense_load with a metric; sb_dense_load means SB_METRIC_COSINE.  Every metric stores the same
+ * fp16 row y = fp16(x / ||x||) (SB_F16 input is normalised too, except for Cosine, which stores it verbatim as before);
+ * Dot and Euclid add one fp64 factor per row, c = ||x|| / ||y||, and the stored vector is v = c * y.  v equals the
+ * input only to the fp16 precision of its direction (Qdrant keeps the input itself).  Rows whose fp64 norm is not finite,
+ * and for Euclid rows whose squared norm is not finite in fp32, are rejected (SB_ERR_ARG) before anything changes; the
+ * same holds for sb_dense_upsert on a Dot / Euclid slot.  Upsert, delete, tags and every top-k entry point follow the
+ * slot's metric.  sb_dense_fetch returns c * y for Dot / Euclid.  Metrics other than these three (Manhattan) are not
+ * supported: an L1 distance is not a GEMM.
+ * sb_dense_metric: the slot's metric, -1 for a bad slot.
+ */
+#define SB_METRIC_COSINE 0
+#define SB_METRIC_DOT 1
+#define SB_METRIC_EUCLID 2
+int sb_dense_load_metric(sb_ctx* ctx, int slot, const void* vecs, int64_t n, int32_t d, int32_t dtype, int64_t id_base,
+                         int32_t metric);
+int32_t sb_dense_metric(sb_ctx* ctx, int slot);
+/*
  * Scan selection: 0 = auto (batches of >= 16 queries use the wgmma batched-query scan, smaller ones the CUDA-core
  * scan), 1 = CUDA-core scan only, 2 = wgmma scan whenever eligible.  Results are identical in every mode.
  */
@@ -104,7 +123,12 @@ int64_t sb_dense_count(sb_ctx* ctx, int slot);
 int32_t sb_dense_dim(sb_ctx* ctx, int slot);
 /*
  * sb_dense_topk: B queries (row-major B x d fp32, need not be normalised: any scale), best-first top-k per query, k <= 1024:
- * out_ids[B*k], out_scores[B*k] (exact fp64 cosine, ties broken by ascending id), out_counts[B] (= min(k, n)).
+ * out_ids[B*k], out_scores[B*k], out_counts[B] (= min(k, n)).  out_scores per the slot's metric (Qdrant's semantics,
+ * reference qdrant_store.py:52, 224-237):
+ *   SB_METRIC_COSINE  exact fp64 cosine, score descending;
+ *   SB_METRIC_DOT     exact fp64 <q, v> with q as given (not normalised), score descending;
+ *   SB_METRIC_EUCLID  exact fp64 ||q - v|| (the distance, not its square), distance ASCENDING;
+ * ties broken by ascending id in every case.
  * The result is the EXACT top-k of the stored rows for every input: the scans rank by an approximate cosine with a per-query
  * error bound eps, every row within 2 eps of the k-th best approximate score is re-scored in fp64, and a query whose window
  * cannot be served that way is answered by a brute-force fp64 kernel (DESIGN.md K1 "Exactness").  Page-locked q / out_*
@@ -130,7 +154,7 @@ int sb_dense_fetch(sb_ctx* ctx, int slot, const int64_t* ids, int32_t n_ids, flo
  * tags[f_field[i]][row] == f_code[i] for every i.  f_code < 0 matches nothing; a query without conditions is
  * unfiltered.  Every field named must have been loaded.  Results: the EXACT top-k of the matching rows, same order and
  * scores as sb_dense_topk, out_counts[b] = min(k, matching rows); an all-zero query gives the first k matching rows
- * with score 0.  A query with at most 2048 matching rows skips the scans (exact fp64 over its matching rows); the others
+ * with score 0 (Cosine / Dot; under Euclid it gives the matching rows nearest the origin).  A query with at most 2048 matching rows skips the scans (exact fp64 over its matching rows); the others
  * are scanned with the match mask applied inside the scan (DESIGN.md K1c).
  * sb_dense_topk_filtered_dev: the same on device buffers (q_dev, f_off_dev[B+1], f_field_dev / f_code_dev[n_conds]).
  * Unlike the other `_dev` entry points it waits on `stream` twice: once to read the conditions, once to read the

@@ -40,6 +40,9 @@ SIGNATURES = {
     "sb_profile": (C.c_int, [C.c_void_p, C.c_int]),
     "sb_profile_read": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_double)]),
     "sb_dense_load": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_int64]),
+    "sb_dense_load_metric": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_int64,
+                                       C.c_int32]),
+    "sb_dense_metric": (C.c_int32, [C.c_void_p, C.c_int]),
     "sb_dense_set_mode": (C.c_int, [C.c_void_p, C.c_int]),
     "sb_dense_count": (C.c_int64, [C.c_void_p, C.c_int]),
     "sb_dense_dim": (C.c_int32, [C.c_void_p, C.c_int]),
@@ -144,7 +147,12 @@ def load_library(path: os.PathLike | None = None) -> C.CDLL:
     return lib
 
 
+class SentioB200ArgError(SentioB200Error, ValueError):
+    """SB_ERR_ARG: the call rejected its input (and changed nothing)."""
+
+
 def check(rc: int, what: str) -> None:
     if rc != 0:
         msg = load_library().sb_last_error()
-        raise SentioB200Error(f"{what} failed (rc={rc}): {msg.decode('utf-8', 'replace') if msg else '?'}")
+        cls = SentioB200ArgError if rc == -2 else SentioB200Error
+        raise cls(f"{what} failed (rc={rc}): {msg.decode('utf-8', 'replace') if msg else '?'}")

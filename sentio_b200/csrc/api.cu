@@ -65,6 +65,8 @@ void sb_destroy(sb_ctx* ctx) {
   for (int s = 0; s < SB_MAX_DENSE_SLOTS; ++s) {
     if (ctx->dense[s].rows) cudaFree(ctx->dense[s].rows);
     if (ctx->dense[s].inv_norm) cudaFree(ctx->dense[s].inv_norm);
+    if (ctx->dense[s].cfac) cudaFree(ctx->dense[s].cfac);
+    if (ctx->dense[s].hh) cudaFree(ctx->dense[s].hh);
     for (int f = 0; f < SB_MAX_TAG_FIELDS; ++f)
       if (ctx->dense[s].tags[f]) cudaFree(ctx->dense[s].tags[f]);
   }

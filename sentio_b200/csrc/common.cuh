@@ -93,8 +93,16 @@ struct DenseIndex {
   int32_t d = 0;        // logical dimension
   int32_t d_pad = 0;    // stored row length in halves (multiple of 8 -> 16 B aligned rows)
   int64_t id_base = 0;
-  __half* rows = nullptr;    // [n_cap][d_pad]
-  float* inv_norm = nullptr; // [n_cap], 1/||row|| of the STORED fp16 row (0 for zero rows)
+  int32_t metric = SB_METRIC_COSINE;
+  __half* rows = nullptr;    // [n_cap][d_pad] y = fp16(x / ||x||) (Cosine: also fp16 input verbatim)
+  // per-row scan scale, what the scans multiply their fp32 dot product by: Cosine 1/||y|| of the STORED fp16 row (0 for
+  // zero rows); Dot / Euclid (float)c
+  float* inv_norm = nullptr; // [n_cap]
+  // Dot / Euclid (DESIGN.md K1e): the stored vector is v = c * y with c = ||x|| / ||y|| (fp64, 0 for zero rows)
+  double* cfac = nullptr;    // [n_cap], nullptr for Cosine
+  float* hh = nullptr;       // [n_cap] Euclid only: h >= ||v||^2 / 2 rounded up to fp32
+  double rho_max = 0.0;      // >= max ||v|| over every row ever stored since the load (an upsert may raise it)
+  double h_max = 0.0;        // Euclid: >= max h, likewise
   // cached CUtensorMap (128 bytes, 64-byte aligned) over rows[0, n_pad) for the wgmma batched scan; valid iff
   // tm_rows_ptr == rows and tm_n_pad == n_pad (an append within capacity keeps `rows` but widens n_pad)
   alignas(64) unsigned char tm_rows[128] = {0};

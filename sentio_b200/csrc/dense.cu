@@ -15,9 +15,11 @@
 //                       lists raise a flag and are answered by dense_exact_fallback_kernel (brute force, fp64).
 //
 // Algorithmic HBM bytes per pass = n_pad * d_pad * 2 (+ n_pad * 4 for the inverse norms); see DESIGN.md.
+#include <float.h>
 #include <math.h>
 #include <string.h>
 #include <algorithm>
+#include <cmath>
 
 #include "dense_common.cuh"
 #include "dense_mma.cuh"
@@ -34,10 +36,13 @@ constexpr int kRowPad = 128;  // n_pad granularity (tile rows of the wgmma scan;
 // One warp per row.  f32 input: x16 = fp16(x / ||x||) (division in fp64, single rounding); f16 input: verbatim.
 // inv_norm = 1/||x16|| of the stored values (fp64 accumulate), 0 for all-zero rows.  Input row r goes to row row0 + r,
 // or to dst_rows[r] when a destination list is given (sb_dense_upsert).
+// Dot / Euclid (cfac != nullptr, always normalised): cfac = c = ||x|| / ||x16|| in fp64 (0 for a zero row), the scan
+// scale inv_norm = (float)c, and for Euclid hh = ||v||^2 / 2 = c^2 ||x16||^2 / 2 rounded UP to fp32.
 template <typename TIn>
 __global__ void dense_store_rows_kernel(const TIn* __restrict__ in, int64_t n_rows, int32_t d, int32_t d_pad,
                                         __half* __restrict__ rows, float* __restrict__ inv_norm, int64_t row0,
-                                        const int64_t* __restrict__ dst_rows, bool normalise) {
+                                        const int64_t* __restrict__ dst_rows, bool normalise,
+                                        double* __restrict__ cfac, float* __restrict__ hh) {
   int64_t r = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   int lane = threadIdx.x & 31;
   if (r >= n_rows) return;
@@ -66,7 +71,15 @@ __global__ void dense_store_rows_kernel(const TIn* __restrict__ in, int64_t n_ro
     ss16 += hv * hv;
   }
   for (int o = 16; o; o >>= 1) ss16 += __shfl_xor_sync(0xffffffffu, ss16, o);
-  if (lane == 0) inv_norm[out_row] = ss16 > 0.0 ? (float)(1.0 / sqrt(ss16)) : 0.f;
+  if (lane != 0) return;
+  if (cfac == nullptr) {
+    inv_norm[out_row] = ss16 > 0.0 ? (float)(1.0 / sqrt(ss16)) : 0.f;
+    return;
+  }
+  const double c = ss16 > 0.0 ? scale / sqrt(ss16) : 0.0;
+  cfac[out_row] = c;
+  inv_norm[out_row] = (float)c;
+  if (hh) hh[out_row] = __double2float_ru(0.5 * (c * c) * ss16);
 }
 
 // ------------------------------------------------------------------------------------------------ mutation kernels
@@ -75,6 +88,8 @@ __global__ void dense_store_rows_kernel(const TIn* __restrict__ in, int64_t n_ro
 struct MoveParams {
   __half* rows;
   float* inv_norm;
+  double* cfac;                       // Dot / Euclid, else nullptr
+  float* hh;                          // Euclid, else nullptr
   int32_t* tags[SB_MAX_TAG_FIELDS];   // nullptr = field not loaded
   const int64_t* from;
   const int64_t* to;
@@ -90,7 +105,11 @@ __global__ void __launch_bounds__(256) dense_move_rows_kernel(const MoveParams p
   const uint4* src = reinterpret_cast<const uint4*>(p.rows) + s * p.ch;
   uint4* dst = reinterpret_cast<uint4*>(p.rows) + t * p.ch;
   for (int c = lane; c < p.ch; c += 32) dst[c] = src[c];
-  if (lane == 0) p.inv_norm[t] = p.inv_norm[s];
+  if (lane == 0) {
+    p.inv_norm[t] = p.inv_norm[s];
+    if (p.cfac) p.cfac[t] = p.cfac[s];
+    if (p.hh) p.hh[t] = p.hh[s];
+  }
 #pragma unroll
   for (int f = 0; f < SB_MAX_TAG_FIELDS; ++f)
     if (lane == f + 1 && p.tags[f] != nullptr) p.tags[f][t] = p.tags[f][s];
@@ -123,6 +142,9 @@ struct ScanParams {
   const uint32_t* mask;
   int32_t mask_qs;
   const int32_t* state;
+  // EUCLID only: per-row h (>= ||v||^2 / 2) and per-query r = (float)||q|| of this pass's queries
+  const float* hh;
+  const float* rq;
 };
 
 // Sum V per-lane partials across the warp: afterwards the lanes with (lane % (32/V)) == 0 hold value index lane/(32/V).
@@ -263,7 +285,9 @@ __device__ __forceinline__ unsigned long long h2_to_f2(uint32_t h2) {
   return pack_f2(f.x, f.y);
 }
 
-template <int NCHUNK, int QB, int RW, bool EXACT, bool FILTER>
+// Key of a row: Cosine / Dot  acc * scale[row];  EUCLID  r * (acc * scale[row]) - h[row] = (||q||^2 - ||q - v||^2) / 2
+// up to the error bound of DESIGN.md K1e (larger = nearer).
+template <int NCHUNK, int QB, int RW, bool EXACT, bool FILTER, bool EUCLID>
 __global__ void __launch_bounds__(kScanThreads, 1) dense_scan_kernel(const ScanParams p) {
   constexpr int R = kConsumerWarps * RW;  // rows per tile
   constexpr int V = RW * QB;              // partial sums per lane
@@ -395,6 +419,8 @@ __global__ void __launch_bounds__(kScanThreads, 1) dense_scan_kernel(const ScanP
   const int ri = vi / QB, qi = vi % QB;
   const bool leader = (lane % LPV) == 0;
   const int trigger = p.bcap - R;  // a batch is handed over while it still has room for one more tile
+  float rq = 0.f;
+  if constexpr (EUCLID) rq = __ldg(p.rq + qi);
 
   for (int i = 0; i < my_tiles; ++i) {
     const int s = i % stages;
@@ -404,6 +430,9 @@ __global__ void __launch_bounds__(kScanThreads, 1) dense_scan_kernel(const ScanP
     mbar_wait(bar_full0 + 8 * s, use & 1u);
     float invn = 0.f;
     if (leader) invn = __ldg(p.inv_norm + grow);  // consumed after the reduction: latency hides under the FMAs
+    float hrow = 0.f;
+    if constexpr (EUCLID)
+      if (leader) hrow = __ldg(p.hh + grow);
     uint32_t mword = 0u;
     if constexpr (FILTER)
       if (leader) mword = __ldg(p.mask + (size_t)(grow >> 5) * p.mask_qs + qi);
@@ -448,7 +477,8 @@ __global__ void __launch_bounds__(kScanThreads, 1) dense_scan_kernel(const ScanP
       part[v] = __uint_as_float((uint32_t)(acc[v] & 0xffffffffull)) + __uint_as_float((uint32_t)(acc[v] >> 32));
     const float dot = warp_reduce_multi<V>(part, lane);
     if (leader) {
-      const float score = dot * invn;
+      float score = dot * invn;
+      if constexpr (EUCLID) score = __fsub_rn(__fmul_rn(rq, score), hrow);
       bool match = true;
       if constexpr (FILTER) match = (mword >> (grow & 31)) & 1u;
       if (grow < p.n && score > thr[qi] && match) {
@@ -511,6 +541,8 @@ struct MergeParams {
   double* out_scores;        // [nq][k]
   int32_t* out_counts;       // [nq]
   const int32_t* state;      // FILTER only: [nq] 1 = answered by the gather path (nothing to merge)
+  int32_t metric;
+  const double* cfac;
 };
 
 __device__ __forceinline__ void block_sort_desc_u64(unsigned long long* a, int len, int tid, int nt) {
@@ -606,6 +638,8 @@ __global__ void __launch_bounds__(kMergeThreads, 1) dense_merge_kernel(const Mer
   ra.out_ids = p.out_ids + (size_t)qi * p.k;
   ra.out_scores = p.out_scores + (size_t)qi * p.k;
   ra.out_count = p.out_counts + qi;
+  ra.metric = p.metric;
+  ra.cfac = p.cfac;
   rescore_and_emit(sel, nsel, P, ek, ei, &qq_s, q_s, ra);
 }
 
@@ -613,9 +647,19 @@ __global__ void __launch_bounds__(kMergeThreads, 1) dense_merge_kernel(const Mer
 // One CTA per operand row r (rows >= nq are padding): qn[r] = q[r] / ||q[r]|| in fp32 (the scans rank by cosine, so the
 // caller's scale must not reach the fp32 / fp16 arithmetic), optionally q16[r] = fp16(qn[r]) for the wgmma scan, and
 // eps[r] = the bound on |approximate - exact cosine| the hand-off window uses (0 for an all-zero query).
+// Dot / Euclid (DESIGN.md K1e): eps[r] bounds |approximate - exact key| in key units, from the cosine bound and the slot's
+// norm bounds rho (>= max ||v||) and hmax (>= max h); Euclid also writes rq[r] = (float)||q[r]||.  A query whose key
+// could leave the fp32 range, or whose exact fp64 distances cannot resolve the window, gets its fallback flag fb[r].
+struct PrepMetric {
+  int32_t metric;
+  double rho, hmax;
+  float* rq;      // [rows] Euclid
+  int32_t* fb;    // [rows]
+};
+
 __global__ void __launch_bounds__(256) dense_prep_queries_kernel(const float* __restrict__ q_pad, int nq, int d_pad,
                                                                  float* __restrict__ qn, __half* __restrict__ q16,
-                                                                 float* __restrict__ eps, int mma) {
+                                                                 float* __restrict__ eps, int mma, const PrepMetric pm) {
   __shared__ double s_red[8];
   __shared__ double s_tot;
   const int r = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -638,6 +682,7 @@ __global__ void __launch_bounds__(256) dense_prep_queries_kernel(const float* __
   __syncthreads();
   const double nrm = sqrt(s_tot);
   const bool zero = !(nrm > 0.0) || !real;
+  if (pm.rq && tid == 0) pm.rq[r] = zero ? 0.f : (float)nrm;
   double dd = 0.0;  // ||fp16(qn) - qn||^2
   for (int i = tid; i < d_pad; i += blockDim.x) {
     const float v = zero ? 0.f : (float)((double)src[i] / nrm);
@@ -659,6 +704,24 @@ __global__ void __launch_bounds__(256) dense_prep_queries_kernel(const float* __
     for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += s_red[w];
     float e = 0.f;
     if (!zero) e = mma ? (float)(sqrt(t) * 1.0001) + dense_eps_mma_acc(d_pad) : dense_eps_fp32(d_pad);
+    if (pm.metric != SB_METRIC_COSINE) {
+      // Dot: |acc * (float)c - <qn, v>| <= c (e + 2^-22) with c <= rho (1 + 2^-10); the zero query keeps eps 0 (every key
+      // is exactly 0).  Euclid: key = r * (acc * s) - h; r * eps_dot + r rho 2^-22 (r and its product) + hmax 2^-22 (h
+      // rounded up) + (r rho + hmax) 2^-24 (the subtraction), all inside (r rho + hmax) 2^-20.
+      const double ed = ((double)e + 0x1p-20) * pm.rho * 1.001;
+      const bool fits = pm.rho <= 1e36;
+      if (pm.metric == SB_METRIC_DOT) {
+        e = zero ? 0.f : __double2float_ru(ed);
+        if (!fits) pm.fb[r] = 1;
+      } else {
+        const double rr = zero ? 0.0 : (double)(float)nrm;
+        const double ee = (rr * ed + (rr * pm.rho + pm.hmax) * 0x1p-20) * 1.001;
+        e = __double2float_ru(ee);
+        // the fp64 exact stage resolves ||q - v||^2 to (r + rho)^2 2^-41 (d <= 4096 terms); it must stay far below eps
+        const double res = (rr + pm.rho) * (rr + pm.rho) * 0x1p-41;
+        if (!(rr * pm.rho <= 1e36 && pm.hmax <= 1e36 && fits && res * 1024.0 <= ee)) pm.fb[r] = 1;
+      }
+    }
     eps[r] = e;
   }
 }
@@ -684,6 +747,8 @@ struct FallbackParams {
   unsigned long long* counter;   // [1] queries answered here since the context was created
   const uint32_t* mask;          // FILTER only: match bits, mask[(row / 32) * mask_qs + query]
   int32_t mask_qs;
+  int32_t metric;
+  const double* cfac;
 };
 
 template <bool FILTER>
@@ -698,7 +763,9 @@ __global__ void __launch_bounds__(kFbThreads, 1) dense_exact_fallback_kernel(con
   if (tid == 0) atomicAdd(p.counter, 1ull);
   const float* q = p.q + (size_t)qi * p.d_pad;
   const double qn = query_norm_cta(q, p.d_pad, &qq_s);
-  if (FILTER && !(qn > 0.0)) {
+  // Cosine / Dot: the all-zero query scores 0 on every row.  Euclid: it does not (the nearest rows are the smallest).
+  const bool zero_shortcut = !(qn > 0.0) && p.metric != SB_METRIC_EUCLID;
+  if (FILTER && zero_shortcut) {
     // all-zero query: every cosine is 0 -> the first k MATCHING rows in index order (one warp walks the mask words)
     if (warp != 0) return;
     const int64_t n_words = (p.n + 31) / 32;
@@ -728,7 +795,7 @@ __global__ void __launch_bounds__(kFbThreads, 1) dense_exact_fallback_kernel(con
     if (lane == 0) p.out_counts[qi] = m;
     return;
   }
-  if (!(qn > 0.0)) {
+  if (zero_shortcut) {
     // all-zero query: every cosine is exactly 0 -> the first k rows in index order, no scan needed
     const int m = (int)min((int64_t)p.k, p.n);
     for (int i = tid; i < p.k; i += nt) {
@@ -755,7 +822,7 @@ __global__ void __launch_bounds__(kFbThreads, 1) dense_exact_fallback_kernel(con
       if constexpr (FILTER)
         if (row < p.n) match = (p.mask[(size_t)(row >> 5) * p.mask_qs + qi] >> (row & 31)) & 1u;
       if (row < p.n && match) {
-        okey = f64_orderable(exact_cosine_warp(p.rows, (uint32_t)row, q, p.d_pad, p.ch, qn, lane));
+        okey = f64_orderable(exact_key_warp(p.metric, p.rows, p.cfac, (uint32_t)row, q, p.d_pad, p.ch, qn, lane));
         if (okey == 0ull) okey = 1ull;
       }
       if (lane == 0) {
@@ -779,6 +846,8 @@ __global__ void __launch_bounds__(kFbThreads, 1) dense_exact_fallback_kernel(con
   ra.out_ids = p.out_ids + (size_t)qi * p.k;
   ra.out_scores = p.out_scores + (size_t)qi * p.k;
   ra.out_count = p.out_counts + qi;
+  ra.metric = p.metric;
+  ra.cfac = p.cfac;
   emit_exact_pairs(ek, ei, kFbBest, ra);
 }
 
@@ -848,6 +917,8 @@ struct GatherParams {
   int64_t* out_ids;
   double* out_scores;
   int32_t* out_counts;
+  int32_t metric;
+  const double* cfac;
 };
 
 __global__ void __launch_bounds__(kMergeThreads, 1) dense_filter_gather_kernel(const GatherParams p) {
@@ -882,6 +953,8 @@ __global__ void __launch_bounds__(kMergeThreads, 1) dense_filter_gather_kernel(c
   ra.out_ids = p.out_ids + (size_t)qi * p.k;
   ra.out_scores = p.out_scores + (size_t)qi * p.k;
   ra.out_count = p.out_counts + qi;
+  ra.metric = p.metric;
+  ra.cfac = p.cfac;
   rescore_and_emit(sel, nsel, P, ek, ei, &qq_s, q_s, ra);
 }
 
@@ -949,14 +1022,14 @@ int make_plan(sb_ctx* ctx, const DenseIndex& ix, int k, ScanPlan* pl) {
   return SB_OK;
 }
 
-template <int NCHUNK, int QB, int RW, bool FILTER>
+template <int NCHUNK, int QB, int RW, bool FILTER, bool EUCLID>
 int launch_scan(const ScanParams& sp, const ScanPlan& pl, cudaStream_t st) {
   if (sp.ch == NCHUNK * 32) {
-    auto kern = dense_scan_kernel<NCHUNK, QB, RW, true, FILTER>;
+    auto kern = dense_scan_kernel<NCHUNK, QB, RW, true, FILTER, EUCLID>;
     SB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.scan_smem));
     kern<<<pl.grid, kScanThreads, pl.scan_smem, st>>>(sp);
   } else {
-    auto kern = dense_scan_kernel<NCHUNK, QB, RW, false, FILTER>;
+    auto kern = dense_scan_kernel<NCHUNK, QB, RW, false, FILTER, EUCLID>;
     SB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.scan_smem));
     kern<<<pl.grid, kScanThreads, pl.scan_smem, st>>>(sp);
   }
@@ -964,31 +1037,38 @@ int launch_scan(const ScanParams& sp, const ScanPlan& pl, cudaStream_t st) {
   return SB_OK;
 }
 
-template <int NCHUNK, int RW, bool FILTER>
+template <int NCHUNK, int RW, bool FILTER, bool EUCLID>
 int dispatch_qb(int qb, const ScanParams& sp, const ScanPlan& pl, cudaStream_t st) {
   if constexpr (NCHUNK <= 4) {
-    if (qb == 4) return launch_scan<NCHUNK, 4, RW, FILTER>(sp, pl, st);
+    if (qb == 4) return launch_scan<NCHUNK, 4, RW, FILTER, EUCLID>(sp, pl, st);
   }
   if constexpr (NCHUNK <= 8) {
-    if (qb == 2) return launch_scan<NCHUNK, 2, RW, FILTER>(sp, pl, st);
+    if (qb == 2) return launch_scan<NCHUNK, 2, RW, FILTER, EUCLID>(sp, pl, st);
   }
-  return launch_scan<NCHUNK, 1, RW, FILTER>(sp, pl, st);
+  return launch_scan<NCHUNK, 1, RW, FILTER, EUCLID>(sp, pl, st);
 }
 
-template <bool FILTER>
+template <bool FILTER, bool EUCLID>
 int dispatch_scan(int qb, const ScanParams& sp, const ScanPlan& pl, cudaStream_t st) {
   switch (pl.nchunk) {
-    case 1: return dispatch_qb<1, 4, FILTER>(qb, sp, pl, st);
-    case 2: return dispatch_qb<2, 4, FILTER>(qb, sp, pl, st);
-    case 3: return dispatch_qb<3, 4, FILTER>(qb, sp, pl, st);
-    case 4: return dispatch_qb<4, 4, FILTER>(qb, sp, pl, st);
-    case 6: return dispatch_qb<6, 2, FILTER>(qb, sp, pl, st);
-    case 8: return dispatch_qb<8, 2, FILTER>(qb, sp, pl, st);
-    case 12: return dispatch_qb<12, 1, FILTER>(qb, sp, pl, st);
-    case 16: return dispatch_qb<16, 1, FILTER>(qb, sp, pl, st);
+    case 1: return dispatch_qb<1, 4, FILTER, EUCLID>(qb, sp, pl, st);
+    case 2: return dispatch_qb<2, 4, FILTER, EUCLID>(qb, sp, pl, st);
+    case 3: return dispatch_qb<3, 4, FILTER, EUCLID>(qb, sp, pl, st);
+    case 4: return dispatch_qb<4, 4, FILTER, EUCLID>(qb, sp, pl, st);
+    case 6: return dispatch_qb<6, 2, FILTER, EUCLID>(qb, sp, pl, st);
+    case 8: return dispatch_qb<8, 2, FILTER, EUCLID>(qb, sp, pl, st);
+    case 12: return dispatch_qb<12, 1, FILTER, EUCLID>(qb, sp, pl, st);
+    case 16: return dispatch_qb<16, 1, FILTER, EUCLID>(qb, sp, pl, st);
   }
   sb_set_error("dense: unsupported chunk count %d", pl.nchunk);
   return SB_ERR_UNSUPPORTED;
+}
+
+// Cosine and Dot run the same (acc * scale) kernels; Euclid its own instantiations
+int dispatch_scan_metric(int metric, bool filter, int qb, const ScanParams& sp, const ScanPlan& pl, cudaStream_t st) {
+  if (metric == SB_METRIC_EUCLID)
+    return filter ? dispatch_scan<true, true>(qb, sp, pl, st) : dispatch_scan<false, true>(qb, sp, pl, st);
+  return filter ? dispatch_scan<true, false>(qb, sp, pl, st) : dispatch_scan<false, false>(qb, sp, pl, st);
 }
 
 // q_pad: [B][d_pad] fp32 device, zero padded.  Enqueues all scan passes of a chunk of queries, then ONE merge launch
@@ -1008,9 +1088,9 @@ int dense_topk_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int B, i
   rc = ctx->cand_dev.reserve((size_t)chunk * per_q * 8);
   if (rc) return rc;
   // normalised queries for the scan, eps + fallback flags for the hand-off
-  float *qn = nullptr, *eps = nullptr;
+  float *qn = nullptr, *eps = nullptr, *rq = nullptr;
   int32_t* fb = nullptr;
-  if ((rc = dense_prep_queries(ctx, ix, q_pad, B, B, /*mma=*/false, &qn, nullptr, &eps, &fb, st))) return rc;
+  if ((rc = dense_prep_queries(ctx, ix, q_pad, B, B, /*mma=*/false, &qn, nullptr, &eps, &fb, &rq, st))) return rc;
   if (flt) SB_CUDA(cudaFuncSetAttribute(dense_merge_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                         (int)pl.merge_smem));
   else SB_CUDA(cudaFuncSetAttribute(dense_merge_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -1045,9 +1125,11 @@ int dense_topk_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int B, i
       sp.mask = flt ? flt->mask + (c0 + b0) : nullptr;
       sp.mask_qs = flt ? flt->qs : 0;
       sp.state = flt ? flt->state + (c0 + b0) : nullptr;
+      sp.hh = ix.hh;
+      sp.rq = rq ? rq + (c0 + b0) : nullptr;
       {
         ProfScope ps(ctx, SB_PROF_DENSE_SCAN, st);
-        rc = flt ? dispatch_scan<true>(qb, sp, pl, st) : dispatch_scan<false>(qb, sp, pl, st);
+        rc = dispatch_scan_metric(ix.metric, flt != nullptr, qb, sp, pl, st);
       }
       if (rc) return rc;
       b0 += qb;
@@ -1070,6 +1152,8 @@ int dense_topk_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int B, i
     mp.out_scores = out_scores + (size_t)c0 * k;
     mp.out_counts = out_counts + c0;
     mp.state = flt ? flt->state + c0 : nullptr;
+    mp.metric = ix.metric;
+    mp.cfac = ix.cfac;
     {
       ProfScope ps(ctx, SB_PROF_DENSE_MERGE, st);
       if (flt) dense_merge_kernel<true><<<nq, kMergeThreads, pl.merge_smem, st>>>(mp);
@@ -1089,13 +1173,20 @@ __global__ void fill_empty_topk_kernel(int64_t* ids, double* sc, int32_t* cnt, i
   if (i < B) cnt[i] = 0;
 }
 
-__global__ void dense_fetch_kernel(const __half* rows, int d, int d_pad, int64_t n, int64_t id_base,
+// the stored vector: y (Cosine), c * y in fp64 rounded to fp32 (Dot / Euclid, cfac != nullptr)
+__global__ void dense_fetch_kernel(const __half* rows, const double* cfac, int d, int d_pad, int64_t n, int64_t id_base,
                                    const int64_t* ids, int n_ids, float* out) {
   int r = blockIdx.x;
   if (r >= n_ids) return;
   int64_t idx = ids[r] - id_base;
-  for (int i = threadIdx.x; i < d; i += blockDim.x)
-    out[(size_t)r * d + i] = (idx >= 0 && idx < n) ? __half2float(rows[(size_t)idx * d_pad + i]) : 0.f;
+  const bool live = idx >= 0 && idx < n;
+  const double c = (cfac && live) ? cfac[idx] : 1.0;
+  for (int i = threadIdx.x; i < d; i += blockDim.x) {
+    float v = 0.f;
+    if (live) v = cfac ? (float)(c * (double)__half2float(rows[(size_t)idx * d_pad + i]))
+                       : __half2float(rows[(size_t)idx * d_pad + i]);
+    out[(size_t)r * d + i] = v;
+  }
 }
 
 }  // namespace
@@ -1103,11 +1194,18 @@ __global__ void dense_fetch_kernel(const __half* rows, int d, int d_pad, int64_t
 // Shared with dense_mma.cu: query preparation (normalised fp32 copy, optional fp16 operand rows, eps, cleared fallback
 // flags) and the brute-force fallback launch.  `rows` >= B operand rows are prepared (rows >= B are zero padding).
 int dense_prep_queries(sb_ctx* ctx, const DenseIndex& ix, const float* q_pad, int B, int rows, bool mma, float** qn_out,
-                       __half* q16, float** eps_out, int32_t** fb_out, cudaStream_t st) {
+                       __half* q16, float** eps_out, int32_t** fb_out, float** rq_out, cudaStream_t st) {
   int rc;
-  if ((rc = ctx->qaux_dev.reserve((size_t)rows * 8 + 64))) return rc;
+  if ((rc = ctx->qaux_dev.reserve((size_t)rows * 12 + 64))) return rc;
   float* eps = ctx->qaux_dev.as<float>();
   int32_t* fb = reinterpret_cast<int32_t*>(eps + rows);
+  PrepMetric pm;
+  pm.metric = ix.metric;
+  pm.rho = ix.rho_max;
+  pm.hmax = ix.h_max;
+  pm.rq = ix.metric == SB_METRIC_EUCLID ? reinterpret_cast<float*>(fb + rows) : nullptr;
+  pm.fb = fb;
+  *rq_out = pm.rq;
   float* qn = nullptr;
   if (qn_out) {
     if ((rc = ctx->qn_dev.reserve((size_t)rows * ix.d_pad * sizeof(float)))) return rc;
@@ -1116,7 +1214,7 @@ int dense_prep_queries(sb_ctx* ctx, const DenseIndex& ix, const float* q_pad, in
   }
   SB_CUDA(cudaMemsetAsync(fb, 0, (size_t)rows * 4, st));
   ctx->launches += 1;
-  dense_prep_queries_kernel<<<rows, 256, 0, st>>>(q_pad, B, ix.d_pad, qn, q16, eps, mma ? 1 : 0);
+  dense_prep_queries_kernel<<<rows, 256, 0, st>>>(q_pad, B, ix.d_pad, qn, q16, eps, mma ? 1 : 0, pm);
   SB_CUDA(cudaGetLastError());
   *eps_out = eps;
   *fb_out = fb;
@@ -1146,6 +1244,8 @@ int dense_fallback_enqueue(sb_ctx* ctx, const DenseIndex& ix, const float* q_pad
   fp.out_ids = out_ids;
   fp.out_scores = out_scores;
   fp.out_counts = out_counts;
+  fp.metric = ix.metric;
+  fp.cfac = ix.cfac;
   ctx->launches += 1;
   if (flt) dense_exact_fallback_kernel<true><<<B, kFbThreads, 0, st>>>(fp);
   else dense_exact_fallback_kernel<false><<<B, kFbThreads, 0, st>>>(fp);
@@ -1259,6 +1359,8 @@ int dense_topk_filtered_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad,
       gp.out_ids = oi;
       gp.out_scores = os;
       gp.out_counts = oc;
+      gp.metric = ix.metric;
+      gp.cfac = ix.cfac;
       ProfScope ps(ctx, SB_PROF_DENSE_GATHER, st);
       dense_filter_gather_kernel<<<n_gather, kMergeThreads, gather_smem, st>>>(gp);
     }
@@ -1297,25 +1399,31 @@ int dense_store_staged(sb_ctx* ctx, DenseIndex& ix, const void* vecs, int64_t n,
     const int64_t* dst = dst_dev ? dst_dev + r0 : nullptr;
     if (dtype == SB_F32)
       dense_store_rows_kernel<float><<<blocks, wpb * 32, 0, ctx->stream>>>(ctx->misc_dev.as<float>(), nr, d, ix.d_pad,
-                                                                           ix.rows, ix.inv_norm, row0 + r0, dst, true);
-    else
+                                                                           ix.rows, ix.inv_norm, row0 + r0, dst, true,
+                                                                           ix.cfac, ix.hh);
+    else   // Cosine keeps fp16 input verbatim; Dot / Euclid normalise it like fp32 input
       dense_store_rows_kernel<__half><<<blocks, wpb * 32, 0, ctx->stream>>>(ctx->misc_dev.as<__half>(), nr, d, ix.d_pad,
-                                                                            ix.rows, ix.inv_norm, row0 + r0, dst, false);
+                                                                            ix.rows, ix.inv_norm, row0 + r0, dst,
+                                                                            ix.cfac != nullptr, ix.cfac, ix.hh);
     SB_CUDA(cudaGetLastError());
     SB_CUDA(cudaStreamSynchronize(ctx->stream));  // staging buffer is reused by the next chunk
   }
   return SB_OK;
 }
 
-// Reallocate rows / inv_norm / every loaded tag column to n_cap rows (> ix.n_cap): the [0, n_pad) prefix is copied
-// device to device, the rest is zero (tags -1).  Old and new buffers coexist during the copy.
+// Reallocate rows / inv_norm / cfac / hh / every loaded tag column to n_cap rows (> ix.n_cap): the [0, n_pad) prefix is
+// copied device to device, the rest is zero (tags -1).  Old and new buffers coexist during the copy.
 int dense_grow(sb_ctx* ctx, DenseIndex& ix, int64_t n_cap) {
   const size_t rb = (size_t)ix.d_pad * sizeof(__half);
   __half* rows = nullptr;
   float* inv = nullptr;
+  double* cfac = nullptr;
+  float* hh = nullptr;
   int32_t* tags[SB_MAX_TAG_FIELDS] = {};
   cudaError_t e = cudaMalloc(&rows, (size_t)n_cap * rb);
   if (e == cudaSuccess) e = cudaMalloc(&inv, (size_t)n_cap * sizeof(float));
+  if (e == cudaSuccess && ix.metric != SB_METRIC_COSINE) e = cudaMalloc(&cfac, (size_t)n_cap * sizeof(double));
+  if (e == cudaSuccess && ix.metric == SB_METRIC_EUCLID) e = cudaMalloc(&hh, (size_t)n_cap * sizeof(float));
   for (int f = 0; f < SB_MAX_TAG_FIELDS && e == cudaSuccess; ++f)
     if (ix.tags[f]) e = cudaMalloc(&tags[f], (size_t)n_cap * 4);
   const int64_t keep = ix.n_pad;
@@ -1325,6 +1433,15 @@ int dense_grow(sb_ctx* ctx, DenseIndex& ix, int64_t n_cap) {
     e = cudaMemcpyAsync(inv, ix.inv_norm, (size_t)keep * sizeof(float), cudaMemcpyDeviceToDevice, st);
   if (e == cudaSuccess) e = cudaMemsetAsync(rows + (size_t)keep * ix.d_pad, 0, (size_t)(n_cap - keep) * rb, st);
   if (e == cudaSuccess) e = cudaMemsetAsync(inv + keep, 0, (size_t)(n_cap - keep) * sizeof(float), st);
+  if (cfac) {
+    if (e == cudaSuccess && keep)
+      e = cudaMemcpyAsync(cfac, ix.cfac, (size_t)keep * sizeof(double), cudaMemcpyDeviceToDevice, st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(cfac + keep, 0, (size_t)(n_cap - keep) * sizeof(double), st);
+  }
+  if (hh) {
+    if (e == cudaSuccess && keep) e = cudaMemcpyAsync(hh, ix.hh, (size_t)keep * sizeof(float), cudaMemcpyDeviceToDevice, st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(hh + keep, 0, (size_t)(n_cap - keep) * sizeof(float), st);
+  }
   for (int f = 0; f < SB_MAX_TAG_FIELDS && e == cudaSuccess; ++f) {
     if (!tags[f]) continue;
     if (keep) e = cudaMemcpyAsync(tags[f], ix.tags[f], (size_t)keep * 4, cudaMemcpyDeviceToDevice, st);
@@ -1335,14 +1452,20 @@ int dense_grow(sb_ctx* ctx, DenseIndex& ix, int64_t n_cap) {
     cudaStreamSynchronize(st);
     cudaFree(rows);
     cudaFree(inv);
+    cudaFree(cfac);
+    cudaFree(hh);
     for (int f = 0; f < SB_MAX_TAG_FIELDS; ++f) cudaFree(tags[f]);
     sb_set_error("dense: growing slot to %lld rows failed: %s", (long long)n_cap, cudaGetErrorString(e));
     return SB_ERR_CUDA;
   }
   cudaFree(ix.rows);
   cudaFree(ix.inv_norm);
+  cudaFree(ix.cfac);
+  cudaFree(ix.hh);
   ix.rows = rows;
   ix.inv_norm = inv;
+  ix.cfac = cfac;
+  ix.hh = hh;
   for (int f = 0; f < SB_MAX_TAG_FIELDS; ++f)
     if (ix.tags[f]) {
       cudaFree(ix.tags[f]);
@@ -1364,6 +1487,38 @@ int check_rows(const char* who, const int64_t* rows, int64_t n, int64_t limit, s
   return SB_OK;
 }
 
+// Dot / Euclid input rows, checked on the host before anything changes: every fp64 norm finite and, for Euclid, every
+// squared norm finite in fp32.  Returns the norm bounds the rows need: *rho >= max ||v||, *hmax >= max h (DESIGN.md K1e;
+// the device sums in another order, which the 2^-20 margin covers many times over).
+int check_metric_rows(const char* who, int metric, const void* vecs, int64_t n, int d, int32_t dtype, double* rho,
+                      double* hmax) {
+  double mx = 0.0;
+  for (int64_t r = 0; r < n; ++r) {
+    double ss = 0.0;
+    if (dtype == SB_F32) {
+      const float* v = reinterpret_cast<const float*>(vecs) + (size_t)r * d;
+      for (int i = 0; i < d; ++i) ss += (double)v[i] * (double)v[i];
+    } else {
+      const __half* v = reinterpret_cast<const __half*>(vecs) + (size_t)r * d;
+      for (int i = 0; i < d; ++i) {
+        const double x = (double)__half2float(v[i]);
+        ss += x * x;
+      }
+    }
+    SB_REQUIRE(std::isfinite(ss), SB_ERR_ARG, "%s: row %lld has a non-finite norm", who, (long long)r);
+    SB_REQUIRE(metric != SB_METRIC_EUCLID || ss <= (double)FLT_MAX, SB_ERR_ARG,
+               "%s: row %lld has a squared norm %g beyond the fp32 range (Euclid)", who, (long long)r, ss);
+    mx = std::max(mx, ss);
+  }
+  const double m = 1.0 + 0x1p-20;
+  *rho = sqrt(mx) * m;
+  const double hv = 0.5 * mx * m;
+  float hf = (float)hv;
+  if ((double)hf < hv) hf = nextafterf(hf, INFINITY);
+  *hmax = metric == SB_METRIC_EUCLID ? (double)hf : 0.0;
+  return SB_OK;
+}
+
 }  // namespace
 
 // Shared with other translation units (hybrid batch path, scorers).
@@ -1382,19 +1537,29 @@ int sb_dense_pad_queries(sb_ctx* ctx, const DenseIndex& ix, const float* q, int 
 
 extern "C" {
 
-int sb_dense_load(sb_ctx* ctx, int slot, const void* vecs, int64_t n, int32_t d, int32_t dtype, int64_t id_base) {
+int sb_dense_load_metric(sb_ctx* ctx, int slot, const void* vecs, int64_t n, int32_t d, int32_t dtype, int64_t id_base,
+                         int32_t metric) {
   SB_REQUIRE(ctx != nullptr, SB_ERR_ARG, "sb_dense_load: ctx is NULL");
   SB_REQUIRE(slot >= 0 && slot < SB_MAX_DENSE_SLOTS, SB_ERR_ARG, "sb_dense_load: bad slot %d", slot);
   SB_REQUIRE(n >= 0 && d > 0 && d <= 4096, SB_ERR_ARG, "sb_dense_load: bad shape n=%lld d=%d", (long long)n, d);
   SB_REQUIRE(n < (1ll << 31), SB_ERR_ARG, "sb_dense_load: a shard holds at most 2^31-1 rows");
   SB_REQUIRE(dtype == SB_F32 || dtype == SB_F16, SB_ERR_ARG, "sb_dense_load: dtype must be SB_F32 or SB_F16");
   SB_REQUIRE(n == 0 || vecs != nullptr, SB_ERR_ARG, "sb_dense_load: vecs is NULL");
+  SB_REQUIRE(metric == SB_METRIC_COSINE || metric == SB_METRIC_DOT || metric == SB_METRIC_EUCLID, SB_ERR_ARG,
+             "sb_dense_load: metric %d is not supported (SB_METRIC_COSINE, SB_METRIC_DOT or SB_METRIC_EUCLID)", metric);
+  double rho = 0.0, hmax = 0.0;
+  if (metric != SB_METRIC_COSINE) {
+    int rc = check_metric_rows("sb_dense_load", metric, vecs, n, d, dtype, &rho, &hmax);
+    if (rc) return rc;
+  }
   std::lock_guard<std::mutex> lk(ctx->mu);
   DeviceGuard g(ctx->device);
   DenseIndex& ix = ctx->dense[slot];
   SB_CUDA(cudaStreamSynchronize(ctx->stream));
   if (ix.rows) cudaFree(ix.rows);
   if (ix.inv_norm) cudaFree(ix.inv_norm);
+  if (ix.cfac) cudaFree(ix.cfac);
+  if (ix.hh) cudaFree(ix.hh);
   for (int f = 0; f < SB_MAX_TAG_FIELDS; ++f)
     if (ix.tags[f]) cudaFree(ix.tags[f]);
   ix = DenseIndex();
@@ -1403,13 +1568,34 @@ int sb_dense_load(sb_ctx* ctx, int slot, const void* vecs, int64_t n, int32_t d,
   ix.d_pad = (d + 7) / 8 * 8;
   ix.n_pad = round_rows(n);
   ix.id_base = id_base;
+  ix.metric = metric;
+  ix.rho_max = rho;
+  ix.h_max = hmax;
   if (n == 0) return SB_OK;
   ix.n_cap = ix.n_pad;
   SB_CUDA(cudaMalloc(&ix.rows, (size_t)ix.n_cap * ix.d_pad * sizeof(__half)));
   SB_CUDA(cudaMalloc(&ix.inv_norm, (size_t)ix.n_cap * sizeof(float)));
   SB_CUDA(cudaMemsetAsync(ix.rows, 0, (size_t)ix.n_cap * ix.d_pad * sizeof(__half), ctx->stream));
   SB_CUDA(cudaMemsetAsync(ix.inv_norm, 0, (size_t)ix.n_cap * sizeof(float), ctx->stream));
+  if (metric != SB_METRIC_COSINE) {
+    SB_CUDA(cudaMalloc(&ix.cfac, (size_t)ix.n_cap * sizeof(double)));
+    SB_CUDA(cudaMemsetAsync(ix.cfac, 0, (size_t)ix.n_cap * sizeof(double), ctx->stream));
+  }
+  if (metric == SB_METRIC_EUCLID) {
+    SB_CUDA(cudaMalloc(&ix.hh, (size_t)ix.n_cap * sizeof(float)));
+    SB_CUDA(cudaMemsetAsync(ix.hh, 0, (size_t)ix.n_cap * sizeof(float), ctx->stream));
+  }
   return dense_store_staged(ctx, ix, vecs, n, dtype, nullptr, 0);
+}
+
+int sb_dense_load(sb_ctx* ctx, int slot, const void* vecs, int64_t n, int32_t d, int32_t dtype, int64_t id_base) {
+  return sb_dense_load_metric(ctx, slot, vecs, n, d, dtype, id_base, SB_METRIC_COSINE);
+}
+
+int32_t sb_dense_metric(sb_ctx* ctx, int slot) {
+  if (!ctx || slot < 0 || slot >= SB_MAX_DENSE_SLOTS) return -1;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  return ctx->dense[slot].metric;
 }
 
 int sb_dense_reserve(sb_ctx* ctx, int slot, int64_t n_cap) {
@@ -1445,6 +1631,9 @@ int sb_dense_upsert(sb_ctx* ctx, int slot, const int64_t* rows, const void* vecs
   const int64_t m = sorted.end() - std::lower_bound(sorted.begin(), sorted.end(), ix.n);
   SB_REQUIRE(m == 0 || (sorted[n - m] == ix.n && sorted[n - 1] == ix.n + m - 1), SB_ERR_ARG,
              "sb_dense_upsert: appended rows must be exactly %lld .. %lld", (long long)ix.n, (long long)(ix.n + m - 1));
+  double rho = 0.0, hmax = 0.0;
+  if (ix.metric != SB_METRIC_COSINE)
+    if ((rc = check_metric_rows("sb_dense_upsert", ix.metric, vecs, n, ix.d, dtype, &rho, &hmax))) return rc;
   SB_CUDA(cudaDeviceSynchronize());   // searches enqueued on other streams may still read the slot
   const int64_t n_new = ix.n + m;
   if (round_rows(n_new) > ix.n_cap)
@@ -1460,6 +1649,9 @@ int sb_dense_upsert(sb_ctx* ctx, int slot, const int64_t* rows, const void* vecs
   SB_CUDA(cudaStreamSynchronize(ctx->stream));
   ix.n = n_new;
   ix.n_pad = round_rows(n_new);
+  // the bounds only rise: an overwritten or deleted row's larger norm leaves a stale bound, which is still a bound
+  ix.rho_max = std::max(ix.rho_max, rho);
+  ix.h_max = std::max(ix.h_max, hmax);
   return SB_OK;
 }
 
@@ -1530,6 +1722,8 @@ int sb_dense_delete(sb_ctx* ctx, int slot, const int64_t* rows, int64_t n, int64
     MoveParams mp;
     mp.rows = ix.rows;
     mp.inv_norm = ix.inv_norm;
+    mp.cfac = ix.cfac;
+    mp.hh = ix.hh;
     memcpy(mp.tags, ix.tags, sizeof(mp.tags));
     mp.from = f_dev;
     mp.to = f_dev + mv;
@@ -1541,6 +1735,8 @@ int sb_dense_delete(sb_ctx* ctx, int slot, const int64_t* rows, int64_t n, int64
   // the vacated tail [keep, n) returns to the zero state of unused capacity
   SB_CUDA(cudaMemsetAsync(ix.rows + (size_t)keep * ix.d_pad, 0, (size_t)n * ix.d_pad * sizeof(__half), ctx->stream));
   SB_CUDA(cudaMemsetAsync(ix.inv_norm + keep, 0, (size_t)n * sizeof(float), ctx->stream));
+  if (ix.cfac) SB_CUDA(cudaMemsetAsync(ix.cfac + keep, 0, (size_t)n * sizeof(double), ctx->stream));
+  if (ix.hh) SB_CUDA(cudaMemsetAsync(ix.hh + keep, 0, (size_t)n * sizeof(float), ctx->stream));
   for (int f = 0; f < SB_MAX_TAG_FIELDS; ++f)
     if (ix.tags[f]) SB_CUDA(cudaMemsetAsync(ix.tags[f] + keep, 0xff, (size_t)n * 4, ctx->stream));
   SB_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -1657,7 +1853,7 @@ int sb_dense_fetch(sb_ctx* ctx, int slot, const int64_t* ids, int32_t n_ids, flo
   if ((rc = ctx->misc2_dev.reserve((size_t)n_ids * 8))) return rc;
   if ((rc = ctx->misc3_dev.reserve((size_t)n_ids * ix.d * 4))) return rc;
   SB_CUDA(cudaMemcpyAsync(ctx->misc2_dev.p, ids, (size_t)n_ids * 8, cudaMemcpyHostToDevice, ctx->stream));
-  dense_fetch_kernel<<<n_ids, 128, 0, ctx->stream>>>(ix.rows, ix.d, ix.d_pad, ix.n, ix.id_base,
+  dense_fetch_kernel<<<n_ids, 128, 0, ctx->stream>>>(ix.rows, ix.cfac, ix.d, ix.d_pad, ix.n, ix.id_base,
                                                      ctx->misc2_dev.as<int64_t>(), n_ids, ctx->misc3_dev.as<float>());
   SB_CUDA(cudaGetLastError());
   SB_CUDA(cudaMemcpyAsync(out, ctx->misc3_dev.p, (size_t)n_ids * ix.d * 4, cudaMemcpyDeviceToHost, ctx->stream));

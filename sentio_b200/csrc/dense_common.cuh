@@ -12,6 +12,8 @@ struct RescoreArgs {
   int64_t* out_ids;     // [k] of this query
   double* out_scores;   // [k]
   int32_t* out_count;   // [1]
+  int32_t metric;       // SB_METRIC_*
+  const double* cfac;   // [rows] c of v = c * y (Dot / Euclid)
 };
 
 // ---- approximate -> exact hand-off (DESIGN.md "K1: exactness") --------------------------------------------------------
@@ -104,14 +106,78 @@ __device__ __forceinline__ void sort_exact_pairs(unsigned long long* ek, uint32_
   }
 }
 
-// first min(k, P) sorted pairs -> this query's output rows
+// Exact fp64 ordering key of NR stored rows under Dot or Euclid (DESIGN.md K1e), one full warp; every lane returns them.
+//   Dot:    c * sum q_i y_i                   (the score)
+//   Euclid: -sqrt(sum (q_i - c y_i)^2)        (minus the distance: larger = better, like every other key; computed
+//                                              directly, not as ||q||^2 - 2<q,v> + ||v||^2, which cancels when q ~ v)
+// NR = 1 and NR = 2 perform the same operations in the same order per row, so they agree bit for bit.
+template <int NR>
+__device__ __forceinline__ void exact_metric_warp(int metric, const __half* rows, const double* cfac,
+                                                  const uint32_t (&idx)[NR], const float* q, int d_pad, int nch,
+                                                  int lane, double (&out)[NR]) {
+  const bool euclid = metric == SB_METRIC_EUCLID;
+  const uint4* r[NR];
+  double c[NR], acc[NR];
+#pragma unroll
+  for (int i = 0; i < NR; ++i) {
+    r[i] = reinterpret_cast<const uint4*>(rows + (size_t)idx[i] * d_pad);
+    c[i] = __ldg(cfac + idx[i]);
+    acc[i] = 0.0;
+  }
+  for (int ch = lane; ch < nch; ch += 32) {
+    const float4 qa = *reinterpret_cast<const float4*>(q + (size_t)ch * 8);
+    const float4 qb = *reinterpret_cast<const float4*>(q + (size_t)ch * 8 + 4);
+    const float qv[8] = {qa.x, qa.y, qa.z, qa.w, qb.x, qb.y, qb.z, qb.w};
+    uint4 raw[NR];
+#pragma unroll
+    for (int i = 0; i < NR; ++i) raw[i] = __ldg(r[i] + ch);
+#pragma unroll
+    for (int i = 0; i < NR; ++i) {
+      const __half2* h2 = reinterpret_cast<const __half2*>(&raw[i]);
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const float2 xf = __half22float2(h2[e]);
+        const double x0 = (double)xf.x, x1 = (double)xf.y;
+        if (euclid) {
+          const double t0 = __fma_rn(-c[i], x0, (double)qv[2 * e]);
+          const double t1 = __fma_rn(-c[i], x1, (double)qv[2 * e + 1]);
+          acc[i] = __fma_rn(t0, t0, acc[i]);
+          acc[i] = __fma_rn(t1, t1, acc[i]);
+        } else {
+          acc[i] = __fma_rn(x0, (double)qv[2 * e], acc[i]);
+          acc[i] = __fma_rn(x1, (double)qv[2 * e + 1], acc[i]);
+        }
+      }
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < NR; ++i) {
+    for (int o = 16; o; o >>= 1) acc[i] += __shfl_xor_sync(0xffffffffu, acc[i], o);
+    out[i] = euclid ? -sqrt(acc[i]) : c[i] * acc[i];
+  }
+}
+
+// exact ordering key of one stored row under the slot's metric (Cosine: the existing cosine path)
+__device__ __forceinline__ double exact_key_warp(int metric, const __half* rows, const double* cfac, uint32_t idx,
+                                                 const float* q, int d_pad, int nch, double qn, int lane) {
+  if (metric == SB_METRIC_COSINE) return exact_cosine_warp(rows, idx, q, d_pad, nch, qn, lane);
+  const uint32_t ix[1] = {idx};
+  double s[1];
+  exact_metric_warp<1>(metric, rows, cfac, ix, q, d_pad, nch, lane, s);
+  return s[0];
+}
+
+// first min(k, P) sorted pairs -> this query's output rows (Euclid keys are minus the distance: the score is the distance)
 __device__ __forceinline__ void emit_exact_pairs(const unsigned long long* ek, const uint32_t* ei, int P,
                                                  const RescoreArgs& p) {
   const int tid = threadIdx.x, nt = blockDim.x;
+  const bool euclid = p.metric == SB_METRIC_EUCLID;
   for (int i = tid; i < p.k; i += nt) {
     const bool valid = (i < P) && ek[i] != 0ull;
     p.out_ids[i] = valid ? p.id_base + (int64_t)ei[i] : -1;
-    p.out_scores[i] = valid ? orderable_f64(ek[i]) : 0.0;
+    double s = 0.0;
+    if (valid) s = euclid ? -orderable_f64(ek[i]) : orderable_f64(ek[i]);
+    p.out_scores[i] = s;
   }
   if (tid == 0) {
     int lo = 0, hi = min(p.k, P);  // valid entries are a prefix (empty keys sort last)
@@ -181,15 +247,23 @@ __device__ __forceinline__ void rescore_and_emit(const unsigned long long* sel, 
       i0 = key32_idx(key0);
       i1 = key32_idx(key1);
       double s0, s1;
-      exact_cosine_warp2(p.rows, i0, i1, q_s, p.d_pad, p.ch, qn, lane, &s0, &s1);
+      if (p.metric == SB_METRIC_COSINE) {
+        exact_cosine_warp2(p.rows, i0, i1, q_s, p.d_pad, p.ch, qn, lane, &s0, &s1);
+      } else {
+        const uint32_t ix[2] = {i0, i1};
+        double s[2];
+        exact_metric_warp<2>(p.metric, p.rows, p.cfac, ix, q_s, p.d_pad, p.ch, lane, s);
+        s0 = s[0];
+        s1 = s[1];
+      }
       o0 = f64_orderable(s0);
       o1 = f64_orderable(s1);
     } else if (key0 != 0ull) {
       i0 = key32_idx(key0);
-      o0 = f64_orderable(exact_cosine_warp(p.rows, i0, q_s, p.d_pad, p.ch, qn, lane));
+      o0 = f64_orderable(exact_key_warp(p.metric, p.rows, p.cfac, i0, q_s, p.d_pad, p.ch, qn, lane));
     } else if (key1 != 0ull) {
       i1 = key32_idx(key1);
-      o1 = f64_orderable(exact_cosine_warp(p.rows, i1, q_s, p.d_pad, p.ch, qn, lane));
+      o1 = f64_orderable(exact_key_warp(p.metric, p.rows, p.cfac, i1, q_s, p.d_pad, p.ch, qn, lane));
     }
     if (key0 != 0ull && o0 == 0ull) o0 = 1ull;  // keep 0 reserved for "empty"
     if (key1 != 0ull && o1 == 0ull) o1 = 1ull;

@@ -78,9 +78,12 @@ struct MmaScanParams {
   int32_t prefetch;             // boxes (16 KB) prefetched into L2 beyond the shared-memory ring (0 = off)
   const uint32_t* mask;         // FILTER only: match bits of the group's queries, mask[(row / 32) * mask_qs + column]
   int32_t mask_qs;
+  const float* hh;              // EUCLID only: per-row h (>= ||v||^2 / 2)
+  const float* rq;              // EUCLID only: [QBN] (float)||q|| of the group's queries
 };
 
-template <int QBN, bool FILTER>
+// Key of a row (dense.cu dense_scan_kernel): acc * scale[row], EUCLID r * (acc * scale[row]) - h[row].
+template <int QBN, bool FILTER, bool EUCLID>
 __global__ void __launch_bounds__(kMmaThreads, 1)
 dense_scan_mma_kernel(const __grid_constant__ CUtensorMap tm_rows, const __grid_constant__ CUtensorMap tm_q,
                       const MmaScanParams p) {
@@ -94,6 +97,7 @@ dense_scan_mma_kernel(const __grid_constant__ CUtensorMap tm_rows, const __grid_
   const uint32_t bar_full = smem_u32(bars), bar_empty = smem_u32(bars + p.stages);
   volatile float* thr = reinterpret_cast<volatile float*>(bars + 2 * p.stages);   // [QBN]
   int* cnt = reinterpret_cast<int*>(const_cast<float*>(thr) + QBN);              // [QBN]
+  float* rq_s = reinterpret_cast<float*>(cnt + QBN);                             // [QBN] EUCLID only
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int grid = gridDim.x, cta = blockIdx.x;
@@ -112,6 +116,7 @@ dense_scan_mma_kernel(const __grid_constant__ CUtensorMap tm_rows, const __grid_
   for (int i = threadIdx.x; i < QBN; i += blockDim.x) {
     thr[i] = p.thr_init ? p.thr_init[i] : -INFINITY;
     cnt[i] = 0;
+    if constexpr (EUCLID) rq_s[i] = p.rq[i];
   }
   __syncthreads();
 
@@ -172,6 +177,16 @@ dense_scan_mma_kernel(const __grid_constant__ CUtensorMap tm_rows, const __grid_
       const bool live0 = row0 < p.n, live1 = row0 + 8 < p.n;
       const float invn0 = live0 ? __ldg(p.inv_norm + row0) : 0.f;
       const float invn1 = live1 ? __ldg(p.inv_norm + row0 + 8) : 0.f;
+      float h0 = 0.f, h1 = 0.f;
+      if constexpr (EUCLID) {
+        h0 = live0 ? __ldg(p.hh + row0) : 0.f;
+        h1 = live1 ? __ldg(p.hh + row0 + 8) : 0.f;
+      }
+      auto key = [&](float a, float invn, float h, int col) {
+        float s = a * invn;
+        if constexpr (EUCLID) s = __fsub_rn(__fmul_rn(rq_s[col], s), h);
+        return s;
+      };
       // FILTER: row0 and row0 + 8 lie in one 32-row mask word; columns 4 j + 2 (lane % 4) + {0, 1} are one 8-byte load
       const uint32_t* mrow = nullptr;
       if constexpr (FILTER) mrow = p.mask + (size_t)(row0 >> 5) * p.mask_qs + 2 * (lane & 3);
@@ -195,13 +210,13 @@ dense_scan_mma_kernel(const __grid_constant__ CUtensorMap tm_rows, const __grid_
               m0 = m0 && ((w >> sh0) & 1u);
               m1 = m1 && ((w >> sh1) & 1u);
             }
-            const float s0 = m0 ? acc[2 * j + e] * invn0 : -INFINITY;
-            const float s1 = m1 ? acc[2 * j + 2 + e] * invn1 : -INFINITY;
+            const int col = 4 * j + 2 * (lane & 3) + e;
+            const float s0 = m0 ? key(acc[2 * j + e], invn0, h0, col) : -INFINITY;
+            const float s1 = m1 ? key(acc[2 * j + 2 + e], invn1, h1, col) : -INFINITY;
             uint32_t best = max(f32_orderable(s0), f32_orderable(s1));
             best = max(best, __shfl_xor_sync(0xffffffffu, best, 4));
             best = max(best, __shfl_xor_sync(0xffffffffu, best, 8));
             best = max(best, __shfl_xor_sync(0xffffffffu, best, 16));
-            const int col = 4 * j + 2 * (lane & 3) + e;
             if (lane < 4) my_cand[(size_t)col * q_stride + slot] = ((unsigned long long)best << 32) | 0xffffffffull;
           }
         }
@@ -215,10 +230,11 @@ dense_scan_mma_kernel(const __grid_constant__ CUtensorMap tm_rows, const __grid_
             if (!(h ? live1 : live0)) continue;
             const int64_t row = row0 + 8 * h;
             const float invn = h ? invn1 : invn0;
+            const float hrow = h ? h1 : h0;
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
               const int col = 4 * j + 2 * (lane & 3) + e;
-              const float score = acc[2 * j + 2 * h + e] * invn;
+              const float score = key(acc[2 * j + 2 * h + e], invn, hrow, col);
               bool match = true;
               if constexpr (FILTER) match = ((e ? mw.y : mw.x) >> (h ? sh1 : sh0)) & 1u;
               if (score >= thr[col] && match) {
@@ -258,6 +274,8 @@ struct SelectParams {
   double* out_scores;
   int32_t* out_counts;
   const int32_t* state;             // FILTER only: [nq] 1 = answered by the gather path (threshold +inf, no emit)
+  int32_t metric;
+  const double* cfac;
 };
 
 // One CTA per query.  A lower bound of the k-th best approximate key among the survivors of all CTAs by an MSB-first
@@ -291,7 +309,10 @@ __global__ void __launch_bounds__(kSelectThreads, 2) dense_select_kernel(const S
       return;
     }
   }
-  if (p.mode == 1 && p.fallback[qi] != 0) return;   // a list overflowed: the brute-force kernel answers this query
+  if (p.fallback[qi] != 0) {   // a list overflowed, or (mode 0) the query's keys are unbounded: brute force answers it
+    if (p.mode == 0 && tid == 0) p.thr_out[qi] = INFINITY;
+    return;
+  }
   const int32_t* counts = p.counts + (size_t)qi * G;
   const unsigned long long* cand = p.cand + (size_t)qi * G * p.capg;
   // exclusive prefix of the per-CTA survivor counts (G <= blockDim): one element per thread
@@ -403,6 +424,8 @@ __global__ void __launch_bounds__(kSelectThreads, 2) dense_select_kernel(const S
   ra.out_ids = p.out_ids + (size_t)qi * p.k;
   ra.out_scores = p.out_scores + (size_t)qi * p.k;
   ra.out_count = p.out_counts + qi;
+  ra.metric = p.metric;
+  ra.cfac = p.cfac;
   // the staged survivors are dead (the window lives in `top`): their shared memory becomes the query staging area
   rescore_and_emit(top, ntop, P, ek, ei, &qq_s, reinterpret_cast<float*>(keys), ra);
 }
@@ -432,35 +455,37 @@ int encode_map(CUtensorMap* map, const void* ptr, int64_t rows, int64_t cols, in
   return SB_OK;
 }
 
-// ring stages of a QBN-query group: corpus box + query box each, capped by SB_DENSE_STAGES
-int mma_stages(const sb_ctx* ctx, int qbn) {
+// ring stages of a QBN-query group: corpus box + query box each, capped by SB_DENSE_STAGES.  Per query: threshold and
+// count, and for Euclid the query norm r.
+size_t mma_per_query(bool euclid) { return euclid ? 12 : 8; }
+int mma_stages(const sb_ctx* ctx, int qbn, bool euclid = false) {
   const size_t stage = kATileBytes + (size_t)qbn * kBK * 2 + 16;   // + its full / empty barriers
-  const size_t fixed = 1024 + (size_t)qbn * 8;                     // alignment slack + thresholds and counts
+  const size_t fixed = 1024 + (size_t)qbn * mma_per_query(euclid); // alignment slack + per-query values
   return std::min((int)((ctx->smem_optin - fixed) / stage), ctx->dense_max_stages);
 }
-size_t mma_smem(int qbn, int stages) {
-  return 1024 + (size_t)stages * (kATileBytes + (size_t)qbn * kBK * 2 + 16) + (size_t)qbn * 8;
+size_t mma_smem(int qbn, int stages, bool euclid) {
+  return 1024 + (size_t)stages * (kATileBytes + (size_t)qbn * kBK * 2 + 16) + (size_t)qbn * mma_per_query(euclid);
 }
 
-template <int QBN, bool FILTER>
+template <int QBN, bool FILTER, bool EUCLID>
 int launch_mma(const CUtensorMap& tm_rows, const CUtensorMap& tm_q, const MmaScanParams& mp, int grid, size_t smem,
                cudaStream_t st) {
-  auto kern = dense_scan_mma_kernel<QBN, FILTER>;
+  auto kern = dense_scan_mma_kernel<QBN, FILTER, EUCLID>;
   SB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   kern<<<grid, kMmaThreads, smem, st>>>(tm_rows, tm_q, mp);
   SB_CUDA(cudaGetLastError());
   return SB_OK;
 }
 
-template <bool FILTER>
+template <bool FILTER, bool EUCLID>
 int dispatch_mma(int qbn, const CUtensorMap& tm_rows, const CUtensorMap& tm_q, const MmaScanParams& mp, int grid,
                  size_t smem, cudaStream_t st) {
   switch (qbn) {
-    case 16: return launch_mma<16, FILTER>(tm_rows, tm_q, mp, grid, smem, st);
-    case 32: return launch_mma<32, FILTER>(tm_rows, tm_q, mp, grid, smem, st);
-    case 64: return launch_mma<64, FILTER>(tm_rows, tm_q, mp, grid, smem, st);
-    case 128: return launch_mma<128, FILTER>(tm_rows, tm_q, mp, grid, smem, st);
-    case 256: return launch_mma<256, FILTER>(tm_rows, tm_q, mp, grid, smem, st);
+    case 16: return launch_mma<16, FILTER, EUCLID>(tm_rows, tm_q, mp, grid, smem, st);
+    case 32: return launch_mma<32, FILTER, EUCLID>(tm_rows, tm_q, mp, grid, smem, st);
+    case 64: return launch_mma<64, FILTER, EUCLID>(tm_rows, tm_q, mp, grid, smem, st);
+    case 128: return launch_mma<128, FILTER, EUCLID>(tm_rows, tm_q, mp, grid, smem, st);
+    case 256: return launch_mma<256, FILTER, EUCLID>(tm_rows, tm_q, mp, grid, smem, st);
   }
   sb_set_error("dense_mma: unsupported query block %d", qbn);
   return SB_ERR_UNSUPPORTED;
@@ -536,13 +561,19 @@ int dense_mma_topk_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int 
     if (flt) dense_select_kernel<true><<<nblocks, kSelectThreads, sel_smem, st>>>(s);
     else dense_select_kernel<false><<<nblocks, kSelectThreads, sel_smem, st>>>(s);
   };
+  const bool euclid = ix.metric == SB_METRIC_EUCLID;   // Cosine and Dot run the same (acc * scale) kernels
   auto run_mma = [&](int qbn, const CUtensorMap& tm_q, const MmaScanParams& m, int g, size_t smem) {
-    return flt ? dispatch_mma<true>(qbn, tm_rows, tm_q, m, g, smem, st) : dispatch_mma<false>(qbn, tm_rows, tm_q, m, g, smem, st);
+    if (euclid)
+      return flt ? dispatch_mma<true, true>(qbn, tm_rows, tm_q, m, g, smem, st)
+                 : dispatch_mma<false, true>(qbn, tm_rows, tm_q, m, g, smem, st);
+    return flt ? dispatch_mma<true, false>(qbn, tm_rows, tm_q, m, g, smem, st)
+               : dispatch_mma<false, false>(qbn, tm_rows, tm_q, m, g, smem, st);
   };
-  // normalised fp16 operand rows of the whole batch (rows beyond B are zero), eps, cleared fallback flags
-  float* eps = nullptr;
+  // normalised fp16 operand rows of the whole batch (rows beyond B are zero), eps, cleared fallback flags (and r)
+  float *eps = nullptr, *rq = nullptr;
   int32_t* fb = nullptr;
-  if ((rc = dense_prep_queries(ctx, ix, q_pad, B, n_groups * gsz, /*mma=*/true, nullptr, q16, &eps, &fb, st))) return rc;
+  if ((rc = dense_prep_queries(ctx, ix, q_pad, B, n_groups * gsz, /*mma=*/true, nullptr, q16, &eps, &fb, &rq, st)))
+    return rc;
 
   for (int c0 = 0; c0 < B; c0 += gmax * gsz) {
     const int nq_chunk = std::min(B - c0, gmax * gsz);   // real queries of this chunk of groups
@@ -558,8 +589,8 @@ int dense_mma_topk_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int 
       while (G.qbn > 16 && G.qbn / 2 >= left) G.qbn >>= 1;
       G.nq = std::min(G.qbn, left);
       if ((rc = encode_map(&G.tm_q, q16g, G.qbn, ix.d_pad, G.qbn))) return rc;
-      G.stages = mma_stages(ctx, G.qbn);
-      G.smem = mma_smem(G.qbn, G.stages);
+      G.stages = mma_stages(ctx, G.qbn, euclid);
+      G.smem = mma_smem(G.qbn, G.stages, euclid);
       rows_total = g * gsz + G.qbn;
     }
     MmaScanParams mp;
@@ -569,7 +600,10 @@ int dense_mma_topk_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int 
     mp.capg = capg;
     mp.prefetch = ctx->dense_prefetch;
     mp.mask_qs = flt ? flt->qs : 0;
+    mp.hh = ix.hh;
     SelectParams sp;
+    sp.metric = ix.metric;
+    sp.cfac = ix.cfac;
     sp.cand = cand;
     sp.counts = counts;
     sp.capg = capg;
@@ -602,6 +636,7 @@ int dense_mma_topk_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int 
         mp.counts = counts + (size_t)g * gsz * sgrid;
         mp.stages = G.stages;
         mp.mask = flt ? flt->mask + c0 + (size_t)g * gsz : nullptr;
+        mp.rq = rq ? rq + c0 + (size_t)g * gsz : nullptr;
         if ((rc = run_mma(G.qbn, G.tm_q, mp, sgrid, G.smem))) return rc;
       }
       sp.grid = sgrid;
@@ -621,6 +656,7 @@ int dense_mma_topk_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int 
       mp.counts = counts + (size_t)g * gsz * grid;
       mp.stages = G.stages;
       mp.mask = flt ? flt->mask + c0 + (size_t)g * gsz : nullptr;
+      mp.rq = rq ? rq + c0 + (size_t)g * gsz : nullptr;
       ProfScope ps(ctx, SB_PROF_DENSE_SCAN, st);
       if ((rc = run_mma(G.qbn, G.tm_q, mp, grid, G.smem))) return rc;
     }

@@ -21,9 +21,11 @@ bool dense_mma_eligible(const sb_ctx* ctx, const DenseIndex& ix, int B);
 int dense_mma_topk_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int B, int k, int64_t* out_ids,
                            double* out_scores, int32_t* out_counts, cudaStream_t st, const DenseFilter* flt = nullptr);
 
-// dense.cu: normalised fp32 queries / fp16 operand rows / eps / cleared fallback flags for `rows` >= B operand rows
+// dense.cu: normalised fp32 queries / fp16 operand rows / eps / cleared fallback flags for `rows` >= B operand rows, and
+// for a Euclid slot the fp32 query norms r (*rq_out; nullptr for Cosine / Dot).  Flags of Dot / Euclid queries whose
+// keys the scans cannot bound are raised here already (DESIGN.md K1e).
 int dense_prep_queries(sb_ctx* ctx, const DenseIndex& ix, const float* q_pad, int B, int rows, bool mma, float** qn_out,
-                       __half* q16, float** eps_out, int32_t** fb_out, cudaStream_t st);
+                       __half* q16, float** eps_out, int32_t** fb_out, float** rq_out, cudaStream_t st);
 // dense.cu: brute-force fp64 answer for every query whose fallback flag is raised (one CTA per query, idle CTAs exit)
 int dense_fallback_enqueue(sb_ctx* ctx, const DenseIndex& ix, const float* q_pad, int B, int k, const int32_t* fb,
                            int64_t* out_ids, double* out_scores, int32_t* out_counts, cudaStream_t st,

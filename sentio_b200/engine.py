@@ -87,7 +87,15 @@ class B200Engine:
         return C.c_void_p(h if h else 1)
 
     # ------------------------------------------------------------------ K1 dense
-    def load_dense(self, vecs: np.ndarray, id_base: int = 0, slot: int = 0) -> None:
+    METRICS = {"cosine": 0, "dot": 1, "euclid": 2}   # SB_METRIC_* (include/sentio_b200.h)
+
+    def load_dense(self, vecs: np.ndarray, id_base: int = 0, slot: int = 0, metric: str = "cosine") -> None:
+        """``metric``: "cosine" (default), "dot" or "euclid" -- the slot's distance (DESIGN.md K1e); every search,
+        upsert and delete on the slot follows it.  Dot scores are <q, v>, Euclid scores the distance ||q - v||
+        (ascending)."""
+        m = self.METRICS.get(str(metric).lower())
+        if m is None:
+            raise ValueError(f"metric {metric!r} is not supported (cosine, dot or euclid)")
         v = np.ascontiguousarray(vecs)
         if v.ndim != 2:
             raise ValueError("vecs must be [n, d]")
@@ -97,9 +105,21 @@ class B200Engine:
             v = np.ascontiguousarray(v, dtype=np.float32)
             dt = 0
         n, d = v.shape
-        check(self._lib.sb_dense_load(self._h, slot, _ptr(v), n, d, dt, int(id_base)), "sb_dense_load")
+        if m == 0:
+            check(self._lib.sb_dense_load(self._h, slot, _ptr(v), n, d, dt, int(id_base)), "sb_dense_load")
+        else:
+            check(self._lib.sb_dense_load_metric(self._h, slot, _ptr(v), n, d, dt, int(id_base), m),
+                  "sb_dense_load_metric")
         self.dense_dim[slot] = d
         self.dense_count[slot] = n
+
+    def dense_metric(self, slot: int = 0) -> str:
+        """The slot's metric: "cosine", "dot" or "euclid"."""
+        m = int(self._lib.sb_dense_metric(self._h, slot))
+        names = {v: k for k, v in self.METRICS.items()}
+        if m not in names:
+            raise SentioB200Error(f"sb_dense_metric: bad slot {slot}")
+        return names[m]
 
     def dense_set_mode(self, mode: int) -> None:
         """0 = auto, 1 = CUDA-core scan only, 2 = wgmma batched scan whenever eligible."""

@@ -54,6 +54,9 @@ class UpdateResult:
 
 class Distance(enum.Enum):
     COSINE = "Cosine"
+    DOT = "Dot"
+    EUCLID = "Euclid"
+    MANHATTAN = "Manhattan"   # accepted by the parser so it can be refused by name: an L1 distance is not a GEMM
 
 
 @dataclass
@@ -93,6 +96,22 @@ def _distance_name(dist) -> str:
     return str(getattr(dist, "name", dist))
 
 
+def parse_distance(dist) -> Distance:
+    """A Qdrant distance given as this module's ``Distance``, ``qdrant_client``'s ``Distance`` enum (read by ``.name``)
+    or a plain string, case-insensitive ("Cosine", "DOT", "euclid", ...).  Manhattan raises ``ValueError``."""
+    name = _distance_name(dist).strip().lower()
+    for d in Distance:
+        if name in (d.name.lower(), d.value.lower()):
+            if d is Distance.MANHATTAN:
+                raise ValueError("distance Manhattan is not supported: an L1 distance is not a GEMM "
+                                 "(supported: Cosine, Dot, Euclid)")
+            return d
+    raise ValueError(f"distance {_distance_name(dist)!r} is not supported (supported: Cosine, Dot, Euclid)")
+
+
+_ENGINE_METRIC = {Distance.COSINE: "cosine", Distance.DOT: "dot", Distance.EUCLID: "euclid"}
+
+
 class _Collection:
     def __init__(self, name: str, device: int):
         self.name = name
@@ -101,6 +120,7 @@ class _Collection:
         self.payloads: list[dict] = []
         self.row_of: dict[Any, int] = {}
         self.dim = 0
+        self.distance = Distance.COSINE
         self.lock = threading.RLock()
         self._payload_index: PayloadIndex | None = None
 
@@ -148,13 +168,18 @@ class B200VectorStore:
                           vectors_config=None, **_ignored) -> None:
         """Upload a whole collection (brute-force search needs no incremental index), or, with Qdrant's
         ``vectors_config=VectorParams(size, distance)`` and no vectors, create an empty one that ``upsert`` fills.
-        Only the Cosine distance exists here; any other raises ``ValueError``."""
+        The distance is Cosine (the default without ``vectors_config``), Dot or Euclid (Qdrant's semantics: Dot scores
+        <q, v>, Euclid scores the distance ||q - v|| and ranks it ascending); Manhattan raises ``ValueError``."""
+        dist = Distance.COSINE
         if vectors_config is not None:
             if isinstance(vectors_config, dict):
                 raise ValueError("create_collection: named vectors are not supported (one unnamed vector per point)")
-            dist = _distance_name(getattr(vectors_config, "distance", "Cosine"))
-            if dist.lower() != "cosine":
-                raise ValueError(f"create_collection: distance {dist} is not supported (only Cosine)")
+            dist = parse_distance(getattr(vectors_config, "distance", "Cosine"))
+        # an engine lists the metrics its load_dense accepts in METRICS; one without the table loads Cosine only
+        supported = getattr(B200Engine, "METRICS", {"cosine": 0})
+        if _ENGINE_METRIC[dist] not in supported:
+            raise ValueError(f"create_collection: distance {dist.value} is not supported by {B200Engine.__name__} "
+                             f"(it loads {', '.join(sorted(supported))})")
         if vectors is None:
             if vectors_config is None:
                 raise ValueError("create_collection: give vectors or vectors_config")
@@ -162,7 +187,15 @@ class B200VectorStore:
         vecs = np.asarray(vectors)
         n = vecs.shape[0]
         col = _Collection(collection_name, self._device)
-        col.engine.load_dense(vecs, id_base=0, slot=0)
+        col.distance = dist
+        try:
+            if dist is Distance.COSINE:
+                col.engine.load_dense(vecs, id_base=0, slot=0)
+            else:
+                col.engine.load_dense(vecs, id_base=0, slot=0, metric=_ENGINE_METRIC[dist])
+        except BaseException:
+            col.engine.close()
+            raise
         col.ids = list(ids) if ids is not None else [str(i) for i in range(n)]
         col.payloads = list(payloads) if payloads is not None else [{} for _ in range(n)]
         if len(col.ids) != n or len(col.payloads) != n:
@@ -183,7 +216,7 @@ class B200VectorStore:
         col = self._get(collection_name)
         with col.lock:
             return CollectionInfo(points_count=len(col.ids),
-                                  config=CollectionConfig(CollectionParams(VectorParams(col.dim, Distance.COSINE))))
+                                  config=CollectionConfig(CollectionParams(VectorParams(col.dim, col.distance))))
 
     def get_collections(self) -> CollectionsResponse:
         return CollectionsResponse([CollectionDescription(name) for name in list(self._collections)])
@@ -291,7 +324,8 @@ class B200VectorStore:
 
     def retrieve(self, collection_name: str, ids: Sequence[Any], with_payload: bool = True, with_vectors: bool = False,
                  **_ignored) -> list[Record]:
-        """Points by id (unknown ids are skipped, as in Qdrant); vectors are the stored fp16 values, widened."""
+        """Points by id (unknown ids are skipped, as in Qdrant); vectors are the stored fp16 values, widened (Dot /
+        Euclid: c * y, the input to the fp16 precision of its direction; Qdrant would return the input itself)."""
         col = self._get(collection_name)
         with col.lock:
             rows = [col.row_of[i] for i in ids if i in col.row_of]
