@@ -74,7 +74,8 @@ int64_t sb_launch_count(sb_ctx* ctx);
  * Optional per-kernel timing for the roofline leg of bench.py: when enabled every launch of the kernels below is
  * bracketed by a CUDA event pair on the launching stream; sb_profile_read drains the finished pairs of one kernel id
  * (0 dense_scan, 1 dense_merge, 2 bm25_score, 3 bm25_select+final, 4 fuse, 5 cross-encoder forward, 6 dense sampling
- * passes + threshold select, 7 filtered-search match mask, 8 filtered-search gather path) and returns the
+ * passes + threshold select, 7 filtered-search match mask, 8 filtered-search gather path, 9 grouped-search collect,
+ * 10 grouped-search completion assembly) and returns the
  * launch count and the summed device time in milliseconds.
  */
 int sb_profile(sb_ctx* ctx, int enable);
@@ -172,6 +173,27 @@ int sb_dense_topk_filtered_dev(sb_ctx* ctx, int slot, const float* q_dev, int32_
                                const int32_t* f_code_dev, int64_t* out_ids_dev, double* out_scores_dev,
                                int32_t* out_counts_dev, void* stream);
 int64_t sb_dense_fallback_count(sb_ctx* ctx);
+/*
+ * Grouped dense search -- Qdrant's `search_groups(group_by=, limit=L, group_size=G, query_filter=)`: one answer per
+ * document, not per chunk (the reference stamps every chunk with metadata.parent_id, text_splitter.py:143).
+ *
+ * sb_dense_groups: B queries (row-major B x d fp32, host), group field `group_field` (a loaded tag column; code -1 = the
+ * row is in no group and is never returned), 1 <= L <= 1024 groups of 1 <= G <= 1024 hits, and optional conditions as
+ * sb_dense_topk_filtered (f_off == NULL: none).  Over the rows that satisfy query b's conditions, ordered exactly as
+ * sb_dense_topk orders them (score descending, Euclid distance ascending, ties by ascending id): the groups ranked by
+ * their best row, the first min(L, groups) of them, each with its best min(G, rows) rows.  Outputs:
+ * out_n_groups[b]; out_group_code[b*L + g] (-1 past the groups found); out_group_hits[b*L + g];
+ * out_ids[(b*L + g)*G + r] and out_scores[...] (the fp64 scores sb_dense_topk returns for those rows; -1 / 0 past the
+ * hits).  Exact for every input (DESIGN.md K1f): rounds of exact top-K prefixes, exclusion rounds for queries whose
+ * prefix held fewer than L groups, and one filtered top-G per group short of G hits.  Everything is validated before
+ * any launch.  sb_dense_fallback_count includes the inner searches.
+ * sb_dense_group_rounds: hist[r] = grouped queries answered in r + 1 rounds since the context was created (round 1 plus
+ * r exclusion rounds); the last entry also counts every query that took more rounds.
+ */
+int sb_dense_groups(sb_ctx* ctx, int slot, const float* q, int32_t B, int32_t group_field, int32_t L, int32_t G,
+                    const int32_t* f_off, const int32_t* f_field, const int32_t* f_code, int32_t* out_group_code,
+                    int32_t* out_group_hits, int64_t* out_ids, double* out_scores, int32_t* out_n_groups);
+int sb_dense_group_rounds(sb_ctx* ctx, int64_t* hist, int32_t n);
 /*
  * Point upsert / delete in place -- the write half of the Qdrant client (`client.upsert(collection, points=...)`,
  * `client.delete(collection, points_selector=PointIdsList(...))`, reference src/core/vector_store/qdrant_store.py:196-206,

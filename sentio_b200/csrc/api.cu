@@ -96,6 +96,10 @@ void sb_destroy(sb_ctx* ctx) {
   ctx->fb_count_dev.release();
   ctx->filt_dev.release();
   ctx->filt_pin.release();
+  ctx->grp_res_dev.release();
+  ctx->grp_round_dev.release();
+  ctx->grp_q_dev.release();
+  ctx->grp_cmp_dev.release();
   ctx->doc_chars_dev.release();
   ctx->pin_in.release();
   ctx->pin_out.release();

@@ -163,6 +163,9 @@ struct sb_ctx {
   DevBuf fb_count_dev;   // dense: [1] u64, queries answered by the exact fallback kernel (sb_dense_fallback_count)
   DevBuf filt_dev;       // filtered dense: match mask | per-query counts / state | conditions (CSR)
   PinBuf filt_pin;       // filtered dense: host copies of the conditions and the per-query match counts
+  // grouped dense search (sb_dense_groups): result [B][L][G] | one round's prefixes | replicated queries | completions
+  DevBuf grp_res_dev, grp_round_dev, grp_q_dev, grp_cmp_dev;
+  std::vector<int64_t> grp_rounds;   // [r]: grouped queries answered in r + 1 rounds (sb_dense_group_rounds)
   DevBuf doc_chars_dev;  // K7: characters of every document's usable text (0 = blank), sb_doc_chars_load
   int64_t doc_chars_n = 0, doc_chars_base = 0;
   PinBuf pin_in, pin_out;
@@ -188,7 +191,8 @@ struct DeviceGuard {
 // kernel ids for sb_profile_read
 enum { SB_PROF_DENSE_SCAN = 0, SB_PROF_DENSE_MERGE = 1, SB_PROF_BM25_SCORE = 2, SB_PROF_BM25_SELECT = 3,
        SB_PROF_FUSE = 4, SB_PROF_CE = 5, SB_PROF_DENSE_SAMPLE = 6, SB_PROF_DENSE_FILTER = 7,
-       SB_PROF_DENSE_GATHER = 8, SB_PROF_COUNT = 9 };
+       SB_PROF_DENSE_GATHER = 8, SB_PROF_DENSE_GROUP_COLLECT = 9, SB_PROF_DENSE_GROUP_ASSEMBLE = 10,
+       SB_PROF_COUNT = 11 };
 
 static inline cudaEvent_t prof_event(sb_ctx* ctx) {
   if (!ctx->prof_pool.empty()) {

@@ -867,7 +867,27 @@ struct MaskParams {
   int32_t nq, qs;
   uint32_t* mask;               // [n_words][qs]
   int32_t* counts;              // [nq], zeroed by the caller
+  // exclusion mode (grouped search, K1f): x_field >= 0 also requires tags[x_field][row] >= 0 and absent from the query's
+  // codes [x_off[q], x_off[q+1]) of x_code, sorted ascending.  x_field = -1: off.
+  int32_t x_field;
+  const int32_t* x_off;         // [nq + 1] (absolute offsets into x_code)
+  const int32_t* x_code;
 };
+
+// true iff v is one of the n ascending codes at a
+__device__ __forceinline__ bool sorted_codes_contain(const int32_t* __restrict__ a, int n, int32_t v) {
+  int lo = 0, len = n;
+  while (len > 0) {
+    const int h = len >> 1;
+    if (__ldg(a + lo + h) < v) {
+      lo += h + 1;
+      len -= h + 1;
+    } else {
+      len = h;
+    }
+  }
+  return lo < n && __ldg(a + lo) == v;
+}
 
 __global__ void __launch_bounds__(256) dense_filter_mask_kernel(const MaskParams p) {
   const int lane = threadIdx.x & 31;
@@ -889,6 +909,11 @@ __global__ void __launch_bounds__(256) dense_filter_mask_kernel(const MaskParams
         for (int i = __ldg(p.f_off + q); i < e && m; ++i) {
           const int32_t code = __ldg(p.f_code + i);
           m = code >= 0 && __ldg(p.tags[__ldg(p.f_field + i)] + row) == code;
+        }
+        if (m && p.x_field >= 0) {
+          const int32_t g = __ldg(p.tags[p.x_field] + row);
+          const int x0 = __ldg(p.x_off + q);
+          m = g >= 0 && !sorted_codes_contain(p.x_code + x0, __ldg(p.x_off + q + 1) - x0, g);
         }
         const uint32_t bits = __ballot_sync(0xffffffffu, m);
         if (lane == j) mine = bits;
@@ -956,6 +981,133 @@ __global__ void __launch_bounds__(kMergeThreads, 1) dense_filter_gather_kernel(c
   ra.metric = p.metric;
   ra.cfac = p.cfac;
   rescore_and_emit(sel, nsel, P, ek, ei, &qq_s, q_s, ra);
+}
+
+// ------------------------------------------------------------------------------------------------ grouped search (K1f)
+constexpr int kGroupThreads = 1024;   // >= the longest round prefix (kDenseMaxK)
+
+struct GroupCollectParams {
+  const int64_t* ids;       // [nq][K] one round's exact prefix, best first (id_base + row)
+  const double* scores;     // [nq][K]
+  const int32_t* counts;    // [nq] prefix length (= K: the prefix is full)
+  const int32_t* qmap;      // [nq] grouped query of each round query; nullptr = the identity
+  const int32_t* tag;       // the group_by tag column
+  int64_t id_base;
+  int32_t K, L, G;
+  int32_t* n_groups;        // [B] groups found so far
+  int32_t* g_code;          // [B][L] group codes, in order of their best row
+  int32_t* g_hits;          // [B][L] hits recorded per group (<= G)
+  int64_t* h_ids;           // [B][L][G]
+  double* h_scores;         // [B][L][G]
+};
+
+// One CTA per round query; thread t owns prefix position t.  Sorting the (code, position) pairs gives every position its
+// rank inside its group, its group's first position and the group's count in the prefix; an exclusive scan over "first
+// position of its group" numbers the groups in the order of their best row.  A round's groups are all new (an exclusion
+// round excludes the groups found before it), so they are numbered on from n_groups.  A position is recorded iff its
+// group number is < L and its rank < G.
+__global__ void __launch_bounds__(kGroupThreads) dense_group_collect_kernel(const GroupCollectParams p) {
+  __shared__ unsigned long long key[kGroupThreads];
+  __shared__ int rank_of[kGroupThreads], first_of[kGroupThreads], run_of[kGroupThreads], ord[kGroupThreads];
+  __shared__ int warp_sum[kGroupThreads / 32];
+  const int qi = blockIdx.x, t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  const int b = p.qmap ? p.qmap[qi] : qi;
+  const int cnt = p.counts[qi];
+  const int base = p.n_groups[b];
+  const int64_t* ids = p.ids + (size_t)qi * p.K;
+  int32_t code = -1;
+  if (t < cnt) code = __ldg(p.tag + (ids[t] - p.id_base));
+  // (code, position) ascending, rows without a group last: sorted descending as complements (0 = no group)
+  key[t] = code >= 0 ? ~(((unsigned long long)(uint32_t)code << 32) | (uint32_t)t) : 0ull;
+  rank_of[t] = -1;
+  __syncthreads();
+  int P = 32;
+  while (P < cnt) P <<= 1;
+  block_sort_desc_u64(key, P, t, kGroupThreads);
+  if (t < P && key[t] != 0ull) {
+    const uint32_t c = (uint32_t)(~key[t] >> 32);
+    int lo = 0, hi = t;   // first sorted position of code c
+    while (lo < hi) {
+      const int m = (lo + hi) >> 1;
+      if ((uint32_t)(~key[m] >> 32) < c) lo = m + 1;
+      else hi = m;
+    }
+    int lo2 = t + 1, hi2 = P;   // first sorted position past code c (a complemented 0 reads as code 0xffffffff)
+    while (lo2 < hi2) {
+      const int m = (lo2 + hi2) >> 1;
+      if ((uint32_t)(~key[m] >> 32) <= c) lo2 = m + 1;
+      else hi2 = m;
+    }
+    const int pos = (int)(uint32_t)~key[t];
+    rank_of[pos] = t - lo;
+    first_of[pos] = (int)(uint32_t)~key[lo];
+    run_of[pos] = lo2 - lo;
+  }
+  __syncthreads();
+  const int flag = (t < cnt && rank_of[t] == 0) ? 1 : 0;
+  int incl = flag;
+  for (int o = 1; o < 32; o <<= 1) {
+    const int y = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl += y;
+  }
+  if (lane == 31) warp_sum[warp] = incl;
+  __syncthreads();
+  if (warp == 0) {
+    int v = warp_sum[lane];
+    for (int o = 1; o < 32; o <<= 1) {
+      const int y = __shfl_up_sync(0xffffffffu, v, o);
+      if (lane >= o) v += y;
+    }
+    warp_sum[lane] = v;
+  }
+  __syncthreads();
+  ord[t] = incl - flag + (warp ? warp_sum[warp - 1] : 0);
+  __syncthreads();
+  if (t < cnt && rank_of[t] >= 0) {
+    const int g = base + ord[first_of[t]];
+    const int r = rank_of[t];
+    if (g < p.L && r < p.G) {
+      const size_t h = ((size_t)b * p.L + g) * p.G + r;
+      p.h_ids[h] = ids[t];
+      p.h_scores[h] = p.scores[(size_t)qi * p.K + t];
+      if (r == 0) {
+        p.g_code[(size_t)b * p.L + g] = code;
+        p.g_hits[(size_t)b * p.L + g] = min(run_of[t], p.G);
+      }
+    }
+  }
+  if (t == 0) p.n_groups[b] = min(p.L, base + warp_sum[31]);
+}
+
+// out[r] = q_pad[src[r]]: one operand row per round query or completion pair
+__global__ void __launch_bounds__(256) dense_group_queries_kernel(const float* __restrict__ q_pad,
+                                                                  const int32_t* __restrict__ src, int d_pad,
+                                                                  float* __restrict__ out) {
+  const float* s = q_pad + (size_t)src[blockIdx.x] * d_pad;
+  for (int i = threadIdx.x; i < d_pad; i += blockDim.x) out[(size_t)blockIdx.x * d_pad + i] = s[i];
+}
+
+// A completion's top-G of one group (filtered search, [np][G]) replaces that group's hits: pair i -> group dest[i]
+struct GroupAssembleParams {
+  const int64_t* ids;
+  const double* scores;
+  const int32_t* counts;
+  const int32_t* dest;      // [np] b * L + g
+  int32_t G;
+  int64_t n;                // np * G
+  int32_t* g_hits;
+  int64_t* h_ids;
+  double* h_scores;
+};
+
+__global__ void __launch_bounds__(256) dense_group_assemble_kernel(const GroupAssembleParams p) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= p.n) return;
+  const int64_t pr = i / p.G, r = i % p.G;
+  const int32_t g = p.dest[pr];
+  p.h_ids[(size_t)g * p.G + r] = p.ids[i];
+  p.h_scores[(size_t)g * p.G + r] = p.scores[i];
+  if (r == 0) p.g_hits[g] = p.counts[pr];
 }
 
 // ------------------------------------------------------------------------------------------------ host side
@@ -1257,10 +1409,12 @@ namespace {
 
 // Filtered top-k of B queries (q_pad on the device; conditions as host CSR arrays) in chunks of <= 256 queries: per
 // chunk the match mask + match counts, one wait for the counts, then the gather path for low-cardinality queries and
-// the masked scans for the rest.
+// the masked scans for the rest.  x_field >= 0 adds the exclusion mode of the mask (MaskParams; host CSR x_off / x_code):
+// every query is then filtered.
 int dense_topk_filtered_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int B, int k, const int32_t* f_off,
                                 const int32_t* f_field, const int32_t* f_code, int64_t* out_ids, double* out_scores,
-                                int32_t* out_counts, cudaStream_t st) {
+                                int32_t* out_counts, cudaStream_t st, int x_field = -1, const int32_t* x_off = nullptr,
+                                const int32_t* x_code = nullptr) {
   SB_REQUIRE(k <= kDenseMaxK, SB_ERR_UNSUPPORTED, "dense: top_k %d too large (max %d per call)", k, kDenseMaxK);
   SB_REQUIRE(f_off[0] == 0, SB_ERR_ARG, "sb_dense_topk_filtered: f_off[0] must be 0");
   for (int b = 0; b < B; ++b)
@@ -1271,16 +1425,21 @@ int dense_topk_filtered_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad,
     SB_REQUIRE(f >= 0 && f < SB_MAX_TAG_FIELDS, SB_ERR_ARG, "sb_dense_topk_filtered: field %d out of range", f);
     SB_REQUIRE(ix.tags[f] != nullptr, SB_ERR_STATE, "sb_dense_topk_filtered: field %d has no tag column loaded", f);
   }
-  if (n_conds == 0)   // no query has a condition: exactly the unfiltered search
+  const bool excl = x_field >= 0;
+  if (n_conds == 0 && !excl)   // no query has a condition: exactly the unfiltered search
     return dense_topk_enqueue(ctx, ix, q_pad, B, k, out_ids, out_scores, out_counts, st);
+  const int n_x = excl ? x_off[B] : 0;
 
   const int64_t n_words = ix.n_pad / 32;
   int qchunk = 256;   // queries per mask; the mask (n_pad * qchunk / 8 bytes) is kept under 1 GB
   while (qchunk > 32 && (size_t)n_words * 4 * qchunk > (1ull << 30)) qchunk >>= 1;
-  // device: tag pointers | f_off | f_field | f_code | counts [qchunk] | state [qchunk] | qlist [qchunk] | mask
+  // device: tag pointers | f_off | f_field | f_code | x_off | x_code | counts [qchunk] | state [qchunk] | qlist [qchunk] |
+  // mask
   const size_t o_off = 128, o_field = o_off + ((size_t)(B + 1) * 4 + 15) / 16 * 16;
   const size_t o_code = o_field + ((size_t)n_conds * 4 + 15) / 16 * 16;
-  const size_t o_cnt = o_code + ((size_t)n_conds * 4 + 15) / 16 * 16;
+  const size_t o_xoff = o_code + ((size_t)n_conds * 4 + 15) / 16 * 16;
+  const size_t o_xcode = o_xoff + (excl ? ((size_t)(B + 1) * 4 + 15) / 16 * 16 : 0);
+  const size_t o_cnt = o_xcode + ((size_t)n_x * 4 + 15) / 16 * 16;
   const size_t o_state = o_cnt + (size_t)qchunk * 4, o_qlist = o_state + (size_t)qchunk * 4;
   const size_t o_mask = (o_qlist + (size_t)qchunk * 4 + 255) / 256 * 256;
   const size_t dev_bytes = o_mask + (size_t)n_words * qchunk * 4;
@@ -1294,6 +1453,10 @@ int dense_topk_filtered_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad,
   memcpy(hp + o_off, f_off, (size_t)(B + 1) * 4);
   memcpy(hp + o_field, f_field, (size_t)n_conds * 4);
   memcpy(hp + o_code, f_code, (size_t)n_conds * 4);
+  if (excl) {
+    memcpy(hp + o_xoff, x_off, (size_t)(B + 1) * 4);
+    memcpy(hp + o_xcode, x_code, (size_t)n_x * 4);
+  }
   SB_CUDA(cudaMemcpyAsync(dv, hp, o_cnt, cudaMemcpyHostToDevice, st));
   int32_t* cnt_h = reinterpret_cast<int32_t*>(hp + o_cnt);
   int32_t* state_h = reinterpret_cast<int32_t*>(hp + o_state);
@@ -1320,6 +1483,9 @@ int dense_topk_filtered_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad,
     mk.qs = qs;
     mk.mask = mask;
     mk.counts = cnt_d;
+    mk.x_field = x_field;
+    mk.x_off = excl ? reinterpret_cast<const int32_t*>(dv + o_xoff) + c0 : nullptr;
+    mk.x_code = excl ? reinterpret_cast<const int32_t*>(dv + o_xcode) : nullptr;
     const int64_t blocks = std::min<int64_t>((n_words + 7) / 8, (int64_t)ctx->num_sms * 8);
     {
       ProfScope ps(ctx, SB_PROF_DENSE_FILTER, st);
@@ -1333,7 +1499,7 @@ int dense_topk_filtered_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad,
     int n_gather = 0;
     int64_t c_min = ix.n;
     for (int q = 0; q < nq; ++q) {
-      const bool filtered = f_off[c0 + q + 1] > f_off[c0 + q];
+      const bool filtered = excl || f_off[c0 + q + 1] > f_off[c0 + q];
       const bool gather = filtered && cnt_h[q] <= kGatherMax;
       state_h[q] = gather ? 1 : 0;
       if (gather) qlist_h[n_gather++] = q;
@@ -1375,6 +1541,189 @@ int dense_topk_filtered_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad,
       if ((rc = dense_topk_enqueue(ctx, ix, qc, nq, k, oi, os, oc, st, &flt))) return rc;
     }
   }
+  return SB_OK;
+}
+
+size_t align16(size_t v) { return (v + 15) / 16 * 16; }
+
+// Grouped search of B padded queries (DESIGN.md K1f) into ctx->grp_res_dev, laid out n_groups [B] | g_code [B][L] |
+// g_hits [B][L] | h_ids [B][L][G] | h_scores [B][L][G] (offsets in *o).  Every step consumes an exact ordered prefix:
+//   round 1      the exact top-K of the rows matching the query's conditions;
+//   exclusion    while a query's prefix was full and it has fewer than L groups: the exact top-K of its matching rows
+//                that have a group not found yet -- their first groups are the next groups in the ranking;
+//   completion   a group found with fewer than G hits in a full prefix: the top-G of "conditions and group_by == code".
+// f_off == nullptr: no conditions.  Inputs are validated by the caller.
+struct GroupLayout {
+  size_t n_groups, g_code, g_hits, h_ids, h_scores, total;
+};
+
+int dense_groups_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int B, int gf, int L, int G,
+                         const int32_t* f_off, const int32_t* f_field, const int32_t* f_code, GroupLayout* o,
+                         cudaStream_t st) {
+  const int K = std::min(kDenseMaxK, std::max(128, 4 * L * G));
+  const size_t BL = (size_t)B * L, BLG = BL * G;
+  o->n_groups = 0;
+  o->g_code = align16((size_t)B * 4);
+  o->g_hits = o->g_code + align16(BL * 4);
+  o->h_ids = o->g_hits + align16(BL * 4);
+  o->h_scores = o->h_ids + BLG * 8;
+  o->total = o->h_scores + BLG * 8;
+  int rc;
+  if ((rc = ctx->grp_res_dev.reserve(o->total))) return rc;
+  uint8_t* res = ctx->grp_res_dev.as<uint8_t>();
+  int32_t* n_groups = reinterpret_cast<int32_t*>(res + o->n_groups);
+  int32_t* g_code = reinterpret_cast<int32_t*>(res + o->g_code);
+  int32_t* g_hits = reinterpret_cast<int32_t*>(res + o->g_hits);
+  int64_t* h_ids = reinterpret_cast<int64_t*>(res + o->h_ids);
+  double* h_scores = reinterpret_cast<double*>(res + o->h_scores);
+  SB_CUDA(cudaMemsetAsync(n_groups, 0, (size_t)B * 4, st));
+  SB_CUDA(cudaMemsetAsync(g_code, 0xff, BL * 4, st));
+  SB_CUDA(cudaMemsetAsync(g_hits, 0, BL * 4, st));
+  SB_CUDA(cudaMemsetAsync(h_ids, 0xff, BLG * 8, st));
+  SB_CUDA(cudaMemsetAsync(h_scores, 0, BLG * 8, st));
+  // one round: prefixes ids [B][K] | scores [B][K] | counts [B] | qmap [B]
+  const size_t r_sc = (size_t)B * K * 8, r_cnt = r_sc + (size_t)B * K * 8, r_map = r_cnt + align16((size_t)B * 4);
+  if ((rc = ctx->grp_round_dev.reserve(r_map + (size_t)B * 4))) return rc;
+  uint8_t* rd = ctx->grp_round_dev.as<uint8_t>();
+  int64_t* rids = reinterpret_cast<int64_t*>(rd);
+  double* rsc = reinterpret_cast<double*>(rd + r_sc);
+  int32_t* rcnt = reinterpret_cast<int32_t*>(rd + r_cnt);
+  int32_t* rmap = reinterpret_cast<int32_t*>(rd + r_map);
+  const int32_t* tag = ix.tags[gf];
+
+  GroupCollectParams cp;
+  cp.ids = rids;
+  cp.scores = rsc;
+  cp.counts = rcnt;
+  cp.tag = tag;
+  cp.id_base = ix.id_base;
+  cp.K = K;
+  cp.L = L;
+  cp.G = G;
+  cp.n_groups = n_groups;
+  cp.g_code = g_code;
+  cp.g_hits = g_hits;
+  cp.h_ids = h_ids;
+  cp.h_scores = h_scores;
+
+  std::vector<int32_t> qmap(B), cnt_h(B), ng_h(B), prev(B, 0), rounds(B, 1), code_h(BL), hits_h(BL);
+  for (int b = 0; b < B; ++b) qmap[b] = b;
+  std::vector<int32_t> incomplete;   // b * L + g
+  auto no_conds = [&](int b) { return f_off == nullptr || f_off[b + 1] == f_off[b]; };
+  int nq = B;
+  for (int round = 0; nq > 0; ++round) {
+    if (round == 0) {
+      if (f_off == nullptr) rc = dense_topk_enqueue(ctx, ix, q_pad, B, K, rids, rsc, rcnt, st);
+      else rc = dense_topk_filtered_enqueue(ctx, ix, q_pad, B, K, f_off, f_field, f_code, rids, rsc, rcnt, st);
+      if (rc) return rc;
+      cp.qmap = nullptr;
+    } else {
+      // the short queries' conditions, and their groups found so far (ascending) as the exclusion list
+      std::vector<int32_t> off(nq + 1, 0), fld, code, xoff(nq + 1, 0), xcode;
+      for (int i = 0; i < nq; ++i) {
+        const int b = qmap[i];
+        if (!no_conds(b))
+          for (int j = f_off[b]; j < f_off[b + 1]; ++j) {
+            fld.push_back(f_field[j]);
+            code.push_back(f_code[j]);
+          }
+        off[i + 1] = (int32_t)fld.size();
+        const size_t x0 = xcode.size();
+        xcode.insert(xcode.end(), code_h.begin() + (size_t)b * L, code_h.begin() + (size_t)b * L + ng_h[b]);
+        std::sort(xcode.begin() + x0, xcode.end());
+        xoff[i + 1] = (int32_t)xcode.size();
+      }
+      if ((rc = ctx->grp_q_dev.reserve((size_t)nq * ix.d_pad * 4))) return rc;
+      float* qr = ctx->grp_q_dev.as<float>();
+      SB_CUDA(cudaMemcpyAsync(rmap, qmap.data(), (size_t)nq * 4, cudaMemcpyHostToDevice, st));
+      ctx->launches += 1;
+      dense_group_queries_kernel<<<nq, 256, 0, st>>>(q_pad, rmap, ix.d_pad, qr);
+      SB_CUDA(cudaGetLastError());
+      if ((rc = dense_topk_filtered_enqueue(ctx, ix, qr, nq, K, off.data(), fld.data(), code.data(), rids, rsc, rcnt, st,
+                                            gf, xoff.data(), xcode.data())))
+        return rc;
+      cp.qmap = rmap;
+    }
+    {
+      ProfScope ps(ctx, SB_PROF_DENSE_GROUP_COLLECT, st);
+      dense_group_collect_kernel<<<nq, kGroupThreads, 0, st>>>(cp);
+    }
+    SB_CUDA(cudaGetLastError());
+    SB_CUDA(cudaMemcpyAsync(cnt_h.data(), rcnt, (size_t)nq * 4, cudaMemcpyDeviceToHost, st));
+    SB_CUDA(cudaMemcpyAsync(ng_h.data(), n_groups, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
+    SB_CUDA(cudaMemcpyAsync(code_h.data(), g_code, BL * 4, cudaMemcpyDeviceToHost, st));
+    SB_CUDA(cudaMemcpyAsync(hits_h.data(), g_hits, BL * 4, cudaMemcpyDeviceToHost, st));
+    SB_CUDA(cudaStreamSynchronize(st));
+    // a full prefix proves nothing past its end: its groups short of G hits need completion, and a query short of L
+    // groups goes on to an exclusion round.  A prefix that is not full held every remaining matching row.
+    int next = 0;
+    for (int i = 0; i < nq; ++i) {
+      const int b = qmap[i];
+      if (cnt_h[i] < K) continue;
+      for (int g = prev[b]; g < ng_h[b]; ++g)
+        if (hits_h[(size_t)b * L + g] < G) incomplete.push_back((int32_t)((size_t)b * L + g));
+      prev[b] = ng_h[b];
+      if (ng_h[b] < L) {
+        qmap[next++] = b;
+        rounds[b] += 1;
+      }
+    }
+    nq = next;
+  }
+  for (int b = 0; b < B; ++b) {
+    const size_t r = (size_t)rounds[b] - 1;
+    if (ctx->grp_rounds.size() <= r) ctx->grp_rounds.resize(r + 1, 0);
+    ctx->grp_rounds[r] += 1;
+  }
+
+  const int np = (int)incomplete.size();
+  if (np == 0) return SB_OK;
+  std::vector<int32_t> src(np), off(np + 1, 0), fld, code;
+  for (int i = 0; i < np; ++i) {
+    const int b = incomplete[i] / L;
+    src[i] = b;
+    if (!no_conds(b))
+      for (int j = f_off[b]; j < f_off[b + 1]; ++j) {
+        fld.push_back(f_field[j]);
+        code.push_back(f_code[j]);
+      }
+    fld.push_back(gf);
+    code.push_back(code_h[incomplete[i]]);
+    off[i + 1] = (int32_t)fld.size();
+  }
+  // completions: ids [np][G] | scores [np][G] | counts [np] | src [np] | dest [np]
+  const size_t c_sc = (size_t)np * G * 8, c_cnt = c_sc + (size_t)np * G * 8, c_src = c_cnt + align16((size_t)np * 4);
+  const size_t c_dst = c_src + align16((size_t)np * 4);
+  if ((rc = ctx->grp_cmp_dev.reserve(c_dst + (size_t)np * 4))) return rc;
+  if ((rc = ctx->grp_q_dev.reserve((size_t)np * ix.d_pad * 4))) return rc;
+  uint8_t* cd = ctx->grp_cmp_dev.as<uint8_t>();
+  int32_t* src_d = reinterpret_cast<int32_t*>(cd + c_src);
+  int32_t* dst_d = reinterpret_cast<int32_t*>(cd + c_dst);
+  float* qr = ctx->grp_q_dev.as<float>();
+  SB_CUDA(cudaMemcpyAsync(src_d, src.data(), (size_t)np * 4, cudaMemcpyHostToDevice, st));
+  SB_CUDA(cudaMemcpyAsync(dst_d, incomplete.data(), (size_t)np * 4, cudaMemcpyHostToDevice, st));
+  ctx->launches += 1;
+  dense_group_queries_kernel<<<np, 256, 0, st>>>(q_pad, src_d, ix.d_pad, qr);
+  SB_CUDA(cudaGetLastError());
+  GroupAssembleParams ap;
+  ap.ids = reinterpret_cast<int64_t*>(cd);
+  ap.scores = reinterpret_cast<double*>(cd + c_sc);
+  ap.counts = reinterpret_cast<int32_t*>(cd + c_cnt);
+  if ((rc = dense_topk_filtered_enqueue(ctx, ix, qr, np, G, off.data(), fld.data(), code.data(),
+                                        const_cast<int64_t*>(ap.ids), const_cast<double*>(ap.scores),
+                                        const_cast<int32_t*>(ap.counts), st)))
+    return rc;
+  ap.dest = dst_d;
+  ap.G = G;
+  ap.n = (int64_t)np * G;
+  ap.g_hits = g_hits;
+  ap.h_ids = h_ids;
+  ap.h_scores = h_scores;
+  {
+    ProfScope ps(ctx, SB_PROF_DENSE_GROUP_ASSEMBLE, st);
+    dense_group_assemble_kernel<<<(unsigned)((ap.n + 255) / 256), 256, 0, st>>>(ap);
+  }
+  SB_CUDA(cudaGetLastError());
   return SB_OK;
 }
 
@@ -1961,6 +2310,74 @@ int sb_dense_topk_filtered(sb_ctx* ctx, int slot, const float* q, int32_t B, int
   SB_CUDA(cudaMemcpyAsync(out_scores, ctx->out_sc_dev.p, nid * 8, cudaMemcpyDeviceToHost, st));
   SB_CUDA(cudaMemcpyAsync(out_counts, ctx->out_cnt_dev.p, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
   SB_CUDA(cudaStreamSynchronize(st));
+  return SB_OK;
+}
+
+int sb_dense_groups(sb_ctx* ctx, int slot, const float* q, int32_t B, int32_t group_field, int32_t L, int32_t G,
+                    const int32_t* f_off, const int32_t* f_field, const int32_t* f_code, int32_t* out_group_code,
+                    int32_t* out_group_hits, int64_t* out_ids, double* out_scores, int32_t* out_n_groups) {
+  SB_REQUIRE(ctx != nullptr, SB_ERR_ARG, "sb_dense_groups: ctx is NULL");
+  SB_REQUIRE(slot >= 0 && slot < SB_MAX_DENSE_SLOTS, SB_ERR_ARG, "sb_dense_groups: bad slot %d", slot);
+  SB_REQUIRE(B >= 0, SB_ERR_ARG, "sb_dense_groups: bad B=%d", B);
+  SB_REQUIRE(L >= 1 && L <= kDenseMaxK && G >= 1 && G <= kDenseMaxK, SB_ERR_ARG,
+             "sb_dense_groups: limit %d and group_size %d must be in [1, %d]", L, G, kDenseMaxK);
+  SB_REQUIRE(group_field >= 0 && group_field < SB_MAX_TAG_FIELDS, SB_ERR_ARG,
+             "sb_dense_groups: group field %d out of range [0,%d)", group_field, SB_MAX_TAG_FIELDS);
+  if (B == 0) return SB_OK;
+  SB_REQUIRE(q && out_group_code && out_group_hits && out_ids && out_scores && out_n_groups, SB_ERR_ARG,
+             "sb_dense_groups: NULL buffer");
+  int n_conds = 0;
+  if (f_off) {
+    SB_REQUIRE(f_off[0] == 0, SB_ERR_ARG, "sb_dense_groups: f_off[0] must be 0");
+    for (int b = 0; b < B; ++b)
+      SB_REQUIRE(f_off[b + 1] >= f_off[b], SB_ERR_ARG, "sb_dense_groups: f_off is not non-decreasing at %d", b);
+    n_conds = f_off[B];
+    SB_REQUIRE(n_conds == 0 || (f_field && f_code), SB_ERR_ARG, "sb_dense_groups: NULL conditions");
+    for (int i = 0; i < n_conds; ++i)
+      SB_REQUIRE(f_field[i] >= 0 && f_field[i] < SB_MAX_TAG_FIELDS, SB_ERR_ARG, "sb_dense_groups: field %d out of range",
+                 f_field[i]);
+  }
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  DeviceGuard g(ctx->device);
+  cudaStream_t st = ctx->stream;
+  DenseIndex& ix = ctx->dense[slot];
+  SB_REQUIRE(ix.d > 0, SB_ERR_STATE, "sb_dense_groups: dense slot %d has no index loaded", slot);
+  SB_REQUIRE(ix.tags[group_field] != nullptr, SB_ERR_STATE, "sb_dense_groups: field %d has no tag column loaded",
+             group_field);
+  for (int i = 0; i < n_conds; ++i)
+    SB_REQUIRE(ix.tags[f_field[i]] != nullptr, SB_ERR_STATE, "sb_dense_groups: field %d has no tag column loaded",
+               f_field[i]);
+  const size_t BL = (size_t)B * L, BLG = BL * G;
+  if (ix.n == 0) {
+    for (int b = 0; b < B; ++b) out_n_groups[b] = 0;
+    for (size_t i = 0; i < BL; ++i) { out_group_code[i] = -1; out_group_hits[i] = 0; }
+    for (size_t i = 0; i < BLG; ++i) { out_ids[i] = -1; out_scores[i] = 0.0; }
+    return SB_OK;
+  }
+  int rc;
+  const size_t qbytes = (size_t)B * ix.d * sizeof(float);
+  if ((rc = ctx->pin_in.reserve(qbytes))) return rc;
+  SB_CUDA(cudaStreamSynchronize(st));
+  memcpy(ctx->pin_in.p, q, qbytes);
+  float* q_pad = nullptr;
+  if ((rc = sb_dense_pad_queries(ctx, ix, ctx->pin_in.as<float>(), B, false, &q_pad, st))) return rc;
+  GroupLayout o;
+  if ((rc = dense_groups_enqueue(ctx, ix, q_pad, B, group_field, L, G, f_off, f_field, f_code, &o, st))) return rc;
+  const uint8_t* res = ctx->grp_res_dev.as<uint8_t>();
+  SB_CUDA(cudaMemcpyAsync(out_n_groups, res + o.n_groups, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
+  SB_CUDA(cudaMemcpyAsync(out_group_code, res + o.g_code, BL * 4, cudaMemcpyDeviceToHost, st));
+  SB_CUDA(cudaMemcpyAsync(out_group_hits, res + o.g_hits, BL * 4, cudaMemcpyDeviceToHost, st));
+  SB_CUDA(cudaMemcpyAsync(out_ids, res + o.h_ids, BLG * 8, cudaMemcpyDeviceToHost, st));
+  SB_CUDA(cudaMemcpyAsync(out_scores, res + o.h_scores, BLG * 8, cudaMemcpyDeviceToHost, st));
+  SB_CUDA(cudaStreamSynchronize(st));
+  return SB_OK;
+}
+
+int sb_dense_group_rounds(sb_ctx* ctx, int64_t* hist, int32_t n) {
+  SB_REQUIRE(ctx != nullptr && n >= 0 && (n == 0 || hist != nullptr), SB_ERR_ARG, "sb_dense_group_rounds: bad arguments");
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  for (int i = 0; i < n; ++i) hist[i] = 0;
+  for (size_t r = 0; r < ctx->grp_rounds.size() && n > 0; ++r) hist[std::min<size_t>(r, (size_t)n - 1)] += ctx->grp_rounds[r];
   return SB_OK;
 }
 

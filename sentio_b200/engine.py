@@ -68,7 +68,7 @@ class B200Engine:
         return int(self._lib.sb_launch_count(self._h))
 
     PROF_IDS = {"dense_scan": 0, "dense_merge": 1, "bm25_score": 2, "bm25_select": 3, "fuse": 4, "ce": 5, "dense_sample": 6,
-                "dense_filter_mask": 7, "dense_filter_gather": 8}
+                "dense_filter_mask": 7, "dense_filter_gather": 8, "dense_group_collect": 9, "dense_group_assemble": 10}
 
     def profile(self, enable: bool) -> None:
         check(self._lib.sb_profile(self._h, 1 if enable else 0), "sb_profile")
@@ -226,6 +226,42 @@ class B200Engine:
         check(self._lib.sb_dense_topk_filtered(self._h, slot, _ptr(q), B, k, _ptr(off), _ptr(fld), _ptr(code), _ptr(ids),
                                                _ptr(sc), _ptr(cnt)), "sb_dense_topk_filtered")
         return ids, sc, cnt
+
+    def dense_groups(self, q: np.ndarray, field: int, limit: int, group_size: int, filters=None, slot: int = 0):
+        """Grouped search (``sb_dense_groups``, DESIGN.md K1f): per query the best ``limit`` groups of tag column ``field``
+        (groups ranked by their best row, rows with code -1 in no group), each with its best ``group_size`` rows, over
+        the rows matching ``filters`` (CSR conditions as ``dense_topk``; None = all rows).  Returns (n_groups [B] int32,
+        group codes [B, limit] int32 (-1 past n_groups), hits [B, limit] int32, ids [B, limit, group_size] int64 (-1 past
+        the hits), scores [B, limit, group_size] float64)."""
+        q = np.ascontiguousarray(np.atleast_2d(q), dtype=np.float32)
+        B, d = q.shape
+        if slot not in self.dense_dim:
+            raise SentioB200Error(f"dense slot {slot} has no index loaded")
+        if d != self.dense_dim[slot]:
+            raise ValueError(f"query dimension {d} != index dimension {self.dense_dim[slot]}")
+        L, G = int(limit), int(group_size)
+        if not (1 <= L <= 1024 and 1 <= G <= 1024):
+            raise ValueError(f"limit {L} and group_size {G} must be in [1, 1024]")
+        off = fld = code = None
+        if filters is not None:
+            off, fld, code = (np.ascontiguousarray(a, dtype=np.int32).reshape(-1) for a in filters)
+            if len(off) != B + 1 or len(fld) != len(code) or int(off[-1]) != len(fld):
+                raise ValueError("filters must be CSR (f_off [B+1], f_field [n], f_code [n]) with f_off[B] == n")
+        ng = np.empty(B, dtype=np.int32)
+        gc = np.empty((B, L), dtype=np.int32)
+        gh = np.empty((B, L), dtype=np.int32)
+        ids = np.empty((B, L, G), dtype=np.int64)
+        sc = np.empty((B, L, G), dtype=np.float64)
+        check(self._lib.sb_dense_groups(self._h, slot, _ptr(q), B, int(field), L, G, _ptr(off), _ptr(fld), _ptr(code),
+                                        _ptr(gc), _ptr(gh), _ptr(ids), _ptr(sc), _ptr(ng)), "sb_dense_groups")
+        return ng, gc, gh, ids, sc
+
+    def dense_group_rounds(self, n: int = 8) -> np.ndarray:
+        """Histogram of rounds per grouped query since the engine was created: [r] = queries answered in r + 1 rounds
+        (the last bucket also counts every query that took more)."""
+        h = np.zeros(int(n), dtype=np.int64)
+        check(self._lib.sb_dense_group_rounds(self._h, _ptr(h), int(n)), "sb_dense_group_rounds")
+        return h
 
     def dense_topk_dev(self, q_t, k: int, slot: int = 0, out=None, filters=None):
         """``filters`` = (f_off [B+1], f_field, f_code) int32 CUDA tensors, or None (unfiltered)."""

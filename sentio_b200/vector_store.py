@@ -28,7 +28,8 @@ import numpy as np
 from .engine import B200Engine
 from .payload_filter import PayloadIndex
 
-__all__ = ["B200VectorStore", "ScoredPoint", "Record", "UpdateResult", "CollectionInfo", "Distance"]
+__all__ = ["B200VectorStore", "ScoredPoint", "Record", "UpdateResult", "CollectionInfo", "Distance", "PointGroup",
+           "GroupsResult"]
 
 
 @dataclass
@@ -45,6 +46,17 @@ class Record:
     id: Any
     payload: dict | None = None
     vector: Any = None
+
+
+@dataclass
+class PointGroup:
+    id: Any                 # the group's payload value at ``group_by``
+    hits: list = field(default_factory=list)   # its best ScoredPoints, best first
+
+
+@dataclass
+class GroupsResult:
+    groups: list = field(default_factory=list)
 
 
 @dataclass
@@ -378,6 +390,43 @@ class B200VectorStore:
             return [[ScoredPoint(id=col.ids[int(ids[b, j])], score=float(scores[b, j]),
                                  payload=col.payloads[int(ids[b, j])] if with_payload else None)
                      for j in range(int(counts[b]))] for b in range(q.shape[0])]
+
+    def search_groups(self, collection_name: str, query_vector, group_by: str, limit: int = 10, group_size: int = 1,
+                      query_filter=None, with_payload: bool = True, with_vectors: bool = False, with_lookup=None,
+                      score_threshold=None, **_ignored) -> GroupsResult:
+        """Qdrant ``search_groups``: the best ``limit`` groups of points sharing a payload value at ``group_by`` (a dotted
+        path such as ``metadata.parent_id``), ranked by their best point, each with its best ``group_size`` points, over
+        the points matching ``query_filter``.  Exact, with the scores and order of ``search``.  Points without the key (or
+        with null) are in no group; ``True`` and ``1`` are different groups; a list-valued field raises ``ValueError``.
+        ``with_lookup`` and ``score_threshold`` would change the result and are not supported: they raise ``ValueError``."""
+        if with_lookup is not None:
+            raise ValueError("search_groups: with_lookup is not supported")
+        if score_threshold is not None:
+            raise ValueError("search_groups: score_threshold is not supported")
+        if not isinstance(group_by, str) or not group_by:
+            raise ValueError("search_groups: group_by must be a payload key")
+        L, G = int(limit), int(group_size)
+        if not (1 <= L <= 1024 and 1 <= G <= 1024):
+            raise ValueError(f"search_groups: limit {L} and group_size {G} must be in [1, 1024]")
+        col = self._get(collection_name)
+        if isinstance(query_vector, tuple):  # ("name", vector) form of the named-vector API
+            query_vector = query_vector[1]
+        q = np.asarray(query_vector, dtype=np.float32).reshape(1, -1)
+        with col.lock:
+            pi = col.payload_index()
+            f, table = pi.field(group_by)
+            filters = self._compile_filters(col, [query_filter]) if query_filter is not None else None
+            ng, codes, hits, ids, scores = col.engine.dense_groups(q, f, L, G, filters=filters)
+            value_of = {c: vk[1] for vk, c in table.items()}
+            groups = []
+            for g in range(int(ng[0])):
+                pts = []
+                for r in range(int(hits[0, g])):
+                    row = int(ids[0, g, r])
+                    pts.append(ScoredPoint(id=col.ids[row], score=float(scores[0, g, r]),
+                                           payload=col.payloads[row] if with_payload else None))
+                groups.append(PointGroup(id=value_of[int(codes[0, g])], hits=pts))
+            return GroupsResult(groups=groups)
 
     @staticmethod
     def _compile_filters(col: _Collection, filters):
