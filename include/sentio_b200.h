@@ -116,6 +116,26 @@ int sb_dense_load_metric(sb_ctx* ctx, int slot, const void* vecs, int64_t n, int
                          int32_t metric);
 int32_t sb_dense_metric(sb_ctx* ctx, int slot);
 /*
+ * Storage datatype of a slot -- Qdrant's `VectorParams.datatype` (float32 is Qdrant's default, float16 opt-in there).
+ * SB_STORAGE_F16 is every slot above: results are exact on the stored fp16 representation.  SB_STORAGE_F32 keeps the
+ * same fp16 rows (the scans read them, so they run as fast) and additionally the caller's rows x in fp32 (SB_F16 input
+ * widened exactly): 6 bytes per dimension per row in HBM.  Every score and order is then exact fp64 on x and the
+ * caller's fp32 query q (DESIGN.md K1g):
+ *   SB_METRIC_COSINE  <q, x> / (||q|| ||x||), 0 for a zero row or zero query;
+ *   SB_METRIC_DOT     <q, x>;
+ *   SB_METRIC_EUCLID  sqrt(sum (q_i - x_i)^2), computed directly (a stored point's own vector is at distance 0.0).
+ * sb_dense_fetch returns x bit for bit (Cosine: fl32(x / ||x||), Qdrant's normalised vector); upsert, delete, reserve,
+ * tags, filtered and grouped search follow the slot's storage.  A float32 slot rejects rows with a non-finite fp64 norm
+ * (every metric).
+ * sb_dense_load_storage: sb_dense_load_metric with a storage datatype; sb_dense_load / sb_dense_load_metric mean
+ * SB_STORAGE_F16.  sb_dense_storage: the slot's storage, -1 for a bad slot.
+ */
+#define SB_STORAGE_F16 0
+#define SB_STORAGE_F32 1
+int sb_dense_load_storage(sb_ctx* ctx, int slot, const void* vecs, int64_t n, int32_t d, int32_t dtype, int64_t id_base,
+                          int32_t metric, int32_t storage);
+int32_t sb_dense_storage(sb_ctx* ctx, int slot);
+/*
  * Scan selection: 0 = auto (batches of >= 16 queries use the wgmma batched-query scan, smaller ones the CUDA-core
  * scan), 1 = CUDA-core scan only, 2 = wgmma scan whenever eligible.  Results are identical in every mode.
  */
@@ -139,7 +159,8 @@ int sb_dense_topk(sb_ctx* ctx, int slot, const float* q, int32_t B, int32_t k,
                   int64_t* out_ids, double* out_scores, int32_t* out_counts);
 int sb_dense_topk_dev(sb_ctx* ctx, int slot, const float* q_dev, int32_t B, int32_t k,
                       int64_t* out_ids_dev, double* out_scores_dev, int32_t* out_counts_dev, void* stream);
-/* copies stored (fp16 -> fp32) rows of the given ids back to the host: out[n_ids * d]; used by tests/tools */
+/* copies stored (fp16 -> fp32) rows of the given ids back to the host: out[n_ids * d]; used by tests/tools.  A float32
+ * slot returns x (Cosine: fl32(x / ||x||)) */
 int sb_dense_fetch(sb_ctx* ctx, int slot, const int64_t* ids, int32_t n_ids, float* out);
 /*
  * Filtered dense search -- the `query_filter=` argument of the Qdrant search (reference

@@ -43,6 +43,9 @@ SIGNATURES = {
     "sb_dense_load_metric": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_int64,
                                        C.c_int32]),
     "sb_dense_metric": (C.c_int32, [C.c_void_p, C.c_int]),
+    "sb_dense_load_storage": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_int64,
+                                        C.c_int32, C.c_int32]),
+    "sb_dense_storage": (C.c_int32, [C.c_void_p, C.c_int]),
     "sb_dense_set_mode": (C.c_int, [C.c_void_p, C.c_int]),
     "sb_dense_count": (C.c_int64, [C.c_void_p, C.c_int]),
     "sb_dense_dim": (C.c_int32, [C.c_void_p, C.c_int]),

@@ -67,6 +67,7 @@ void sb_destroy(sb_ctx* ctx) {
     if (ctx->dense[s].inv_norm) cudaFree(ctx->dense[s].inv_norm);
     if (ctx->dense[s].cfac) cudaFree(ctx->dense[s].cfac);
     if (ctx->dense[s].hh) cudaFree(ctx->dense[s].hh);
+    if (ctx->dense[s].rows32) cudaFree(ctx->dense[s].rows32);
     for (int f = 0; f < SB_MAX_TAG_FIELDS; ++f)
       if (ctx->dense[s].tags[f]) cudaFree(ctx->dense[s].tags[f]);
   }
@@ -94,6 +95,7 @@ void sb_destroy(sb_ctx* ctx) {
   ctx->qn_dev.release();
   ctx->qaux_dev.release();
   ctx->fb_count_dev.release();
+  ctx->sigma_dev.release();
   ctx->filt_dev.release();
   ctx->filt_pin.release();
   ctx->grp_res_dev.release();

@@ -103,6 +103,11 @@ struct DenseIndex {
   float* hh = nullptr;       // [n_cap] Euclid only: h >= ||v||^2 / 2 rounded up to fp32
   double rho_max = 0.0;      // >= max ||v|| over every row ever stored since the load (an upsert may raise it)
   double h_max = 0.0;        // Euclid: >= max h, likewise
+  // float32 storage (DESIGN.md K1g): the caller's rows x next to everything above, which the scans still read.  The exact
+  // stage scores x; sigma_max >= max over rows ever stored of ||y^ - x^|| (Cosine) or ||c y - x|| (Dot / Euclid)
+  int32_t storage = SB_STORAGE_F16;
+  float* rows32 = nullptr;   // [n_cap][d_pad] fp32, zero padded; nullptr for float16 storage
+  double sigma_max = 0.0;
   // cached CUtensorMap (128 bytes, 64-byte aligned) over rows[0, n_pad) for the wgmma batched scan; valid iff
   // tm_rows_ptr == rows and tm_n_pad == n_pad (an append within capacity keeps `rows` but widens n_pad)
   alignas(64) unsigned char tm_rows[128] = {0};
@@ -161,6 +166,7 @@ struct sb_ctx {
   DevBuf qn_dev;     // dense: normalised fp32 queries [B][d_pad] fed to the scans
   DevBuf qaux_dev;   // dense: per-query eps [B] fp32 | fallback flags [B] i32
   DevBuf fb_count_dev;   // dense: [1] u64, queries answered by the exact fallback kernel (sb_dense_fallback_count)
+  DevBuf sigma_dev;      // dense float32 storage: [1] u64, bits of the largest sigma of the rows one load / upsert stores
   DevBuf filt_dev;       // filtered dense: match mask | per-query counts / state | conditions (CSR)
   PinBuf filt_pin;       // filtered dense: host copies of the conditions and the per-query match counts
   // grouped dense search (sb_dense_groups): result [B][L][G] | one round's prefixes | replicated queries | completions

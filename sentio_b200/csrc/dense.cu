@@ -82,6 +82,49 @@ __global__ void dense_store_rows_kernel(const TIn* __restrict__ in, int64_t n_ro
   if (hh) hh[out_row] = __double2float_ru(0.5 * (c * c) * ss16);
 }
 
+// Float32 storage (DESIGN.md K1g), launched after dense_store_rows_kernel on the same rows: one warp per row writes
+// rows32 = x (fp16 input widened exactly, zero padded) and folds the row's sigma into *sigma_bits (an fp64 bit pattern;
+// non-negative doubles order like their bits): Cosine ||y/||y|| - x/||x|| ||, Dot / Euclid ||c y - x||, evaluated in
+// fp64 and rounded up by the margin DESIGN.md K1g derives.
+template <typename TIn>
+__global__ void dense_store_rows32_kernel(const TIn* __restrict__ in, int64_t n_rows, int32_t d, int32_t d_pad,
+                                          const __half* __restrict__ rows, float* __restrict__ rows32, int64_t row0,
+                                          const int64_t* __restrict__ dst_rows, const double* __restrict__ cfac,
+                                          unsigned long long* __restrict__ sigma_bits) {
+  const int64_t r = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (r >= n_rows) return;
+  const int64_t out_row = dst_rows ? dst_rows[r] : row0 + r;
+  const TIn* src = in + r * (int64_t)d;
+  const __half* y = rows + out_row * (int64_t)d_pad;
+  float* dst = rows32 + out_row * (int64_t)d_pad;
+  double xx = 0.0, yy = 0.0;
+  for (int i = lane; i < d_pad; i += 32) {
+    const float x = i < d ? (float)src[i] : 0.f;
+    dst[i] = x;
+    const double xd = (double)x, yd = (double)__half2float(y[i]);
+    xx = __fma_rn(xd, xd, xx);
+    yy = __fma_rn(yd, yd, yy);
+  }
+  for (int o = 16; o; o >>= 1) {
+    xx += __shfl_xor_sync(0xffffffffu, xx, o);
+    yy += __shfl_xor_sync(0xffffffffu, yy, o);
+  }
+  const double nx = sqrt(xx), ny = sqrt(yy);
+  const double c = cfac ? cfac[out_row] : 0.0;
+  double ee = 0.0;
+  for (int i = lane; i < d; i += 32) {
+    const double xd = (double)(float)src[i], yd = (double)__half2float(y[i]);
+    const double t = cfac ? __fma_rn(c, yd, -xd) : __dsub_rn(ny > 0.0 ? yd / ny : 0.0, nx > 0.0 ? xd / nx : 0.0);
+    ee = __fma_rn(t, t, ee);
+  }
+  for (int o = 16; o; o >>= 1) ee += __shfl_xor_sync(0xffffffffu, ee, o);
+  if (lane != 0) return;
+  const double m = cfac ? nx : 1.0;
+  const double sig = __fma_ru(sqrt(ee), 1.0 + 0x1p-39, m * 0x1p-39);
+  atomicMax(sigma_bits, (unsigned long long)__double_as_longlong(sig));
+}
+
 // ------------------------------------------------------------------------------------------------ mutation kernels
 // sb_dense_delete's compaction: one warp per move from[m] -> to[m] (sources >= n - |D| > destinations, so one launch
 // has no read/write hazard): the fp16 row in 16-byte copies, its inverse norm and its code in every loaded tag column.
@@ -90,6 +133,7 @@ struct MoveParams {
   float* inv_norm;
   double* cfac;                       // Dot / Euclid, else nullptr
   float* hh;                          // Euclid, else nullptr
+  float* rows32;                      // float32 storage, else nullptr
   int32_t* tags[SB_MAX_TAG_FIELDS];   // nullptr = field not loaded
   const int64_t* from;
   const int64_t* to;
@@ -105,6 +149,11 @@ __global__ void __launch_bounds__(256) dense_move_rows_kernel(const MoveParams p
   const uint4* src = reinterpret_cast<const uint4*>(p.rows) + s * p.ch;
   uint4* dst = reinterpret_cast<uint4*>(p.rows) + t * p.ch;
   for (int c = lane; c < p.ch; c += 32) dst[c] = src[c];
+  if (p.rows32) {   // the fp32 row: 2 * ch 16-byte chunks
+    const uint4* src32 = reinterpret_cast<const uint4*>(p.rows32) + s * 2 * p.ch;
+    uint4* dst32 = reinterpret_cast<uint4*>(p.rows32) + t * 2 * p.ch;
+    for (int c = lane; c < 2 * p.ch; c += 32) dst32[c] = src32[c];
+  }
   if (lane == 0) {
     p.inv_norm[t] = p.inv_norm[s];
     if (p.cfac) p.cfac[t] = p.cfac[s];
@@ -543,6 +592,7 @@ struct MergeParams {
   const int32_t* state;      // FILTER only: [nq] 1 = answered by the gather path (nothing to merge)
   int32_t metric;
   const double* cfac;
+  const float* rows32;       // F32 only
 };
 
 __device__ __forceinline__ void block_sort_desc_u64(unsigned long long* a, int len, int tid, int nt) {
@@ -567,8 +617,8 @@ __device__ __forceinline__ void block_sort_desc_u64(unsigned long long* a, int l
 // One CTA per query.  (1) a lower bound of the global k-th best approximate key = the k-th largest among the first
 // R = ceil(K'/G) entries of every list (G*R >= K' >= k real keys); (2) every list contributes its prefix inside the
 // error window below that key; a FULL list whose last entry is still inside the window may have dropped members ->
-// fallback; (3) exact fp64 re-score of the whole window; (4) final order, emit k.
-template <bool FILTER>
+// fallback; (3) exact fp64 re-score of the whole window (F32: against the float32 rows); (4) final order, emit k.
+template <bool FILTER, bool F32>
 __global__ void __launch_bounds__(kMergeThreads, 1) dense_merge_kernel(const MergeParams p) {
   extern __shared__ __align__(16) uint8_t msmem[];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nt = blockDim.x, nw = nt >> 5;
@@ -640,7 +690,8 @@ __global__ void __launch_bounds__(kMergeThreads, 1) dense_merge_kernel(const Mer
   ra.out_count = p.out_counts + qi;
   ra.metric = p.metric;
   ra.cfac = p.cfac;
-  rescore_and_emit(sel, nsel, P, ek, ei, &qq_s, q_s, ra);
+  ra.rows32 = p.rows32;
+  rescore_and_emit<F32>(sel, nsel, P, ek, ei, &qq_s, q_s, ra);
 }
 
 // ------------------------------------------------------------------------------------------------ query preparation
@@ -650,13 +701,16 @@ __global__ void __launch_bounds__(kMergeThreads, 1) dense_merge_kernel(const Mer
 // Dot / Euclid (DESIGN.md K1e): eps[r] bounds |approximate - exact key| in key units, from the cosine bound and the slot's
 // norm bounds rho (>= max ||v||) and hmax (>= max h); Euclid also writes rq[r] = (float)||q[r]||.  A query whose key
 // could leave the fp32 range, or whose exact fp64 distances cannot resolve the window, gets its fallback flag fb[r].
+// Float32 storage (DESIGN.md K1g) adds sigma (>= ||y^ - x^|| resp. ||v - x|| over the slot's rows): the key of x differs
+// from the key of v by at most sigma (Cosine, Dot) or (r + rho) sigma (Euclid); sigma = 0 for float16 storage.
 struct PrepMetric {
   int32_t metric;
-  double rho, hmax;
+  double rho, hmax, sigma;
   float* rq;      // [rows] Euclid
   int32_t* fb;    // [rows]
 };
 
+template <bool F32>
 __global__ void __launch_bounds__(256) dense_prep_queries_kernel(const float* __restrict__ q_pad, int nq, int d_pad,
                                                                  float* __restrict__ qn, __half* __restrict__ q16,
                                                                  float* __restrict__ eps, int mma, const PrepMetric pm) {
@@ -704,18 +758,23 @@ __global__ void __launch_bounds__(256) dense_prep_queries_kernel(const float* __
     for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += s_red[w];
     float e = 0.f;
     if (!zero) e = mma ? (float)(sqrt(t) * 1.0001) + dense_eps_mma_acc(d_pad) : dense_eps_fp32(d_pad);
+    // float32 storage (DESIGN.md K1g): + sigma (Cosine, Dot), + (r + rho) sigma (Euclid), the first through r * ed
+    if constexpr (F32)
+      if (pm.metric == SB_METRIC_COSINE && !zero) e = __double2float_ru((double)e + pm.sigma);
     if (pm.metric != SB_METRIC_COSINE) {
       // Dot: |acc * (float)c - <qn, v>| <= c (e + 2^-22) with c <= rho (1 + 2^-10); the zero query keeps eps 0 (every key
       // is exactly 0).  Euclid: key = r * (acc * s) - h; r * eps_dot + r rho 2^-22 (r and its product) + hmax 2^-22 (h
       // rounded up) + (r rho + hmax) 2^-24 (the subtraction), all inside (r rho + hmax) 2^-20.
-      const double ed = ((double)e + 0x1p-20) * pm.rho * 1.001;
+      double ed = ((double)e + 0x1p-20) * pm.rho * 1.001;
+      if constexpr (F32) ed += pm.sigma;
       const bool fits = pm.rho <= 1e36;
       if (pm.metric == SB_METRIC_DOT) {
         e = zero ? 0.f : __double2float_ru(ed);
         if (!fits) pm.fb[r] = 1;
       } else {
         const double rr = zero ? 0.0 : (double)(float)nrm;
-        const double ee = (rr * ed + (rr * pm.rho + pm.hmax) * 0x1p-20) * 1.001;
+        double ee = (rr * ed + (rr * pm.rho + pm.hmax) * 0x1p-20) * 1.001;
+        if constexpr (F32) ee += pm.rho * pm.sigma * 1.001;   // | ||v||^2 - ||x||^2 | / 2 <= (rho + sigma / 2) sigma
         e = __double2float_ru(ee);
         // the fp64 exact stage resolves ||q - v||^2 to (r + rho)^2 2^-41 (d <= 4096 terms); it must stay far below eps
         const double res = (rr + pm.rho) * (rr + pm.rho) * 0x1p-41;
@@ -749,9 +808,10 @@ struct FallbackParams {
   int32_t mask_qs;
   int32_t metric;
   const double* cfac;
+  const float* rows32;           // F32 only
 };
 
-template <bool FILTER>
+template <bool FILTER, bool F32>
 __global__ void __launch_bounds__(kFbThreads, 1) dense_exact_fallback_kernel(const FallbackParams p) {
   const int qi = blockIdx.x;
   if (p.flag[qi] == 0) return;
@@ -822,7 +882,8 @@ __global__ void __launch_bounds__(kFbThreads, 1) dense_exact_fallback_kernel(con
       if constexpr (FILTER)
         if (row < p.n) match = (p.mask[(size_t)(row >> 5) * p.mask_qs + qi] >> (row & 31)) & 1u;
       if (row < p.n && match) {
-        okey = f64_orderable(exact_key_warp(p.metric, p.rows, p.cfac, (uint32_t)row, q, p.d_pad, p.ch, qn, lane));
+        okey = f64_orderable(
+            exact_key_row<F32>(p.metric, p.rows, p.cfac, p.rows32, (uint32_t)row, q, p.d_pad, p.ch, qn, lane));
         if (okey == 0ull) okey = 1ull;
       }
       if (lane == 0) {
@@ -944,8 +1005,10 @@ struct GatherParams {
   int32_t* out_counts;
   int32_t metric;
   const double* cfac;
+  const float* rows32;       // F32 only
 };
 
+template <bool F32>
 __global__ void __launch_bounds__(kMergeThreads, 1) dense_filter_gather_kernel(const GatherParams p) {
   extern __shared__ __align__(16) uint8_t gsmem[];
   unsigned long long* sel = reinterpret_cast<unsigned long long*>(gsmem);   // [kGatherMax] (key score field unused)
@@ -980,7 +1043,8 @@ __global__ void __launch_bounds__(kMergeThreads, 1) dense_filter_gather_kernel(c
   ra.out_count = p.out_counts + qi;
   ra.metric = p.metric;
   ra.cfac = p.cfac;
-  rescore_and_emit(sel, nsel, P, ek, ei, &qq_s, q_s, ra);
+  ra.rows32 = p.rows32;
+  rescore_and_emit<F32>(sel, nsel, P, ek, ei, &qq_s, q_s, ra);
 }
 
 // ------------------------------------------------------------------------------------------------ grouped search (K1f)
@@ -1243,10 +1307,10 @@ int dense_topk_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int B, i
   float *qn = nullptr, *eps = nullptr, *rq = nullptr;
   int32_t* fb = nullptr;
   if ((rc = dense_prep_queries(ctx, ix, q_pad, B, B, /*mma=*/false, &qn, nullptr, &eps, &fb, &rq, st))) return rc;
-  if (flt) SB_CUDA(cudaFuncSetAttribute(dense_merge_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        (int)pl.merge_smem));
-  else SB_CUDA(cudaFuncSetAttribute(dense_merge_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    (int)pl.merge_smem));
+  const bool f32 = ix.rows32 != nullptr;
+  auto merge_kern = flt ? (f32 ? dense_merge_kernel<true, true> : dense_merge_kernel<true, false>)
+                        : (f32 ? dense_merge_kernel<false, true> : dense_merge_kernel<false, false>);
+  SB_CUDA(cudaFuncSetAttribute(merge_kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.merge_smem));
   for (int c0 = 0; c0 < B; c0 += chunk) {
     const int nq = std::min(chunk, B - c0);
     int b0 = 0;
@@ -1306,10 +1370,10 @@ int dense_topk_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int B, i
     mp.state = flt ? flt->state + c0 : nullptr;
     mp.metric = ix.metric;
     mp.cfac = ix.cfac;
+    mp.rows32 = ix.rows32;
     {
       ProfScope ps(ctx, SB_PROF_DENSE_MERGE, st);
-      if (flt) dense_merge_kernel<true><<<nq, kMergeThreads, pl.merge_smem, st>>>(mp);
-      else dense_merge_kernel<false><<<nq, kMergeThreads, pl.merge_smem, st>>>(mp);
+      merge_kern<<<nq, kMergeThreads, pl.merge_smem, st>>>(mp);
     }
     SB_CUDA(cudaGetLastError());
   }
@@ -1341,6 +1405,34 @@ __global__ void dense_fetch_kernel(const __half* rows, const double* cfac, int d
   }
 }
 
+// float32 storage: x bit for bit; normalise = Cosine: fl32(x / ||x||) with ||x|| in fp64 (a zero row stays zero)
+__global__ void __launch_bounds__(128) dense_fetch_f32_kernel(const float* rows32, bool normalise, int d, int d_pad,
+                                                              int64_t n, int64_t id_base, const int64_t* ids, int n_ids,
+                                                              float* out) {
+  __shared__ double s_red[4];
+  const int r = blockIdx.x;
+  if (r >= n_ids) return;
+  const int64_t idx = ids[r] - id_base;
+  const bool live = idx >= 0 && idx < n;
+  const float* x = rows32 + (size_t)(live ? idx : 0) * d_pad;
+  double nrm = 1.0;
+  if (normalise) {
+    double ss = 0.0;
+    if (live)
+      for (int i = threadIdx.x; i < d; i += blockDim.x) ss = __fma_rn((double)x[i], (double)x[i], ss);
+    for (int o = 16; o; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
+    if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = ss;
+    __syncthreads();
+    const double t = s_red[0] + s_red[1] + s_red[2] + s_red[3];
+    nrm = t > 0.0 ? sqrt(t) : 1.0;
+  }
+  for (int i = threadIdx.x; i < d; i += blockDim.x) {
+    float v = 0.f;
+    if (live) v = normalise ? (float)((double)x[i] / nrm) : x[i];
+    out[(size_t)r * d + i] = v;
+  }
+}
+
 }  // namespace
 
 // Shared with dense_mma.cu: query preparation (normalised fp32 copy, optional fp16 operand rows, eps, cleared fallback
@@ -1355,7 +1447,8 @@ int dense_prep_queries(sb_ctx* ctx, const DenseIndex& ix, const float* q_pad, in
   pm.metric = ix.metric;
   pm.rho = ix.rho_max;
   pm.hmax = ix.h_max;
-  pm.rq = ix.metric == SB_METRIC_EUCLID ? reinterpret_cast<float*>(fb + rows) : nullptr;
+  pm.sigma = ix.sigma_max;
+  pm.rq =ix.metric == SB_METRIC_EUCLID ? reinterpret_cast<float*>(fb + rows) : nullptr;
   pm.fb = fb;
   *rq_out = pm.rq;
   float* qn = nullptr;
@@ -1366,7 +1459,8 @@ int dense_prep_queries(sb_ctx* ctx, const DenseIndex& ix, const float* q_pad, in
   }
   SB_CUDA(cudaMemsetAsync(fb, 0, (size_t)rows * 4, st));
   ctx->launches += 1;
-  dense_prep_queries_kernel<<<rows, 256, 0, st>>>(q_pad, B, ix.d_pad, qn, q16, eps, mma ? 1 : 0, pm);
+  if (ix.rows32) dense_prep_queries_kernel<true><<<rows, 256, 0, st>>>(q_pad, B, ix.d_pad, qn, q16, eps, mma ? 1 : 0, pm);
+  else dense_prep_queries_kernel<false><<<rows, 256, 0, st>>>(q_pad, B, ix.d_pad, qn, q16, eps, mma ? 1 : 0, pm);
   SB_CUDA(cudaGetLastError());
   *eps_out = eps;
   *fb_out = fb;
@@ -1398,9 +1492,12 @@ int dense_fallback_enqueue(sb_ctx* ctx, const DenseIndex& ix, const float* q_pad
   fp.out_counts = out_counts;
   fp.metric = ix.metric;
   fp.cfac = ix.cfac;
+  fp.rows32 = ix.rows32;
   ctx->launches += 1;
-  if (flt) dense_exact_fallback_kernel<true><<<B, kFbThreads, 0, st>>>(fp);
-  else dense_exact_fallback_kernel<false><<<B, kFbThreads, 0, st>>>(fp);
+  const bool f32 = ix.rows32 != nullptr;
+  auto kern = flt ? (f32 ? dense_exact_fallback_kernel<true, true> : dense_exact_fallback_kernel<true, false>)
+                  : (f32 ? dense_exact_fallback_kernel<false, true> : dense_exact_fallback_kernel<false, false>);
+  kern<<<B, kFbThreads, 0, st>>>(fp);
   SB_CUDA(cudaGetLastError());
   return SB_OK;
 }
@@ -1466,8 +1563,8 @@ int dense_topk_filtered_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad,
   int32_t* qlist_d = reinterpret_cast<int32_t*>(dv + o_qlist);
   uint32_t* mask = reinterpret_cast<uint32_t*>(dv + o_mask);
   const size_t gather_smem = (size_t)kGatherMax * 20 + (size_t)ix.d_pad * 4 + 64;
-  SB_CUDA(cudaFuncSetAttribute(dense_filter_gather_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                               (int)gather_smem));
+  auto gather_kern = ix.rows32 ? dense_filter_gather_kernel<true> : dense_filter_gather_kernel<false>;
+  SB_CUDA(cudaFuncSetAttribute(gather_kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gather_smem));
   for (int c0 = 0; c0 < B; c0 += qchunk) {
     const int nq = std::min(qchunk, B - c0);
     const int qs = std::max(32, next_pow2(nq));   // >= the widest wgmma group of the chunk
@@ -1527,8 +1624,9 @@ int dense_topk_filtered_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad,
       gp.out_counts = oc;
       gp.metric = ix.metric;
       gp.cfac = ix.cfac;
+      gp.rows32 = ix.rows32;
       ProfScope ps(ctx, SB_PROF_DENSE_GATHER, st);
-      dense_filter_gather_kernel<<<n_gather, kMergeThreads, gather_smem, st>>>(gp);
+      gather_kern<<<n_gather, kMergeThreads, gather_smem, st>>>(gp);
     }
     SB_CUDA(cudaGetLastError());
     if (n_gather < nq) {
@@ -1731,14 +1829,21 @@ int64_t round_rows(int64_t n) { return (n + kRowPad - 1) / kRowPad * kRowPad; }
 
 // The one store-rows path of sb_dense_load and sb_dense_upsert: n host rows (SB_F32 / SB_F16) through a device staging
 // buffer in chunks, converted by dense_store_rows_kernel into rows row0 + i, or dst_dev[i] (a device list) when given.
+// A float32 slot also gets rows32 from dense_store_rows32_kernel, and *sigma the largest sigma of the stored rows.
 // Returns after the last chunk has been stored.
 int dense_store_staged(sb_ctx* ctx, DenseIndex& ix, const void* vecs, int64_t n, int32_t dtype, const int64_t* dst_dev,
-                       int64_t row0) {
+                       int64_t row0, double* sigma) {
   const int d = ix.d;
   const size_t esz = dtype == SB_F32 ? 4 : 2;
   const int64_t chunk_rows = std::max<int64_t>(1, (int64_t)((256ull << 20) / ((size_t)d * esz)));
   int rc = ctx->misc_dev.reserve((size_t)std::min<int64_t>(chunk_rows, n) * d * esz);
   if (rc) return rc;
+  unsigned long long* sigma_bits = nullptr;
+  if (ix.rows32) {
+    if ((rc = ctx->sigma_dev.reserve(8))) return rc;
+    sigma_bits = ctx->sigma_dev.as<unsigned long long>();
+    SB_CUDA(cudaMemsetAsync(sigma_bits, 0, 8, ctx->stream));
+  }
   for (int64_t r0 = 0; r0 < n; r0 += chunk_rows) {
     const int64_t nr = std::min<int64_t>(chunk_rows, n - r0);
     const uint8_t* src = reinterpret_cast<const uint8_t*>(vecs) + (size_t)r0 * d * esz;
@@ -1755,7 +1860,22 @@ int dense_store_staged(sb_ctx* ctx, DenseIndex& ix, const void* vecs, int64_t n,
                                                                             ix.rows, ix.inv_norm, row0 + r0, dst,
                                                                             ix.cfac != nullptr, ix.cfac, ix.hh);
     SB_CUDA(cudaGetLastError());
+    if (ix.rows32) {
+      if (dtype == SB_F32)
+        dense_store_rows32_kernel<float><<<blocks, wpb * 32, 0, ctx->stream>>>(
+            ctx->misc_dev.as<float>(), nr, d, ix.d_pad, ix.rows, ix.rows32, row0 + r0, dst, ix.cfac, sigma_bits);
+      else
+        dense_store_rows32_kernel<__half><<<blocks, wpb * 32, 0, ctx->stream>>>(
+            ctx->misc_dev.as<__half>(), nr, d, ix.d_pad, ix.rows, ix.rows32, row0 + r0, dst, ix.cfac, sigma_bits);
+      SB_CUDA(cudaGetLastError());
+    }
     SB_CUDA(cudaStreamSynchronize(ctx->stream));  // staging buffer is reused by the next chunk
+  }
+  *sigma = 0.0;
+  if (sigma_bits) {
+    unsigned long long bits = 0;
+    SB_CUDA(cudaMemcpy(&bits, sigma_bits, 8, cudaMemcpyDeviceToHost));
+    memcpy(sigma, &bits, 8);
   }
   return SB_OK;
 }
@@ -1768,11 +1888,14 @@ int dense_grow(sb_ctx* ctx, DenseIndex& ix, int64_t n_cap) {
   float* inv = nullptr;
   double* cfac = nullptr;
   float* hh = nullptr;
+  float* rows32 = nullptr;
+  const size_t rb32 = (size_t)ix.d_pad * sizeof(float);
   int32_t* tags[SB_MAX_TAG_FIELDS] = {};
   cudaError_t e = cudaMalloc(&rows, (size_t)n_cap * rb);
   if (e == cudaSuccess) e = cudaMalloc(&inv, (size_t)n_cap * sizeof(float));
   if (e == cudaSuccess && ix.metric != SB_METRIC_COSINE) e = cudaMalloc(&cfac, (size_t)n_cap * sizeof(double));
   if (e == cudaSuccess && ix.metric == SB_METRIC_EUCLID) e = cudaMalloc(&hh, (size_t)n_cap * sizeof(float));
+  if (e == cudaSuccess && ix.storage == SB_STORAGE_F32) e = cudaMalloc(&rows32, (size_t)n_cap * rb32);
   for (int f = 0; f < SB_MAX_TAG_FIELDS && e == cudaSuccess; ++f)
     if (ix.tags[f]) e = cudaMalloc(&tags[f], (size_t)n_cap * 4);
   const int64_t keep = ix.n_pad;
@@ -1791,6 +1914,10 @@ int dense_grow(sb_ctx* ctx, DenseIndex& ix, int64_t n_cap) {
     if (e == cudaSuccess && keep) e = cudaMemcpyAsync(hh, ix.hh, (size_t)keep * sizeof(float), cudaMemcpyDeviceToDevice, st);
     if (e == cudaSuccess) e = cudaMemsetAsync(hh + keep, 0, (size_t)(n_cap - keep) * sizeof(float), st);
   }
+  if (rows32) {
+    if (e == cudaSuccess && keep) e = cudaMemcpyAsync(rows32, ix.rows32, (size_t)keep * rb32, cudaMemcpyDeviceToDevice, st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(rows32 + (size_t)keep * ix.d_pad, 0, (size_t)(n_cap - keep) * rb32, st);
+  }
   for (int f = 0; f < SB_MAX_TAG_FIELDS && e == cudaSuccess; ++f) {
     if (!tags[f]) continue;
     if (keep) e = cudaMemcpyAsync(tags[f], ix.tags[f], (size_t)keep * 4, cudaMemcpyDeviceToDevice, st);
@@ -1803,6 +1930,7 @@ int dense_grow(sb_ctx* ctx, DenseIndex& ix, int64_t n_cap) {
     cudaFree(inv);
     cudaFree(cfac);
     cudaFree(hh);
+    cudaFree(rows32);
     for (int f = 0; f < SB_MAX_TAG_FIELDS; ++f) cudaFree(tags[f]);
     sb_set_error("dense: growing slot to %lld rows failed: %s", (long long)n_cap, cudaGetErrorString(e));
     return SB_ERR_CUDA;
@@ -1811,10 +1939,12 @@ int dense_grow(sb_ctx* ctx, DenseIndex& ix, int64_t n_cap) {
   cudaFree(ix.inv_norm);
   cudaFree(ix.cfac);
   cudaFree(ix.hh);
+  cudaFree(ix.rows32);
   ix.rows = rows;
   ix.inv_norm = inv;
   ix.cfac = cfac;
   ix.hh = hh;
+  ix.rows32 = rows32;
   for (int f = 0; f < SB_MAX_TAG_FIELDS; ++f)
     if (ix.tags[f]) {
       cudaFree(ix.tags[f]);
@@ -1886,8 +2016,8 @@ int sb_dense_pad_queries(sb_ctx* ctx, const DenseIndex& ix, const float* q, int 
 
 extern "C" {
 
-int sb_dense_load_metric(sb_ctx* ctx, int slot, const void* vecs, int64_t n, int32_t d, int32_t dtype, int64_t id_base,
-                         int32_t metric) {
+int sb_dense_load_storage(sb_ctx* ctx, int slot, const void* vecs, int64_t n, int32_t d, int32_t dtype, int64_t id_base,
+                          int32_t metric, int32_t storage) {
   SB_REQUIRE(ctx != nullptr, SB_ERR_ARG, "sb_dense_load: ctx is NULL");
   SB_REQUIRE(slot >= 0 && slot < SB_MAX_DENSE_SLOTS, SB_ERR_ARG, "sb_dense_load: bad slot %d", slot);
   SB_REQUIRE(n >= 0 && d > 0 && d <= 4096, SB_ERR_ARG, "sb_dense_load: bad shape n=%lld d=%d", (long long)n, d);
@@ -1896,10 +2026,13 @@ int sb_dense_load_metric(sb_ctx* ctx, int slot, const void* vecs, int64_t n, int
   SB_REQUIRE(n == 0 || vecs != nullptr, SB_ERR_ARG, "sb_dense_load: vecs is NULL");
   SB_REQUIRE(metric == SB_METRIC_COSINE || metric == SB_METRIC_DOT || metric == SB_METRIC_EUCLID, SB_ERR_ARG,
              "sb_dense_load: metric %d is not supported (SB_METRIC_COSINE, SB_METRIC_DOT or SB_METRIC_EUCLID)", metric);
+  SB_REQUIRE(storage == SB_STORAGE_F16 || storage == SB_STORAGE_F32, SB_ERR_ARG,
+             "sb_dense_load: storage %d is not supported (SB_STORAGE_F16 or SB_STORAGE_F32)", storage);
   double rho = 0.0, hmax = 0.0;
-  if (metric != SB_METRIC_COSINE) {
+  if (metric != SB_METRIC_COSINE || storage == SB_STORAGE_F32) {   // float32 storage: finite norms for every metric
     int rc = check_metric_rows("sb_dense_load", metric, vecs, n, d, dtype, &rho, &hmax);
     if (rc) return rc;
+    if (metric == SB_METRIC_COSINE) rho = 0.0;
   }
   std::lock_guard<std::mutex> lk(ctx->mu);
   DeviceGuard g(ctx->device);
@@ -1909,6 +2042,7 @@ int sb_dense_load_metric(sb_ctx* ctx, int slot, const void* vecs, int64_t n, int
   if (ix.inv_norm) cudaFree(ix.inv_norm);
   if (ix.cfac) cudaFree(ix.cfac);
   if (ix.hh) cudaFree(ix.hh);
+  if (ix.rows32) cudaFree(ix.rows32);
   for (int f = 0; f < SB_MAX_TAG_FIELDS; ++f)
     if (ix.tags[f]) cudaFree(ix.tags[f]);
   ix = DenseIndex();
@@ -1918,9 +2052,10 @@ int sb_dense_load_metric(sb_ctx* ctx, int slot, const void* vecs, int64_t n, int
   ix.n_pad = round_rows(n);
   ix.id_base = id_base;
   ix.metric = metric;
+  ix.storage = storage;
   ix.rho_max = rho;
   ix.h_max = hmax;
-  if (n == 0) return SB_OK;
+  if (n == 0) return SB_OK;   // an empty float32 slot gets rows32 with its first growth
   ix.n_cap = ix.n_pad;
   SB_CUDA(cudaMalloc(&ix.rows, (size_t)ix.n_cap * ix.d_pad * sizeof(__half)));
   SB_CUDA(cudaMalloc(&ix.inv_norm, (size_t)ix.n_cap * sizeof(float)));
@@ -1934,7 +2069,16 @@ int sb_dense_load_metric(sb_ctx* ctx, int slot, const void* vecs, int64_t n, int
     SB_CUDA(cudaMalloc(&ix.hh, (size_t)ix.n_cap * sizeof(float)));
     SB_CUDA(cudaMemsetAsync(ix.hh, 0, (size_t)ix.n_cap * sizeof(float), ctx->stream));
   }
-  return dense_store_staged(ctx, ix, vecs, n, dtype, nullptr, 0);
+  if (storage == SB_STORAGE_F32) {
+    SB_CUDA(cudaMalloc(&ix.rows32, (size_t)ix.n_cap * ix.d_pad * sizeof(float)));
+    SB_CUDA(cudaMemsetAsync(ix.rows32, 0, (size_t)ix.n_cap * ix.d_pad * sizeof(float), ctx->stream));
+  }
+  return dense_store_staged(ctx, ix, vecs, n, dtype, nullptr, 0, &ix.sigma_max);
+}
+
+int sb_dense_load_metric(sb_ctx* ctx, int slot, const void* vecs, int64_t n, int32_t d, int32_t dtype, int64_t id_base,
+                         int32_t metric) {
+  return sb_dense_load_storage(ctx, slot, vecs, n, d, dtype, id_base, metric, SB_STORAGE_F16);
 }
 
 int sb_dense_load(sb_ctx* ctx, int slot, const void* vecs, int64_t n, int32_t d, int32_t dtype, int64_t id_base) {
@@ -1945,6 +2089,12 @@ int32_t sb_dense_metric(sb_ctx* ctx, int slot) {
   if (!ctx || slot < 0 || slot >= SB_MAX_DENSE_SLOTS) return -1;
   std::lock_guard<std::mutex> lk(ctx->mu);
   return ctx->dense[slot].metric;
+}
+
+int32_t sb_dense_storage(sb_ctx* ctx, int slot) {
+  if (!ctx || slot < 0 || slot >= SB_MAX_DENSE_SLOTS) return -1;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  return ctx->dense[slot].storage;
 }
 
 int sb_dense_reserve(sb_ctx* ctx, int slot, int64_t n_cap) {
@@ -1980,9 +2130,11 @@ int sb_dense_upsert(sb_ctx* ctx, int slot, const int64_t* rows, const void* vecs
   const int64_t m = sorted.end() - std::lower_bound(sorted.begin(), sorted.end(), ix.n);
   SB_REQUIRE(m == 0 || (sorted[n - m] == ix.n && sorted[n - 1] == ix.n + m - 1), SB_ERR_ARG,
              "sb_dense_upsert: appended rows must be exactly %lld .. %lld", (long long)ix.n, (long long)(ix.n + m - 1));
-  double rho = 0.0, hmax = 0.0;
-  if (ix.metric != SB_METRIC_COSINE)
+  double rho = 0.0, hmax = 0.0, sigma = 0.0;
+  if (ix.metric != SB_METRIC_COSINE || ix.storage == SB_STORAGE_F32) {
     if ((rc = check_metric_rows("sb_dense_upsert", ix.metric, vecs, n, ix.d, dtype, &rho, &hmax))) return rc;
+    if (ix.metric == SB_METRIC_COSINE) rho = 0.0;
+  }
   SB_CUDA(cudaDeviceSynchronize());   // searches enqueued on other streams may still read the slot
   const int64_t n_new = ix.n + m;
   if (round_rows(n_new) > ix.n_cap)
@@ -1990,7 +2142,7 @@ int sb_dense_upsert(sb_ctx* ctx, int slot, const int64_t* rows, const void* vecs
   if ((rc = ctx->misc2_dev.reserve((size_t)n * 8))) return rc;
   int64_t* dst = ctx->misc2_dev.as<int64_t>();
   SB_CUDA(cudaMemcpyAsync(dst, rows, (size_t)n * 8, cudaMemcpyHostToDevice, ctx->stream));
-  if ((rc = dense_store_staged(ctx, ix, vecs, n, dtype, dst, 0))) return rc;
+  if ((rc = dense_store_staged(ctx, ix, vecs, n, dtype, dst, 0, &sigma))) return rc;
   for (int f = 0; f < SB_MAX_TAG_FIELDS; ++f)
     if (ix.tags[f])
       dense_tags_scatter_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(ix.tags[f], dst, nullptr, n);
@@ -2001,6 +2153,7 @@ int sb_dense_upsert(sb_ctx* ctx, int slot, const int64_t* rows, const void* vecs
   // the bounds only rise: an overwritten or deleted row's larger norm leaves a stale bound, which is still a bound
   ix.rho_max = std::max(ix.rho_max, rho);
   ix.h_max = std::max(ix.h_max, hmax);
+  ix.sigma_max = std::max(ix.sigma_max, sigma);
   return SB_OK;
 }
 
@@ -2073,6 +2226,7 @@ int sb_dense_delete(sb_ctx* ctx, int slot, const int64_t* rows, int64_t n, int64
     mp.inv_norm = ix.inv_norm;
     mp.cfac = ix.cfac;
     mp.hh = ix.hh;
+    mp.rows32 = ix.rows32;
     memcpy(mp.tags, ix.tags, sizeof(mp.tags));
     mp.from = f_dev;
     mp.to = f_dev + mv;
@@ -2086,6 +2240,8 @@ int sb_dense_delete(sb_ctx* ctx, int slot, const int64_t* rows, int64_t n, int64
   SB_CUDA(cudaMemsetAsync(ix.inv_norm + keep, 0, (size_t)n * sizeof(float), ctx->stream));
   if (ix.cfac) SB_CUDA(cudaMemsetAsync(ix.cfac + keep, 0, (size_t)n * sizeof(double), ctx->stream));
   if (ix.hh) SB_CUDA(cudaMemsetAsync(ix.hh + keep, 0, (size_t)n * sizeof(float), ctx->stream));
+  if (ix.rows32)
+    SB_CUDA(cudaMemsetAsync(ix.rows32 + (size_t)keep * ix.d_pad, 0, (size_t)n * ix.d_pad * sizeof(float), ctx->stream));
   for (int f = 0; f < SB_MAX_TAG_FIELDS; ++f)
     if (ix.tags[f]) SB_CUDA(cudaMemsetAsync(ix.tags[f] + keep, 0xff, (size_t)n * 4, ctx->stream));
   SB_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -2202,8 +2358,13 @@ int sb_dense_fetch(sb_ctx* ctx, int slot, const int64_t* ids, int32_t n_ids, flo
   if ((rc = ctx->misc2_dev.reserve((size_t)n_ids * 8))) return rc;
   if ((rc = ctx->misc3_dev.reserve((size_t)n_ids * ix.d * 4))) return rc;
   SB_CUDA(cudaMemcpyAsync(ctx->misc2_dev.p, ids, (size_t)n_ids * 8, cudaMemcpyHostToDevice, ctx->stream));
-  dense_fetch_kernel<<<n_ids, 128, 0, ctx->stream>>>(ix.rows, ix.cfac, ix.d, ix.d_pad, ix.n, ix.id_base,
-                                                     ctx->misc2_dev.as<int64_t>(), n_ids, ctx->misc3_dev.as<float>());
+  if (ix.rows32)
+    dense_fetch_f32_kernel<<<n_ids, 128, 0, ctx->stream>>>(ix.rows32, ix.metric == SB_METRIC_COSINE, ix.d, ix.d_pad, ix.n,
+                                                           ix.id_base, ctx->misc2_dev.as<int64_t>(), n_ids,
+                                                           ctx->misc3_dev.as<float>());
+  else
+    dense_fetch_kernel<<<n_ids, 128, 0, ctx->stream>>>(ix.rows, ix.cfac, ix.d, ix.d_pad, ix.n, ix.id_base,
+                                                       ctx->misc2_dev.as<int64_t>(), n_ids, ctx->misc3_dev.as<float>());
   SB_CUDA(cudaGetLastError());
   SB_CUDA(cudaMemcpyAsync(out, ctx->misc3_dev.p, (size_t)n_ids * ix.d * 4, cudaMemcpyDeviceToHost, ctx->stream));
   SB_CUDA(cudaStreamSynchronize(ctx->stream));

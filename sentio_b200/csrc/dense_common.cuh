@@ -14,6 +14,7 @@ struct RescoreArgs {
   int32_t* out_count;   // [1]
   int32_t metric;       // SB_METRIC_*
   const double* cfac;   // [rows] c of v = c * y (Dot / Euclid)
+  const float* rows32;  // float32 storage: [rows][d_pad] the caller's x (read by the F32 instantiations only)
 };
 
 // ---- approximate -> exact hand-off (DESIGN.md "K1: exactness") --------------------------------------------------------
@@ -157,6 +158,68 @@ __device__ __forceinline__ void exact_metric_warp(int metric, const __half* rows
   }
 }
 
+// Exact fp64 ordering key of NR float32-storage rows x (DESIGN.md K1g), one full warp; every lane returns them.
+//   Cosine: <q, x> / (||q|| ||x||)   (0 for a zero row or query; qn = ||q||)
+//   Dot:    <q, x>
+//   Euclid: -sqrt(sum (q_i - x_i)^2)  (computed directly: q = x gives exactly 0)
+// Lane l reads 8 floats of chunk c = l + 32 j of every row with two float4 loads (rows are 32-byte aligned).  NR = 1 and
+// NR = 2 perform the same operations in the same order per row, so they agree bit for bit.
+template <int NR>
+__device__ __forceinline__ void exact_f32_warp(int metric, const float* rows32, const uint32_t (&idx)[NR], const float* q,
+                                               int d_pad, int nch, double qn, int lane, double (&out)[NR]) {
+  const bool euclid = metric == SB_METRIC_EUCLID, cosine = metric == SB_METRIC_COSINE;
+  const float4* r[NR];
+  double acc[NR], xx[NR];
+#pragma unroll
+  for (int i = 0; i < NR; ++i) {
+    r[i] = reinterpret_cast<const float4*>(rows32 + (size_t)idx[i] * d_pad);
+    acc[i] = 0.0;
+    xx[i] = 0.0;
+  }
+  for (int ch = lane; ch < nch; ch += 32) {
+    const float4 qa = *reinterpret_cast<const float4*>(q + (size_t)ch * 8);
+    const float4 qb = *reinterpret_cast<const float4*>(q + (size_t)ch * 8 + 4);
+    const float qv[8] = {qa.x, qa.y, qa.z, qa.w, qb.x, qb.y, qb.z, qb.w};
+    float4 raw[NR][2];
+#pragma unroll
+    for (int i = 0; i < NR; ++i) {
+      raw[i][0] = __ldg(r[i] + 2 * ch);
+      raw[i][1] = __ldg(r[i] + 2 * ch + 1);
+    }
+#pragma unroll
+    for (int i = 0; i < NR; ++i) {
+      const float xv[8] = {raw[i][0].x, raw[i][0].y, raw[i][0].z, raw[i][0].w,
+                           raw[i][1].x, raw[i][1].y, raw[i][1].z, raw[i][1].w};
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        const double x = (double)xv[e], qe = (double)qv[e];
+        if (euclid) {
+          const double t = __dsub_rn(qe, x);
+          acc[i] = __fma_rn(t, t, acc[i]);
+        } else {
+          acc[i] = __fma_rn(x, qe, acc[i]);
+          if (cosine) xx[i] = __fma_rn(x, x, xx[i]);
+        }
+      }
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < NR; ++i) {
+    for (int o = 16; o; o >>= 1) {
+      acc[i] += __shfl_xor_sync(0xffffffffu, acc[i], o);
+      xx[i] += __shfl_xor_sync(0xffffffffu, xx[i], o);
+    }
+    if (euclid) {
+      out[i] = -sqrt(acc[i]);
+    } else if (cosine) {
+      const double den = qn * sqrt(xx[i]);
+      out[i] = den > 0.0 ? acc[i] / den : 0.0;
+    } else {
+      out[i] = acc[i];
+    }
+  }
+}
+
 // exact ordering key of one stored row under the slot's metric (Cosine: the existing cosine path)
 __device__ __forceinline__ double exact_key_warp(int metric, const __half* rows, const double* cfac, uint32_t idx,
                                                  const float* q, int d_pad, int nch, double qn, int lane) {
@@ -165,6 +228,20 @@ __device__ __forceinline__ double exact_key_warp(int metric, const __half* rows,
   double s[1];
   exact_metric_warp<1>(metric, rows, cfac, ix, q, d_pad, nch, lane, s);
   return s[0];
+}
+
+// exact ordering key of one row under the slot's storage: F32 scores the caller's x, else the stored fp16 representation
+template <bool F32>
+__device__ __forceinline__ double exact_key_row(int metric, const __half* rows, const double* cfac, const float* rows32,
+                                                uint32_t idx, const float* q, int d_pad, int nch, double qn, int lane) {
+  if constexpr (F32) {
+    const uint32_t ix[1] = {idx};
+    double s[1];
+    exact_f32_warp<1>(metric, rows32, ix, q, d_pad, nch, qn, lane, s);
+    return s[0];
+  } else {
+    return exact_key_warp(metric, rows, cfac, idx, q, d_pad, nch, qn, lane);
+  }
 }
 
 // first min(k, P) sorted pairs -> this query's output rows (Euclid keys are minus the distance: the score is the distance)
@@ -230,7 +307,9 @@ __device__ __forceinline__ void exact_cosine_warp2(const __half* rows, uint32_t 
 // Exact fp64 re-score of the window members sel[0..nsel) (composite keys) against the STORED fp16 rows and the fp32
 // query, final order (score desc, row asc), emit k results.  Whole-CTA cooperative; ek/ei are P-entry shared-memory
 // arrays (P = power of two >= nsel), qq_s a shared double, q_s a shared-memory staging area for the query (d_pad floats;
-// the L2 round trip of the query per re-scored row was a third of the stage's latency).
+// the L2 round trip of the query per re-scored row was a third of the stage's latency).  F32: float32 storage, the
+// window is re-scored against the caller's fp32 rows (exact_f32_warp).
+template <bool F32>
 __device__ __forceinline__ void rescore_and_emit(const unsigned long long* sel, int nsel, int P, unsigned long long* ek,
                                                  uint32_t* ei, double* qq_s_ptr, float* q_s, const RescoreArgs p) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nt = blockDim.x, nw = nt >> 5;
@@ -247,7 +326,13 @@ __device__ __forceinline__ void rescore_and_emit(const unsigned long long* sel, 
       i0 = key32_idx(key0);
       i1 = key32_idx(key1);
       double s0, s1;
-      if (p.metric == SB_METRIC_COSINE) {
+      if constexpr (F32) {
+        const uint32_t ix[2] = {i0, i1};
+        double s[2];
+        exact_f32_warp<2>(p.metric, p.rows32, ix, q_s, p.d_pad, p.ch, qn, lane, s);
+        s0 = s[0];
+        s1 = s[1];
+      } else if (p.metric == SB_METRIC_COSINE) {
         exact_cosine_warp2(p.rows, i0, i1, q_s, p.d_pad, p.ch, qn, lane, &s0, &s1);
       } else {
         const uint32_t ix[2] = {i0, i1};
@@ -260,10 +345,10 @@ __device__ __forceinline__ void rescore_and_emit(const unsigned long long* sel, 
       o1 = f64_orderable(s1);
     } else if (key0 != 0ull) {
       i0 = key32_idx(key0);
-      o0 = f64_orderable(exact_key_warp(p.metric, p.rows, p.cfac, i0, q_s, p.d_pad, p.ch, qn, lane));
+      o0 = f64_orderable(exact_key_row<F32>(p.metric, p.rows, p.cfac, p.rows32, i0, q_s, p.d_pad, p.ch, qn, lane));
     } else if (key1 != 0ull) {
       i1 = key32_idx(key1);
-      o1 = f64_orderable(exact_key_warp(p.metric, p.rows, p.cfac, i1, q_s, p.d_pad, p.ch, qn, lane));
+      o1 = f64_orderable(exact_key_row<F32>(p.metric, p.rows, p.cfac, p.rows32, i1, q_s, p.d_pad, p.ch, qn, lane));
     }
     if (key0 != 0ull && o0 == 0ull) o0 = 1ull;  // keep 0 reserved for "empty"
     if (key1 != 0ull && o1 == 0ull) o1 = 1ull;

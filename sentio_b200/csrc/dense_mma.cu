@@ -276,6 +276,7 @@ struct SelectParams {
   const int32_t* state;             // FILTER only: [nq] 1 = answered by the gather path (threshold +inf, no emit)
   int32_t metric;
   const double* cfac;
+  const float* rows32;              // F32 only
 };
 
 // One CTA per query.  A lower bound of the k-th best approximate key among the survivors of all CTAs by an MSB-first
@@ -284,8 +285,8 @@ struct SelectParams {
 //   mode 0 (sampling pass): threshold = that score - 2 eps.
 //   mode 1: gather every survivor inside the window below it, exact fp64 re-score of all of them, emit k.
 // Survivors are staged in shared memory when they fit (the normal case: ~0.3 % of the corpus); otherwise every pass
-// streams them from HBM/L2 -- slower, still exact.
-template <bool FILTER>
+// streams them from HBM/L2 -- slower, still exact.  F32: float32 storage, the exact stage scores the caller's rows.
+template <bool FILTER, bool F32>
 __global__ void __launch_bounds__(kSelectThreads, 2) dense_select_kernel(const SelectParams p) {
   extern __shared__ __align__(16) uint8_t ssm[];
   unsigned long long* keys = reinterpret_cast<unsigned long long*>(ssm);  // [kSelStage] staged survivors
@@ -426,8 +427,9 @@ __global__ void __launch_bounds__(kSelectThreads, 2) dense_select_kernel(const S
   ra.out_count = p.out_counts + qi;
   ra.metric = p.metric;
   ra.cfac = p.cfac;
+  ra.rows32 = p.rows32;
   // the staged survivors are dead (the window lives in `top`): their shared memory becomes the query staging area
-  rescore_and_emit(top, ntop, P, ek, ei, &qq_s, reinterpret_cast<float*>(keys), ra);
+  rescore_and_emit<F32>(top, ntop, P, ek, ei, &qq_s, reinterpret_cast<float*>(keys), ra);
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -553,13 +555,12 @@ int dense_mma_topk_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int 
   }
   const CUtensorMap& tm_rows = *reinterpret_cast<const CUtensorMap*>(ix.tm_rows);
   const size_t sel_smem = (size_t)kSelStage * 8 + (size_t)kSelTop * 20 + 64;
-  if (flt) SB_CUDA(cudaFuncSetAttribute(dense_select_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        (int)sel_smem));
-  else SB_CUDA(cudaFuncSetAttribute(dense_select_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    (int)sel_smem));
+  const bool f32 = ix.rows32 != nullptr;
+  auto sel_kern = flt ? (f32 ? dense_select_kernel<true, true> : dense_select_kernel<true, false>)
+                      : (f32 ? dense_select_kernel<false, true> : dense_select_kernel<false, false>);
+  SB_CUDA(cudaFuncSetAttribute(sel_kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sel_smem));
   auto launch_select = [&](int nblocks, const SelectParams& s) {
-    if (flt) dense_select_kernel<true><<<nblocks, kSelectThreads, sel_smem, st>>>(s);
-    else dense_select_kernel<false><<<nblocks, kSelectThreads, sel_smem, st>>>(s);
+    sel_kern<<<nblocks, kSelectThreads, sel_smem, st>>>(s);
   };
   const bool euclid = ix.metric == SB_METRIC_EUCLID;   // Cosine and Dot run the same (acc * scale) kernels
   auto run_mma = [&](int qbn, const CUtensorMap& tm_q, const MmaScanParams& m, int g, size_t smem) {
@@ -604,6 +605,7 @@ int dense_mma_topk_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int 
     SelectParams sp;
     sp.metric = ix.metric;
     sp.cfac = ix.cfac;
+    sp.rows32 = ix.rows32;
     sp.cand = cand;
     sp.counts = counts;
     sp.capg = capg;

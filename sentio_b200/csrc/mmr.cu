@@ -13,15 +13,16 @@ namespace {
 
 constexpr int kGreedyThreads = 1024;
 
-// candidates by id from the stored fp16 corpus -> fp32 matrix
-__global__ void mmr_gather_kernel(const __half* rows, int d, int d_pad, int64_t n_rows, int64_t id_base,
+// candidates by id from the stored corpus -> fp32 matrix: the fp16 rows, or a float32 slot's x (what its search scores)
+template <typename T>
+__global__ void mmr_gather_kernel(const T* rows, int d, int d_pad, int64_t n_rows, int64_t id_base,
                                   const int64_t* ids, int n, float* out) {
   const int r = blockIdx.x;
   if (r >= n) return;
   const int64_t idx = ids[r] - id_base;
   const bool ok = idx >= 0 && idx < n_rows;
   for (int i = threadIdx.x; i < d; i += blockDim.x)
-    out[(size_t)r * d + i] = ok ? __half2float(rows[(size_t)idx * d_pad + i]) : 0.f;
+    out[(size_t)r * d + i] = ok ? (float)rows[(size_t)idx * d_pad + i] : 0.f;
 }
 
 // one warp per candidate: dot(q, c_i), |c_i|^2 ; warp 0 of block 0 also |q|^2
@@ -221,8 +222,12 @@ int sb_semantic_mmr(sb_ctx* ctx, int slot, const float* q, int32_t d, const floa
                "sb_semantic_mmr: dense slot %d is empty or has dimension %d != %d", slot, ix.d, d);
     if ((rc = ctx->misc3_dev.reserve(nd * 8))) return rc;
     SB_CUDA(cudaMemcpyAsync(ctx->misc3_dev.p, cand_ids, nd * 8, cudaMemcpyHostToDevice, st));
-    mmr_gather_kernel<<<n, 128, 0, st>>>(ix.rows, ix.d, ix.d_pad, ix.n, ix.id_base, ctx->misc3_dev.as<int64_t>(), n,
-                                         Cd);
+    if (ix.rows32)
+      mmr_gather_kernel<float><<<n, 128, 0, st>>>(ix.rows32, ix.d, ix.d_pad, ix.n, ix.id_base,
+                                                  ctx->misc3_dev.as<int64_t>(), n, Cd);
+    else
+      mmr_gather_kernel<__half><<<n, 128, 0, st>>>(ix.rows, ix.d, ix.d_pad, ix.n, ix.id_base,
+                                                   ctx->misc3_dev.as<int64_t>(), n, Cd);
     SB_CUDA(cudaGetLastError());
   }
   {

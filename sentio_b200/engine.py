@@ -88,14 +88,20 @@ class B200Engine:
 
     # ------------------------------------------------------------------ K1 dense
     METRICS = {"cosine": 0, "dot": 1, "euclid": 2}   # SB_METRIC_* (include/sentio_b200.h)
+    DATATYPES = {"float16": 0, "float32": 1}         # SB_STORAGE_*
 
-    def load_dense(self, vecs: np.ndarray, id_base: int = 0, slot: int = 0, metric: str = "cosine") -> None:
+    def load_dense(self, vecs: np.ndarray, id_base: int = 0, slot: int = 0, metric: str = "cosine",
+                   storage: str = "float16") -> None:
         """``metric``: "cosine" (default), "dot" or "euclid" -- the slot's distance (DESIGN.md K1e); every search,
         upsert and delete on the slot follows it.  Dot scores are <q, v>, Euclid scores the distance ||q - v||
-        (ascending)."""
+        (ascending).  ``storage``: "float16" (default; scores are exact on the stored fp16 representation) or
+        "float32" (the slot also keeps the input rows x, and every score is exact on x; DESIGN.md K1g)."""
         m = self.METRICS.get(str(metric).lower())
         if m is None:
             raise ValueError(f"metric {metric!r} is not supported (cosine, dot or euclid)")
+        st = self.DATATYPES.get(str(storage).lower())
+        if st is None:
+            raise ValueError(f"storage {storage!r} is not supported (float16 or float32)")
         v = np.ascontiguousarray(vecs)
         if v.ndim != 2:
             raise ValueError("vecs must be [n, d]")
@@ -105,7 +111,10 @@ class B200Engine:
             v = np.ascontiguousarray(v, dtype=np.float32)
             dt = 0
         n, d = v.shape
-        if m == 0:
+        if st != 0:
+            check(self._lib.sb_dense_load_storage(self._h, slot, _ptr(v), n, d, dt, int(id_base), m, st),
+                  "sb_dense_load_storage")
+        elif m == 0:
             check(self._lib.sb_dense_load(self._h, slot, _ptr(v), n, d, dt, int(id_base)), "sb_dense_load")
         else:
             check(self._lib.sb_dense_load_metric(self._h, slot, _ptr(v), n, d, dt, int(id_base), m),
@@ -120,6 +129,14 @@ class B200Engine:
         if m not in names:
             raise SentioB200Error(f"sb_dense_metric: bad slot {slot}")
         return names[m]
+
+    def dense_storage(self, slot: int = 0) -> str:
+        """The slot's storage datatype: "float16" or "float32"."""
+        s = int(self._lib.sb_dense_storage(self._h, slot))
+        names = {v: k for k, v in self.DATATYPES.items()}
+        if s not in names:
+            raise SentioB200Error(f"sb_dense_storage: bad slot {slot}")
+        return names[s]
 
     def dense_set_mode(self, mode: int) -> None:
         """0 = auto, 1 = CUDA-core scan only, 2 = wgmma batched scan whenever eligible."""

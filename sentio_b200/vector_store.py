@@ -28,8 +28,8 @@ import numpy as np
 from .engine import B200Engine
 from .payload_filter import PayloadIndex
 
-__all__ = ["B200VectorStore", "ScoredPoint", "Record", "UpdateResult", "CollectionInfo", "Distance", "PointGroup",
-           "GroupsResult"]
+__all__ = ["B200VectorStore", "ScoredPoint", "Record", "UpdateResult", "CollectionInfo", "Distance", "Datatype",
+           "PointGroup", "GroupsResult"]
 
 
 @dataclass
@@ -71,10 +71,19 @@ class Distance(enum.Enum):
     MANHATTAN = "Manhattan"   # accepted by the parser so it can be refused by name: an L1 distance is not a GEMM
 
 
+class Datatype(enum.Enum):
+    """Qdrant's ``VectorParams.datatype``.  FLOAT16 keeps fp16 rows (scores exact on them); FLOAT32 also keeps the
+    vectors as given, and every score is exact on them (DESIGN.md K1g).  UINT8 is parsed so it can be refused by name."""
+    FLOAT32 = "float32"
+    FLOAT16 = "float16"
+    UINT8 = "uint8"
+
+
 @dataclass
 class VectorParams:
     size: int
     distance: Distance = Distance.COSINE
+    datatype: Datatype | None = None
 
 
 @dataclass
@@ -124,6 +133,21 @@ def parse_distance(dist) -> Distance:
 _ENGINE_METRIC = {Distance.COSINE: "cosine", Distance.DOT: "dot", Distance.EUCLID: "euclid"}
 
 
+def parse_datatype(dt) -> Datatype:
+    """A Qdrant vector datatype given as this module's ``Datatype``, ``qdrant_client``'s ``Datatype`` enum (read by
+    ``.name``), its value or a plain string, case-insensitive ("float32", "FLOAT16", ...); ``None`` is FLOAT16, this
+    store's default.  UINT8 (quantised storage) raises ``ValueError``."""
+    if dt is None:
+        return Datatype.FLOAT16
+    name = _distance_name(dt).strip().lower()
+    for t in Datatype:
+        if name in (t.name.lower(), t.value):
+            if t is Datatype.UINT8:
+                raise ValueError("datatype uint8 is not supported (supported: float32, float16)")
+            return t
+    raise ValueError(f"datatype {_distance_name(dt)!r} is not supported (supported: float32, float16)")
+
+
 class _Collection:
     def __init__(self, name: str, device: int):
         self.name = name
@@ -133,6 +157,7 @@ class _Collection:
         self.row_of: dict[Any, int] = {}
         self.dim = 0
         self.distance = Distance.COSINE
+        self.datatype = Datatype.FLOAT16
         self.lock = threading.RLock()
         self._payload_index: PayloadIndex | None = None
 
@@ -181,17 +206,26 @@ class B200VectorStore:
         """Upload a whole collection (brute-force search needs no incremental index), or, with Qdrant's
         ``vectors_config=VectorParams(size, distance)`` and no vectors, create an empty one that ``upsert`` fills.
         The distance is Cosine (the default without ``vectors_config``), Dot or Euclid (Qdrant's semantics: Dot scores
-        <q, v>, Euclid scores the distance ||q - v|| and ranks it ascending); Manhattan raises ``ValueError``."""
+        <q, v>, Euclid scores the distance ||q - v|| and ranks it ascending); Manhattan raises ``ValueError``.
+        ``vectors_config.datatype``: None or FLOAT16 (this store's default: fp16 rows) or FLOAT32 (the vectors are kept
+        as given and every score is exact on them, at 6 bytes per dimension per point in HBM); UINT8 raises
+        ``ValueError``."""
         dist = Distance.COSINE
+        dtype = Datatype.FLOAT16
         if vectors_config is not None:
             if isinstance(vectors_config, dict):
                 raise ValueError("create_collection: named vectors are not supported (one unnamed vector per point)")
             dist = parse_distance(getattr(vectors_config, "distance", "Cosine"))
+            dtype = parse_datatype(getattr(vectors_config, "datatype", None))
         # an engine lists the metrics its load_dense accepts in METRICS; one without the table loads Cosine only
         supported = getattr(B200Engine, "METRICS", {"cosine": 0})
         if _ENGINE_METRIC[dist] not in supported:
             raise ValueError(f"create_collection: distance {dist.value} is not supported by {B200Engine.__name__} "
                              f"(it loads {', '.join(sorted(supported))})")
+        # likewise DATATYPES: an engine without the table stores float16 only
+        if dtype.value not in getattr(B200Engine, "DATATYPES", {"float16": 0}):
+            raise ValueError(f"create_collection: datatype {dtype.value} is not supported by {B200Engine.__name__} "
+                             "(it stores float16 only)")
         if vectors is None:
             if vectors_config is None:
                 raise ValueError("create_collection: give vectors or vectors_config")
@@ -200,8 +234,11 @@ class B200VectorStore:
         n = vecs.shape[0]
         col = _Collection(collection_name, self._device)
         col.distance = dist
+        col.datatype = dtype
         try:
-            if dist is Distance.COSINE:
+            if dtype is Datatype.FLOAT32:
+                col.engine.load_dense(vecs, id_base=0, slot=0, metric=_ENGINE_METRIC[dist], storage="float32")
+            elif dist is Distance.COSINE:
                 col.engine.load_dense(vecs, id_base=0, slot=0)
             else:
                 col.engine.load_dense(vecs, id_base=0, slot=0, metric=_ENGINE_METRIC[dist])
@@ -228,7 +265,8 @@ class B200VectorStore:
         col = self._get(collection_name)
         with col.lock:
             return CollectionInfo(points_count=len(col.ids),
-                                  config=CollectionConfig(CollectionParams(VectorParams(col.dim, col.distance))))
+                                  config=CollectionConfig(CollectionParams(VectorParams(col.dim, col.distance,
+                                                                                        col.datatype))))
 
     def get_collections(self) -> CollectionsResponse:
         return CollectionsResponse([CollectionDescription(name) for name in list(self._collections)])
@@ -337,7 +375,8 @@ class B200VectorStore:
     def retrieve(self, collection_name: str, ids: Sequence[Any], with_payload: bool = True, with_vectors: bool = False,
                  **_ignored) -> list[Record]:
         """Points by id (unknown ids are skipped, as in Qdrant); vectors are the stored fp16 values, widened (Dot /
-        Euclid: c * y, the input to the fp16 precision of its direction; Qdrant would return the input itself)."""
+        Euclid: c * y, the input to the fp16 precision of its direction).  A FLOAT32 collection returns the vectors as
+        given (Cosine: normalised, x / ||x||), as Qdrant does."""
         col = self._get(collection_name)
         with col.lock:
             rows = [col.row_of[i] for i in ids if i in col.row_of]
