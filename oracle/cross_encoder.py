@@ -13,6 +13,7 @@ from __future__ import annotations
 import math
 
 import numpy as np
+from scipy.special import erf as _erf
 
 
 def hf_model(cfg: dict, seed: int = 0):
@@ -50,9 +51,6 @@ def _ln(x, g, b, eps):
     mu = x.mean(-1, keepdims=True)
     var = ((x - mu) ** 2).mean(-1, keepdims=True)
     return (x - mu) / np.sqrt(var + eps) * g + b
-
-
-_erf = np.vectorize(math.erf)
 
 
 def _gelu(x):

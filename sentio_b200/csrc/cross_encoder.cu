@@ -40,9 +40,9 @@ struct CeModel {
   float *x32 = nullptr, *pre32 = nullptr;          // residual stream, pre-LayerNorm sums  [M,H]
   __half* pre16 = nullptr;                         // pre-LayerNorm sums of the fp16 residual stream  [M,H]
   // fp16 residual stream (the reranker): x16 is BOTH the GEMM operand and the residual, the pre-LN sum is stored in fp16;
-  // half the bytes of the two N = 384 GEMM epilogues and of the LayerNorms.  CPU study (oracle forward with the LayerNorm
-  // inputs and outputs rounded to fp16): sigmoid scores move by 1.6e-4 relative (tolerance 1e-3).  The embedder keeps the
-  // fp32 stream: its output is the hidden state itself, compared element-wise.
+  // half the bytes of the two N = 384 GEMM epilogues and of the LayerNorms.  Its logit error against fp64 is the fp32
+  // stream's (the fp16 GEMM operands dominate both; DESIGN.md K5).  The embedder keeps the fp32 stream: its output is the
+  // hidden state itself, compared element-wise.
   bool fp16_stream = false;
   __half *x16 = nullptr, *qkv16 = nullptr, *ctx16 = nullptr, *ffn16 = nullptr;  // [M,H] [M,3H] [M,H] [M,I]
   CUtensorMap m_x16, m_ctx16, m_ffn16;
@@ -789,12 +789,12 @@ int ce_forward(sb_ctx* ctx, CeModel* m, const int32_t* ids, const int32_t* tts, 
       SB_CUDA(cudaGetLastError());
       return SB_OK;
     }
+    // sb_ce_load admits heads = H / 32 in {4, 8, 12, 24}: every count is divisible by 3 or by 2
+    SB_REQUIRE(heads % 3 == 0 || heads % 2 == 0, SB_ERR_UNSUPPORTED, "ce_forward: %d attention heads", heads);
     if (S <= 128 && heads % 3 == 0)
       ce_attention_mma_kernel<128, 3><<<P * (heads / 3), 128, 0, st>>>(m->qkv16, lens, cu, S, H, heads, m->ctx16);
-    else if (S <= 128 && heads % 2 == 0)
-      ce_attention_mma_kernel<128, 2><<<P * (heads / 2), 128, 0, st>>>(m->qkv16, lens, cu, S, H, heads, m->ctx16);
     else if (S <= 128)
-      ce_attention_mma_kernel<128, 1><<<P * heads, 128, 0, st>>>(m->qkv16, lens, cu, S, H, heads, m->ctx16);
+      ce_attention_mma_kernel<128, 2><<<P * (heads / 2), 128, 0, st>>>(m->qkv16, lens, cu, S, H, heads, m->ctx16);
     else if (S <= 256)
       ce_attention_mma_kernel<256, 1><<<P * heads, 128, 0, st>>>(m->qkv16, lens, cu, S, H, heads, m->ctx16);
     else {

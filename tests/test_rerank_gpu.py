@@ -1,10 +1,11 @@
-"""K5 parity: wgmma GEMM unit test, cross-encoder forward vs the NumPy / HuggingFace oracles (rel 1e-3, abs floor 1e-4),
-and the reranker's control flow vs the reference JinaReranker (golden rerank_flow.json)."""
+"""K5 parity: wgmma GEMM unit test, cross-encoder forward vs the NumPy / HuggingFace oracles (sigmoid: rel 1e-3, abs
+floor 1e-4; logits: the device-emulation tolerance of tests/ce_numerics.py), and the reranker's control flow vs the reference JinaReranker (golden rerank_flow.json)."""
 import math
 
 import numpy as np
 import pytest
 
+import ce_numerics as cn
 from conftest import load_golden
 from oracle import cross_encoder as ce_oracle
 from sentio_b200 import synth
@@ -24,7 +25,11 @@ _erf = np.vectorize(math.erf)
                                        (513, 256, 192, 2),
                                        (2304, 640, 192, 0), (4100, 512, 384, 1), (9000, 1152, 384, 0), (2048, 1536, 128, 1),
                                        # epi 3: the fp16 residual stream (residual operand and output in fp16)
-                                       (96, 384, 384, 3), (700, 384, 1536, 3), (3000, 384, 384, 3), (2600, 384, 1536, 3)])
+                                       (96, 384, 384, 3), (700, 384, 1536, 3), (3000, 384, 384, 3), (2600, 384, 1536, 3),
+                                       # hidden 768 (QKV, FFN up, FFN down on both streams) and hidden 256 (QKV)
+                                       *[(M, N, K, epi) for (N, K, epi) in ((2304, 768, 0), (3072, 768, 1), (768, 3072, 2),
+                                                                            (768, 3072, 3), (768, 256, 0))
+                                         for M in (1, 127, 129)]])
 def test_tcgen05_gemm_matches_numpy(engine, M, N, K, epi):
     rng = np.random.default_rng(M + N + K + epi)
     a = rng.standard_normal((M, K)).astype(np.float32)
@@ -54,6 +59,15 @@ def _pairs(n_docs, seq_len=128):
     return hash_tokenize_pairs("w1 w5 w9 w100 w3 w7", docs, seq_len)
 
 
+def _assert_logits_within_emulated_tolerance(w, ids, tt, lens, logits):
+    """|logit - fp64| within 3 x the distance of the device-rounding emulation (fp16 residual stream, the reranker's
+    default) from fp64, plus 1e-5 (tests/ce_numerics.py)."""
+    ref = cn.forward(w, ids, tt, lens)[0]
+    tol = cn.tolerance(cn.forward(w, ids, tt, lens, mode="fp16")[0], ref)
+    err = np.abs(logits.astype(np.float64) - ref).max()
+    assert err <= tol, f"max|gpu-fp64| {err:.3e} > tol {tol:.3e}"
+
+
 def test_small_model_vs_numpy_oracle(engine):
     cfg = dict(vocab_size=30522, hidden=128, layers=2, heads=4, intermediate=256, max_pos=128, type_vocab=2, ln_eps=1e-12)
     w = CrossEncoderWeights.random(cfg, seed=3, std=0.05)
@@ -63,6 +77,7 @@ def test_small_model_vs_numpy_oracle(engine):
     want_l, want_s = ce_oracle.numpy_forward(w, ids, tt, lens)
     assert np.allclose(sig, want_s, rtol=1e-3, atol=1e-4)
     assert np.allclose(logits, want_l, rtol=1e-2, atol=2e-3)
+    _assert_logits_within_emulated_tolerance(w, ids, tt, lens, logits)
 
 
 @pytest.mark.parametrize("seq_len", [200, 256, 320])
@@ -81,6 +96,7 @@ def test_windows_longer_than_128_tokens(engine, seq_len):
     want_l, want_s = ce_oracle.numpy_forward(w, ids, tt, lens)
     assert want_s.max() - want_s.min() > 0.2
     assert np.allclose(sig, want_s, rtol=2e-3, atol=2e-4), np.abs(sig - want_s).max()   # 5 x the init scale of the path's test
+    _assert_logits_within_emulated_tolerance(w, ids, tt, lens, logits)
 
 
 def test_minilm_l6_vs_huggingface_oracle(engine):
@@ -92,6 +108,8 @@ def test_minilm_l6_vs_huggingface_oracle(engine):
     want_l, want_s = ce_oracle.hf_scores(model, ids, tt, lens)
     assert np.all((sig >= 0) & (sig <= 1))  # Source.score in [0, 1] (reference api/app.py:157)
     assert np.allclose(sig, want_s, rtol=1e-3, atol=1e-4), np.abs(sig - want_s).max()
+    # the fp64 forward of the same weights (pinned to HuggingFace on the CPU) at the device-emulation tolerance
+    _assert_logits_within_emulated_tolerance(w, ids, tt, lens, logits)
     # batch-size independence: 100 pairs in one call == the same pairs in slices
     ids2, tt2, lens2 = _pairs(100, 128)
     a = engine.ce_score(ids2, tt2, lens2)[1]
