@@ -40,3 +40,54 @@ def test_select_dev_matches_host_selector(engine, dtype):
             assert [str(int(i) - 1000) for i in ids[b, :n_sel[b]]] == [d.id for d in want]
             assert [float(x) for x in sc[b, :n_sel[b]]] == [d.metadata["score"] for d in want]
             assert np.all(ids[b, n_sel[b]:] == -1)
+
+
+@pytest.mark.parametrize("dtype", ["float32", "float64"])
+def test_select_dev_at_the_shared_memory_limit(engine, dtype):
+    """k = 4094 candidates (the 48 KB limit of the per-query sort), top_k >= k, and candidate ids outside the loaded
+    doc_chars range, which the selector treats as blank documents."""
+    import torch
+
+    rng = np.random.default_rng(6)
+    n_docs, base, B, k = 500, 1000, 5, 4094
+    chars = rng.integers(0, 600, n_docs).astype(np.int32)
+    chars[rng.random(n_docs) < 0.1] = 0
+    engine.load_doc_chars(chars, id_base=base)
+    cand = rng.integers(base - 20, base + n_docs + 20, size=(B, k)).astype(np.int64)   # some outside the range
+    cand[:, :4] = [0, -1, base - 1, base + n_docs]
+    scores = np.round(rng.random((B, k)), 2).astype(dtype)
+    scores[:, :4] = 2.0                                    # the out-of-range ids are walked first
+    cnt = np.asarray([k, k - 1, 4000, 17, 0], np.int32)
+    inside = (cand >= base) & (cand < base + n_docs)
+    assert (~inside[:, :4]).all() and (~inside[:, 4:]).any()
+
+    def text_of(i):
+        return "x" * int(chars[i - base]) if base <= i < base + n_docs else ""
+
+    for top_k, max_tokens in [(k, 10 ** 8), (5000, 10 ** 8), (4100, 3000)]:
+        out = engine.select_dev(torch.from_numpy(cand).cuda(), torch.from_numpy(scores).cuda(),
+                                torch.from_numpy(cnt).cuda(), top_k, max_tokens)
+        torch.cuda.synchronize()
+        ids, sc, n_sel, toks = [t.cpu().numpy() for t in out]
+        for b in range(B):
+            cands = [Document(id=str(int(cand[b, j])), text=text_of(int(cand[b, j])),
+                              metadata={"score": float(scores[b, j])}) for j in range(int(cnt[b]))]
+            want, want_tokens = select_documents(cands, top_k, max_tokens)
+            assert int(n_sel[b]) == len(want) and int(toks[b]) == want_tokens, (b, top_k, max_tokens)
+            assert [str(int(i)) for i in ids[b, :n_sel[b]]] == [d.id for d in want]
+            assert [float(x) for x in sc[b, :n_sel[b]]] == [d.metadata["score"] for d in want]
+            assert np.all(ids[b, n_sel[b]:] == -1)
+            assert not set(ids[b, :n_sel[b]].tolist()) & {0, -1, base - 1, base + n_docs}
+
+
+def test_select_dev_beyond_the_shared_memory_limit_is_unsupported(engine):
+    import torch
+
+    from sentio_b200._lib import SentioB200Error
+
+    engine.load_doc_chars(np.ones(10, np.int32))
+    k = 4095
+    with pytest.raises(SentioB200Error, match=r"rc=-4\).*too large"):
+        engine.select_dev(torch.zeros((1, k), dtype=torch.int64, device="cuda"),
+                          torch.zeros((1, k), dtype=torch.float32, device="cuda"),
+                          torch.zeros(1, dtype=torch.int32, device="cuda"), 3, 100)
