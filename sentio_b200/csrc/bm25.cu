@@ -84,6 +84,11 @@ __global__ void bm25_dense_fill_kernel(const int64_t* __restrict__ indptr, const
 //                    over the S ranges -> thr[q], a lower bound of the global k-th best score
 //      kModeCollect: every doc with score > 0 and >= thr[q] is appended to the query's candidate list
 //      kModeDump   : the accumulators are written to out[q][doc] (sb_bm25_scores, the bit-exactness hook)
+//  * TERM BLOCKS: the per-term state of a query lives in shared memory, which holds at most range_term_block() terms
+//    (~1870 on an H100).  A longer query is scored in blocks of that many terms: every block but the last dumps its
+//    accumulators to `carry` ([nq][n_docs] fp64, in place), the next block starts from them instead of 0.0.  Each doc still
+//    receives its additions in query order, so the result is bit-identical to a single pass.  Blocks that start from
+//    `carry` run the CARRY instantiation; a query of one block runs the same code as before term blocks existed.
 constexpr int kRange = 8192;            // docs per range (= 16 warps x kSub)
 constexpr unsigned long long kPosZero = 0x8000000000000000ull;  // f64_orderable(+0.0)
 constexpr int kRsThreads = 512;
@@ -95,7 +100,7 @@ enum { kModeSample = 0, kModeCollect = 1, kModeDump = 2 };
 struct RangeParams {
   const int32_t* q_terms;
   const int32_t* q_off;  // offsets of THIS sub-batch (q_off[0] may be > 0)
-  int max_len;           // longest query of the sub-batch (sizes the per-term state in shared memory)
+  int max_len;           // terms of one block (sizes the per-term state in shared memory)
   int ranges_per_cta;
   const int64_t* indptr;
   const int32_t* post_doc;
@@ -112,6 +117,9 @@ struct RangeParams {
   unsigned long long* ckey;  // [nq][n_docs]   kModeCollect
   uint32_t* cidx;            // [nq][n_docs]
   double* dump;              // [nq][n_docs]   kModeDump
+  // term blocks of a long query: query qi scores terms [q_off[qi] + term_lo, +max_len) starting from carry[qi][doc]
+  int term_lo;
+  const double* carry;       // [nq][n_docs] scores of the earlier term blocks, nullptr = start from 0.0 (term_lo = 0)
 };
 
 // first p in [lo, hi) with a[p] >= target (hi if none); all 32 lanes of the warp participate and return the same value
@@ -152,7 +160,8 @@ __device__ __forceinline__ void sts_f64(uint32_t addr, double v) {
   asm volatile("st.shared.f64 [%0], %1;" ::"r"(addr), "d"(v) : "memory");
 }
 
-template <int MODE, bool PLUS>
+// CARRY: a term block after the first of a long query (p.carry != nullptr); the one-block path compiles without it
+template <int MODE, bool PLUS, bool CARRY>
 __global__ void __launch_bounds__(kRsThreads, 2) bm25_range_kernel(const RangeParams p) {
   extern __shared__ __align__(16) uint8_t rsm[];
   double* acc = reinterpret_cast<double*>(rsm);                               // [kRange]: warp w owns [w*kSub, (w+1)*kSub)
@@ -173,8 +182,8 @@ __global__ void __launch_bounds__(kRsThreads, 2) bm25_range_kernel(const RangePa
   const int64_t first = MODE == kModeSample ? ((int64_t)blockIdx.y * n_ranges) / gridDim.y
                                             : (int64_t)blockIdx.y * p.ranges_per_cta;
   const int64_t last = MODE == kModeSample ? first + 1 : min(first + (int64_t)p.ranges_per_cta, n_ranges);  // exclusive
-  const int q0 = p.q_off[qi];
-  const int len = min(p.q_off[qi + 1] - q0, p.max_len);
+  const int q0 = p.q_off[qi] + (CARRY ? p.term_lo : 0);
+  const int len = CARRY ? max(0, min(p.q_off[qi + 1] - q0, p.max_len)) : min(p.q_off[qi + 1] - q0, p.max_len);
   // per-term state shared by the CTA
   for (int j = tid; j < len; j += kRsThreads) {
     const int t = p.q_terms[q0 + j];
@@ -224,6 +233,12 @@ __global__ void __launch_bounds__(kRsThreads, 2) bm25_range_kernel(const RangePa
     const int32_t s0 = (int32_t)s0l;
     const int32_t s1 = (int32_t)min(s0l + kSub, p.n_docs);
     const int nd = s1 - s0;
+    if (CARRY) {   // later term block: continue from the scores of the earlier blocks
+      const double* cin = p.carry + (size_t)qi * p.n_docs + s0;
+#pragma unroll 1
+      for (int i = lane; i < nd; i += 32) a[i] = cin[i];
+      __syncwarp();
+    }
     for (int j = 0; j < len; ++j) {
       const double w = s_idf[j];
       if (w == 0.0) continue;  // warp-uniform
@@ -536,25 +551,73 @@ int pow2_at_least(int v) {
   return p;
 }
 
-size_t range_smem_bytes(int max_len) {
-  return (size_t)kRange * 8 + kRsWarps * 8 + (size_t)std::max(max_len, 1) * (8 + 8 + 4 + 4 + 4 * kRsWarps) + (kRange / 32) * 4 + 16;
+constexpr size_t kRangeSmemFixed = (size_t)kRange * 8 + kRsWarps * 8 + (kRange / 32) * 4 + 16;
+constexpr size_t kRangeSmemPerTerm = 8 + 8 + 4 + 4 + 4 * kRsWarps;
+
+size_t range_smem_bytes(int max_len) { return kRangeSmemFixed + (size_t)std::max(max_len, 1) * kRangeSmemPerTerm; }
+
+// Terms of one block: the most whose per-term state fits one CTA's shared memory next to the accumulators and the
+// largest static shared memory of the variant's six instantiations.  Longer queries are scored in term blocks.
+int range_term_block(sb_ctx* ctx, int* out) {
+  const bool plus = ctx->bm25.variant == SB_BM25_PLUS;
+  const void* fns[6] = {
+      plus ? (const void*)bm25_range_kernel<kModeSample, true, false> : (const void*)bm25_range_kernel<kModeSample, false, false>,
+      plus ? (const void*)bm25_range_kernel<kModeCollect, true, false> : (const void*)bm25_range_kernel<kModeCollect, false, false>,
+      plus ? (const void*)bm25_range_kernel<kModeDump, true, false> : (const void*)bm25_range_kernel<kModeDump, false, false>,
+      plus ? (const void*)bm25_range_kernel<kModeSample, true, true> : (const void*)bm25_range_kernel<kModeSample, false, true>,
+      plus ? (const void*)bm25_range_kernel<kModeCollect, true, true> : (const void*)bm25_range_kernel<kModeCollect, false, true>,
+      plus ? (const void*)bm25_range_kernel<kModeDump, true, true> : (const void*)bm25_range_kernel<kModeDump, false, true>};
+  size_t stat = 0;
+  for (const void* f : fns) {
+    cudaFuncAttributes fa;
+    SB_CUDA(cudaFuncGetAttributes(&fa, f));
+    stat = std::max(stat, fa.sharedSizeBytes);
+  }
+  const size_t avail = ctx->smem_optin > stat + kRangeSmemFixed ? ctx->smem_optin - stat - kRangeSmemFixed : 0;
+  SB_REQUIRE(avail >= kRangeSmemPerTerm, SB_ERR_UNSUPPORTED, "bm25: no room for the per-term state in shared memory");
+  *out = (int)std::min<size_t>(avail / kRangeSmemPerTerm, 1 << 30);
+  return SB_OK;
 }
 
-template <int MODE, bool PLUS>
-int launch_range_kernel(sb_ctx* ctx, const RangeParams& rp, int nq, int n_chunks, cudaStream_t st) {
+// L: the term block of range_term_block()
+template <int MODE, bool PLUS, bool CARRY>
+int launch_range_kernel(const RangeParams& rp, int L, int nq, int n_chunks, cudaStream_t st) {
+  SB_REQUIRE(rp.max_len <= L, SB_ERR_UNSUPPORTED, "bm25: a block of %d terms does not fit the per-CTA term state (max %d)",
+             rp.max_len, L);
   const size_t smem = range_smem_bytes(rp.max_len);
-  SB_REQUIRE(smem <= ctx->smem_optin, SB_ERR_UNSUPPORTED, "bm25: a query of %d terms does not fit the per-CTA term state",
-             rp.max_len);
-  SB_CUDA(cudaFuncSetAttribute(bm25_range_kernel<MODE, PLUS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  bm25_range_kernel<MODE, PLUS><<<dim3((unsigned)nq, (unsigned)n_chunks), kRsThreads, smem, st>>>(rp);
+  SB_CUDA(cudaFuncSetAttribute(bm25_range_kernel<MODE, PLUS, CARRY>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                               (int)smem));
+  bm25_range_kernel<MODE, PLUS, CARRY><<<dim3((unsigned)nq, (unsigned)n_chunks), kRsThreads, smem, st>>>(rp);
   SB_CUDA(cudaGetLastError());
   return SB_OK;
 }
 
 template <int MODE>
-int launch_range(sb_ctx* ctx, const RangeParams& rp, int nq, int n_chunks, cudaStream_t st) {
-  return ctx->bm25.variant == SB_BM25_PLUS ? launch_range_kernel<MODE, true>(ctx, rp, nq, n_chunks, st)
-                                           : launch_range_kernel<MODE, false>(ctx, rp, nq, n_chunks, st);
+int launch_range(sb_ctx* ctx, const RangeParams& rp, int L, int nq, int n_chunks, cudaStream_t st) {
+  const bool plus = ctx->bm25.variant == SB_BM25_PLUS;
+  if (rp.carry)
+    return plus ? launch_range_kernel<MODE, true, true>(rp, L, nq, n_chunks, st)
+                : launch_range_kernel<MODE, false, true>(rp, L, nq, n_chunks, st);
+  return plus ? launch_range_kernel<MODE, true, false>(rp, L, nq, n_chunks, st)
+              : launch_range_kernel<MODE, false, false>(rp, L, nq, n_chunks, st);
+}
+
+// Scores the term blocks of a long query that precede its last one into `carry` and points rp at the last block; a
+// batch whose queries fit one block (max_len <= L) is left untouched.  Expects rp.max_len = min(max_len, L).
+int score_leading_term_blocks(sb_ctx* ctx, RangeParams& rp, int max_len, int L, double* carry, int nq, int n_chunks,
+                              cudaStream_t st) {
+  if (max_len <= L) return SB_OK;
+  const int nblk = (max_len + L - 1) / L;
+  RangeParams dp = rp;
+  dp.dump = carry;
+  for (int blk = 0; blk + 1 < nblk; ++blk) {
+    dp.term_lo = blk * L;
+    dp.carry = blk ? carry : nullptr;
+    if (int rc = launch_range<kModeDump>(ctx, dp, L, nq, n_chunks, st)) return rc;
+  }
+  rp.term_lo = (nblk - 1) * L;
+  rp.carry = carry;
+  return SB_OK;
 }
 
 RangeParams range_params(sb_ctx* ctx, const int32_t* q_terms_dev, const int32_t* q_off_dev, int max_len) {
@@ -591,29 +654,38 @@ int bm25_topk_enqueue(sb_ctx* ctx, const int32_t* q_terms_dev, const int32_t* q_
   Bm25Index& ix = ctx->bm25;
   const int kpow2 = std::max(32, pow2_at_least(k));
   SB_REQUIRE(kpow2 <= 1024, SB_ERR_UNSUPPORTED, "bm25: top_k %d too large (max 1024)", k);
-  // sub-batch: the worst-case candidate lists ((key, idx) per doc per query) of a sub-batch stay under 1.5 GB
-  int64_t sbq = (int64_t)((1536ull << 20) / ((size_t)ix.n_docs * 12 + 1));
+  int L = 0, rc;
+  if ((rc = range_term_block(ctx, &L))) return rc;
+  const bool blocked = max_len > L;   // a query longer than one term block: its earlier blocks are carried in fp64
+  // sub-batch: the worst-case candidate lists ((key, idx) per doc per query) of a sub-batch, and the carried scores of
+  // a batch with a long query, stay under 1.5 GB
+  int64_t sbq = (int64_t)((1536ull << 20) / ((size_t)ix.n_docs * (blocked ? 20 : 12) + 1));
   sbq = std::max<int64_t>(1, std::min<int64_t>(sbq, B));
-  int rc;
   if ((rc = ctx->misc2_dev.reserve((size_t)sbq * ix.n_docs * 8 + (size_t)sbq * 16 + 64))) return rc;
   if ((rc = ctx->misc3_dev.reserve((size_t)sbq * ix.n_docs * 4 + 64))) return rc;
+  if (blocked && (rc = ctx->acc_dev.reserve((size_t)sbq * ix.n_docs * 8))) return rc;
   unsigned long long* ckey = ctx->misc2_dev.as<unsigned long long>();
   unsigned long long* thr = ckey + (size_t)sbq * ix.n_docs;
   int32_t* cnt = reinterpret_cast<int32_t*>(thr + sbq);
   uint32_t* cidx = ctx->misc3_dev.as<uint32_t>();
+  double* carry = blocked ? ctx->acc_dev.as<double>() : nullptr;
   const size_t fin_smem = (size_t)kBmStage * 12 + (size_t)kpow2 * 12 + 64;
   SB_CUDA(cudaFuncSetAttribute(bm25_final_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fin_smem));
   const int64_t n_ranges = (ix.n_docs + kRange - 1) / kRange;
   for (int b0 = 0; b0 < B; b0 += (int)sbq) {
     const int nq = (int)std::min<int64_t>(sbq, B - b0);
-    RangeParams rp = range_params(ctx, q_terms_dev, q_off_dev + b0, max_len);
+    RangeParams rp = range_params(ctx, q_terms_dev, q_off_dev + b0, std::min(max_len, L));
     rp.k = k;
     rp.thr = thr;
     rp.cnt = cnt;
     rp.ckey = ckey;
     rp.cidx = cidx;
+    rp.ranges_per_cta = ranges_per_cta(ctx, nq, n_ranges);   // the sample pass ignores it: one range per CTA
+    const int n_chunks = (int)((n_ranges + rp.ranges_per_cta - 1) / rp.ranges_per_cta);
     {
-      ProfScope ps(ctx, SB_PROF_BM25_SCORE, st, 2);
+      ProfScope ps(ctx, SB_PROF_BM25_SCORE, st, 2 + (blocked ? (max_len - 1) / L : 0));
+      // (0) a long query: every term block but the last one, accumulated into `carry`
+      if ((rc = score_leading_term_blocks(ctx, rp, max_len, L, carry, nq, n_chunks, st))) return rc;
       // (1) safe per-query lower bound of the k-th best score from S sample ranges (exact k-th best when S == 1)
       // (4 sample ranges: a sample CTA pays the full per-warp set-up -- one posting-list search per term -- for a single
       // sub-range, so 8 of them cost 21 % of the collect pass for 6.5 % of its docs; a lower bound from 4 is nearly as tight)
@@ -621,11 +693,9 @@ int bm25_topk_enqueue(sb_ctx* ctx, const int32_t* q_terms_dev, const int32_t* q_
       rp.k = (k + S - 1) / S;
       SB_CUDA(cudaMemsetAsync(thr, 0xff, (size_t)nq * 8, st));
       SB_CUDA(cudaMemsetAsync(cnt, 0, (size_t)nq * 4, st));
-      if ((rc = launch_range<kModeSample>(ctx, rp, nq, S, st))) return rc;
+      if ((rc = launch_range<kModeSample>(ctx, rp, L, nq, S, st))) return rc;
       // (2) score every range in shared memory, keep only docs that can still reach the top k
-      rp.ranges_per_cta = ranges_per_cta(ctx, nq, n_ranges);
-      const int n_chunks = (int)((n_ranges + rp.ranges_per_cta - 1) / rp.ranges_per_cta);
-      if ((rc = launch_range<kModeCollect>(ctx, rp, nq, n_chunks, st))) return rc;
+      if ((rc = launch_range<kModeCollect>(ctx, rp, L, nq, n_chunks, st))) return rc;
     }
     ProfScope ps(ctx, SB_PROF_BM25_SELECT, st, 1);
     // (3) exact k-th largest by radix select over the (few) candidates, ties by ascending doc index, sort the winners
@@ -880,14 +950,18 @@ int sb_bm25_scores(sb_ctx* ctx, const int32_t* q_terms, int32_t n_q, double* out
   if (n_q) SB_CUDA(cudaMemcpyAsync(ctx->q_dev.p, q_terms, (size_t)n_q * 4, cudaMemcpyHostToDevice, st));
   SB_CUDA(cudaMemcpyAsync(ctx->q_dev.as<uint8_t>() + tb, off, 8, cudaMemcpyHostToDevice, st));
   if ((rc = ctx->acc_dev.reserve((size_t)ix.n_docs * sizeof(double)))) return rc;
+  int L = 0;
+  if ((rc = range_term_block(ctx, &L))) return rc;
   RangeParams rp = range_params(ctx, ctx->q_dev.as<int32_t>(),
-                                reinterpret_cast<const int32_t*>(ctx->q_dev.as<uint8_t>() + tb), n_q);
+                                reinterpret_cast<const int32_t*>(ctx->q_dev.as<uint8_t>() + tb), std::min<int>(n_q, L));
   rp.dump = ctx->acc_dev.as<double>();
   const int64_t n_ranges = (ix.n_docs + kRange - 1) / kRange;
   rp.ranges_per_cta = ranges_per_cta(ctx, 1, n_ranges);
-  ctx->launches += 1;
-  if ((rc = launch_range<kModeDump>(ctx, rp, 1, (int)((n_ranges + rp.ranges_per_cta - 1) / rp.ranges_per_cta), st)))
-    return rc;
+  const int n_chunks = (int)((n_ranges + rp.ranges_per_cta - 1) / rp.ranges_per_cta);
+  ctx->launches += 1 + (n_q > L ? (n_q - 1) / L : 0);
+  // a long query: its earlier term blocks are dumped into the output buffer, and each next block continues from it
+  if ((rc = score_leading_term_blocks(ctx, rp, n_q, L, rp.dump, 1, n_chunks, st))) return rc;
+  if ((rc = launch_range<kModeDump>(ctx, rp, L, 1, n_chunks, st))) return rc;
   SB_CUDA(cudaMemcpyAsync(out_scores, ctx->acc_dev.p, (size_t)ix.n_docs * 8, cudaMemcpyDeviceToHost, st));
   SB_CUDA(cudaStreamSynchronize(st));
   return SB_OK;

@@ -43,6 +43,42 @@ def test_gpu_build_equals_host_build(engine, variant, n, vocab):
         assert np.array_equal(engine.bm25_scores(t), s)
 
 
+def _edge_stream(kind):
+    if kind == "empty_docs":     # zero-length docs first, last and in runs between non-empty ones
+        lens = np.array([0, 3, 0, 0, 5, 1, 0, 2, 0])
+        flat = np.arange(lens.sum()) % 4 + 10
+    elif kind == "tf_max":       # one term 65535 times in a doc (the uint16 limit), next to ordinary docs
+        lens = np.array([2, 65535, 3, 65536])
+        flat = np.concatenate([[1, 2], np.full(65535, 7), [7, 1, 3], np.full(65535, 1), [7]])
+    else:                        # a single doc
+        lens = np.array([4])
+        flat = np.array([9, 4, 9, 9])
+    off = np.zeros(len(lens) + 1, np.int64)
+    np.cumsum(lens, out=off[1:])
+    return flat.astype(np.int32), off
+
+
+@pytest.mark.parametrize("kind", ["empty_docs", "tf_max", "one_doc"])
+@pytest.mark.parametrize("variant", ["okapi", "plus"])
+def test_gpu_build_equals_host_build_at_the_edges(engine, kind, variant):
+    flat, off = _edge_stream(kind)
+    want = build_bm25_from_token_ids(flat, off, variant=variant)
+    got = engine.build_bm25_gpu(flat, off, variant=variant, export=True)
+    _assert_same_index(got, want)
+    if kind == "tf_max":
+        assert want.post_tf.max() == 65535
+    terms = [got.term_ids(q) for q in ([7], [1, 7, 3], [9, 4, 9], [10, 11, 12, 13], [2, 99])]
+    a = engine.bm25_topk(terms, 8)
+    sc_a = [engine.bm25_scores(t) for t in terms]
+    engine.load_bm25(want)
+    b = engine.bm25_topk(terms, 8)
+    for x, y in zip(a, b):
+        assert np.array_equal(x.view(np.uint64) if x.dtype == np.float64 else x,
+                              y.view(np.uint64) if y.dtype == np.float64 else y)
+    for t, s in zip(terms, sc_a):
+        assert np.array_equal(engine.bm25_scores(t).view(np.uint64), s.view(np.uint64))
+
+
 def test_gpu_build_without_export_keeps_postings_on_device(engine):
     flat, off = synth.text_corpus_tokens(5000, vocab=700)
     want = build_bm25_from_token_ids(flat, off)
