@@ -289,6 +289,32 @@ int sb_bm25_topk_dev(sb_ctx* ctx, const int32_t* q_terms_dev, const int32_t* q_o
                      int32_t* out_counts_dev, void* stream);
 /* full score vector of ONE query (fp64, n_docs entries) -- bit-exactness checks against get_scores */
 int sb_bm25_scores(sb_ctx* ctx, const int32_t* q_terms, int32_t n_q, double* out_scores);
+/*
+ * Filtered BM25 -- the conditions of sb_dense_topk_filtered applied to the BM25 index (DESIGN.md K2 "Filtered BM25 and
+ * hybrid"), so a tenant- or source-restricted query can use sparse and hybrid retrieval.
+ *
+ * sb_bm25_tags_load: the payload index of the installed BM25 index for field `field` (< SB_MAX_TAG_FIELDS): codes[n]
+ * holds one code per doc (>= 0), -1 = the doc's payload lacks the key; n must equal sb_bm25_count.  The columns belong
+ * to the installed index: sb_bm25_load / sb_bm25_build_finish free them (a failed install keeps the old index and its
+ * columns).  Codes come from one dictionary for the whole corpus, so the shards of a partitioned corpus share them.
+ * sb_bm25_topk_filtered: as sb_bm25_topk (which it extends), over the docs that satisfy each query's conditions (CSR
+ * f_off[B+1] / f_field / f_code, meaning as for sb_dense_topk_filtered; f_code < 0 matches nothing, a query without
+ * conditions is unfiltered).  Result: sb_bm25_topk's order (score desc, id asc, score > 0) restricted to the matching
+ * docs, scores bit-identical; out_counts[b] = min(k, matching docs with score > 0).  Under BM25Plus a matching doc
+ * without any query term still scores idf * delta.  Every condition is checked before the first launch: a field out of
+ * range is SB_ERR_ARG, a field without a BM25 column SB_ERR_STATE.  A batch without conditions runs sb_bm25_topk's path.
+ * sb_bm25_topk_filtered_dev: the same on device buffers (f_off_dev[B+1], f_field_dev / f_code_dev[n_conds]), a pure
+ * enqueue: the kernels read the conditions from device memory, so they are not checked on the host -- a condition
+ * naming a field out of range or without a column matches no doc.
+ */
+int sb_bm25_tags_load(sb_ctx* ctx, int32_t field, const int32_t* codes, int64_t n);
+int sb_bm25_topk_filtered(sb_ctx* ctx, const int32_t* q_terms, const int32_t* q_off, int32_t B, int32_t k,
+                          const int32_t* f_off, const int32_t* f_field, const int32_t* f_code, int64_t* out_ids,
+                          double* out_scores, int32_t* out_counts);
+int sb_bm25_topk_filtered_dev(sb_ctx* ctx, const int32_t* q_terms_dev, const int32_t* q_off_dev, int32_t B,
+                              int32_t n_q_terms, int32_t max_q_len, int32_t k, const int32_t* f_off_dev, int32_t n_conds,
+                              const int32_t* f_field_dev, const int32_t* f_code_dev, int64_t* out_ids_dev,
+                              double* out_scores_dev, int32_t* out_counts_dev, void* stream);
 
 /* ---------------------------------------------------------------- K3: fusion -------------------------------- */
 /*
@@ -326,6 +352,17 @@ int sb_fuse_dev(sb_ctx* ctx, int32_t method, double rrf_k, double w_dense, doubl
 int sb_hybrid_topk(sb_ctx* ctx, const float* q, const int32_t* q_terms, const int32_t* q_off, int32_t B, int32_t k,
                    int32_t method, double rrf_k, double w_dense, double w_sparse, int64_t* out_ids, double* out_scores,
                    int32_t* out_src, int32_t* out_counts);
+/*
+ * sb_hybrid_topk_filtered: sb_hybrid_topk (which it extends) with one CSR of conditions per query (f_off[B+1] / f_field /
+ * f_code as sb_dense_topk_filtered) applied to BOTH signals: field f means dense slot 0's tag column f and the BM25
+ * column f, and both must be loaded (SB_ERR_STATE).  The dense list is sb_dense_topk_filtered's, the sparse list
+ * sb_bm25_topk_filtered's, fusion is unchanged: it sees two lists that hold only matching docs.  A batch without
+ * conditions runs sb_hybrid_topk's path.
+ */
+int sb_hybrid_topk_filtered(sb_ctx* ctx, const float* q, const int32_t* q_terms, const int32_t* q_off, int32_t B,
+                            int32_t k, const int32_t* f_off, const int32_t* f_field, const int32_t* f_code,
+                            int32_t method, double rrf_k, double w_dense, double w_sparse, int64_t* out_ids,
+                            double* out_scores, int32_t* out_src, int32_t* out_counts);
 /*
  * sb_hybrid_rerank_topk: the same followed by the cross-encoder rerank of rerank_node (reference
  * src/core/graph/nodes.py:138-227 / jina_reranker.py:192-295) on the fused top-k: q_tok [B x lq] word pieces and q_len [B]

@@ -78,6 +78,12 @@ SIGNATURES = {
     "sb_bm25_topk_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "sb_bm25_scores": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]),
+    "sb_bm25_tags_load": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int64]),
+    "sb_bm25_topk_filtered": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "sb_bm25_topk_filtered_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
+                                            C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.c_void_p, C.c_void_p, C.c_void_p]),
     "sb_fuse": (C.c_int, [C.c_void_p, C.c_int32, C.c_double, C.c_double, C.c_double, C.c_int32,
                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
@@ -116,6 +122,9 @@ SIGNATURES = {
                                   C.c_int32, C.c_int32, C.c_void_p]),
     "sb_hybrid_topk": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_double,
                                  C.c_double, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "sb_hybrid_topk_filtered": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p,
+                                          C.c_void_p, C.c_void_p, C.c_int32, C.c_double, C.c_double, C.c_double,
+                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "sb_hybrid_rerank_topk": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
                                         C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_double,
                                         C.c_double, C.c_void_p, C.c_void_p, C.c_void_p]),

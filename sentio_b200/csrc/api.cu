@@ -79,6 +79,8 @@ void sb_destroy(sb_ctx* ctx) {
   if (b.idf) cudaFree(b.idf);
   if (b.dense_of_term) cudaFree(b.dense_of_term);
   if (b.dense_ratio) cudaFree(b.dense_ratio);
+  for (int f = 0; f < SB_MAX_TAG_FIELDS; ++f)
+    if (b.tags[f]) cudaFree(b.tags[f]);
   if (ctx->ce) ce_model_free(ctx->ce);
   if (ctx->enc) ce_model_free(ctx->enc);
   if (ctx->ce_tokens) ce_tokens_free(ctx->ce_tokens);

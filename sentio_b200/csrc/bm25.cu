@@ -120,7 +120,25 @@ struct RangeParams {
   // term blocks of a long query: query qi scores terms [q_off[qi] + term_lo, +max_len) starting from carry[qi][doc]
   int term_lo;
   const double* carry;       // [nq][n_docs] scores of the earlier term blocks, nullptr = start from 0.0 (term_lo = 0)
+  // FILTER: query qi's conditions are entries [f_off[qi], f_off[qi+1]) of f_field / f_code (f_off: THIS sub-batch, like
+  // q_off); a doc matches iff tags[f_field[i]][doc] == f_code[i] >= 0 for every i.  The column pointers travel by value
+  // so the kernel needs no device-side table; a field out of range or without a column matches nothing
+  const int32_t* f_off;
+  const int32_t* f_field;
+  const int32_t* f_code;
+  const int32_t* tags[SB_MAX_TAG_FIELDS];
 };
+
+// the conjunction of query qi's conditions [c0, c1) for one doc (no condition: every doc matches)
+__device__ __forceinline__ bool doc_matches(const RangeParams& p, int c0, int c1, int32_t doc) {
+  for (int i = c0; i < c1; ++i) {
+    const int f = __ldg(p.f_field + i);
+    const int32_t code = __ldg(p.f_code + i);
+    const int32_t* col = (unsigned)f < (unsigned)SB_MAX_TAG_FIELDS ? p.tags[f] : nullptr;
+    if (code < 0 || col == nullptr || __ldg(col + doc) != code) return false;
+  }
+  return true;
+}
 
 // first p in [lo, hi) with a[p] >= target (hi if none); all 32 lanes of the warp participate and return the same value
 __device__ __forceinline__ int64_t warp_lower_bound(const int32_t* __restrict__ a, int64_t lo, int64_t hi, int32_t target,
@@ -160,9 +178,12 @@ __device__ __forceinline__ void sts_f64(uint32_t addr, double v) {
   asm volatile("st.shared.f64 [%0], %1;" ::"r"(addr), "d"(v) : "memory");
 }
 
-// CARRY: a term block after the first of a long query (p.carry != nullptr); the one-block path compiles without it
-template <int MODE, bool PLUS, bool CARRY>
+// CARRY: a term block after the first of a long query (p.carry != nullptr); the one-block path compiles without it.
+// FILTER (sample and collect only): docs that fail the query's conditions are dropped where a sub-range is consumed --
+// the scoring itself is unchanged, so every score stays bit-identical; the unfiltered path compiles without it
+template <int MODE, bool PLUS, bool CARRY, bool FILTER = false>
 __global__ void __launch_bounds__(kRsThreads, 2) bm25_range_kernel(const RangeParams p) {
+  static_assert(!FILTER || MODE != kModeDump, "bm25: dump mode is never filtered");
   extern __shared__ __align__(16) uint8_t rsm[];
   double* acc = reinterpret_cast<double*>(rsm);                               // [kRange]: warp w owns [w*kSub, (w+1)*kSub)
   double* s_dummy = acc + kRange;                                             // [kRsWarps] 0.0, read by out-of-range postings
@@ -330,7 +351,9 @@ __global__ void __launch_bounds__(kRsThreads, 2) bm25_range_kernel(const RangePa
       for (int i = lane; i < kSub; i += 32) {
         const double sv = a[i];
         a[i] = 0.0;
-        const bool pass = i < nd && sv > 0.0 && sv >= td && sv <= 1.7976931348623157e308;  // finite positive (NaN fails)
+        bool pass = i < nd && sv > 0.0 && sv >= td && sv <= 1.7976931348623157e308;  // finite positive (NaN fails)
+        // the conditions are read only for the few docs that already passed the score test
+        if (FILTER && pass) pass = doc_matches(p, p.f_off[qi], p.f_off[qi + 1], s0 + i);
         const unsigned m = __ballot_sync(0xffffffffu, pass);
         if (m) {
           int at = 0;
@@ -355,9 +378,12 @@ __global__ void __launch_bounds__(kRsThreads, 2) bm25_range_kernel(const RangePa
     if (tid == 0) npos = 0;
     __syncthreads();
     int local = 0;
+    const int c0 = FILTER ? p.f_off[qi] : 0, c1 = FILTER ? p.f_off[qi + 1] : 0;
     for (int i = tid; i < kRange; i += kRsThreads) {
       const double sc = acc[i];
-      const unsigned long long key = (i < nd && sc > 0.0) ? f64_orderable(sc) : 0ull;
+      // FILTER: a doc that fails the conditions gets key 0, like a non-positive score
+      const bool pos = i < nd && sc > 0.0 && (!FILTER || doc_matches(p, c0, c1, r0 + i));
+      const unsigned long long key = pos ? f64_orderable(sc) : 0ull;
       keys[i] = key;
       local += key != 0ull;
     }
@@ -366,7 +392,8 @@ __global__ void __launch_bounds__(kRsThreads, 2) bm25_range_kernel(const RangePa
     __syncthreads();
     // S sample ranges each report their ceil(k / S)-th best positive score; at least k docs score >= the MINIMUM of
     // those, so it is a lower bound of the global k-th best (a range with too few positives degrades the bound to
-    // "every positive score", never below).  thr[] was preset to all-ones by the host.
+    // "every positive score", never below).  thr[] was preset to all-ones by the host.  FILTER: the same argument over
+    // the matching docs only (non-matching ones hold key 0), so the bound holds for the k-th best MATCHING score.
     unsigned long long t = kPosZero + 1ull;
     if (npos >= p.k) t = block_kth_largest(keys, kRange, p.k, hist, scal, 3);  // sign + exponent + 12 mantissa bits
     if (tid == 0) atomicMin(p.thr + qi, t);
@@ -580,21 +607,32 @@ int range_term_block(sb_ctx* ctx, int* out) {
 }
 
 // L: the term block of range_term_block()
-template <int MODE, bool PLUS, bool CARRY>
+template <int MODE, bool PLUS, bool CARRY, bool FILTER = false>
 int launch_range_kernel(const RangeParams& rp, int L, int nq, int n_chunks, cudaStream_t st) {
   SB_REQUIRE(rp.max_len <= L, SB_ERR_UNSUPPORTED, "bm25: a block of %d terms does not fit the per-CTA term state (max %d)",
              rp.max_len, L);
   const size_t smem = range_smem_bytes(rp.max_len);
-  SB_CUDA(cudaFuncSetAttribute(bm25_range_kernel<MODE, PLUS, CARRY>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+  SB_CUDA(cudaFuncSetAttribute(bm25_range_kernel<MODE, PLUS, CARRY, FILTER>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                (int)smem));
-  bm25_range_kernel<MODE, PLUS, CARRY><<<dim3((unsigned)nq, (unsigned)n_chunks), kRsThreads, smem, st>>>(rp);
+  bm25_range_kernel<MODE, PLUS, CARRY, FILTER><<<dim3((unsigned)nq, (unsigned)n_chunks), kRsThreads, smem, st>>>(rp);
   SB_CUDA(cudaGetLastError());
   return SB_OK;
 }
 
+// rp.f_off != nullptr selects the FILTER instantiations (sample and collect modes; the FILTER kernels declare the same
+// static shared memory as the others, so range_term_block() holds for them too)
 template <int MODE>
 int launch_range(sb_ctx* ctx, const RangeParams& rp, int L, int nq, int n_chunks, cudaStream_t st) {
   const bool plus = ctx->bm25.variant == SB_BM25_PLUS;
+  if constexpr (MODE != kModeDump) {
+    if (rp.f_off) {
+      if (rp.carry)
+        return plus ? launch_range_kernel<MODE, true, true, true>(rp, L, nq, n_chunks, st)
+                    : launch_range_kernel<MODE, false, true, true>(rp, L, nq, n_chunks, st);
+      return plus ? launch_range_kernel<MODE, true, false, true>(rp, L, nq, n_chunks, st)
+                  : launch_range_kernel<MODE, false, false, true>(rp, L, nq, n_chunks, st);
+    }
+  }
   if (rp.carry)
     return plus ? launch_range_kernel<MODE, true, true>(rp, L, nq, n_chunks, st)
                 : launch_range_kernel<MODE, false, true>(rp, L, nq, n_chunks, st);
@@ -610,6 +648,7 @@ int score_leading_term_blocks(sb_ctx* ctx, RangeParams& rp, int max_len, int L, 
   const int nblk = (max_len + L - 1) / L;
   RangeParams dp = rp;
   dp.dump = carry;
+  dp.f_off = nullptr;   // the leading blocks only sum scores: the filter acts where the last block is consumed
   for (int blk = 0; blk + 1 < nblk; ++blk) {
     dp.term_lo = blk * L;
     dp.carry = blk ? carry : nullptr;
@@ -649,8 +688,12 @@ int ranges_per_cta(sb_ctx* ctx, int nq, int64_t n_ranges) {
   return (int)r;
 }
 
+// f_off_dev != nullptr: the filtered top-k (conditions f_off_dev [B+1] / f_field_dev / f_code_dev on the device, checked
+// by the caller); nullptr: exactly the unfiltered path
 int bm25_topk_enqueue(sb_ctx* ctx, const int32_t* q_terms_dev, const int32_t* q_off_dev, int B, int max_len, int k,
-                      int64_t* out_ids, double* out_scores, int32_t* out_counts, cudaStream_t st) {
+                      int64_t* out_ids, double* out_scores, int32_t* out_counts, cudaStream_t st,
+                      const int32_t* f_off_dev = nullptr, const int32_t* f_field_dev = nullptr,
+                      const int32_t* f_code_dev = nullptr) {
   Bm25Index& ix = ctx->bm25;
   const int kpow2 = std::max(32, pow2_at_least(k));
   SB_REQUIRE(kpow2 <= 1024, SB_ERR_UNSUPPORTED, "bm25: top_k %d too large (max 1024)", k);
@@ -680,6 +723,12 @@ int bm25_topk_enqueue(sb_ctx* ctx, const int32_t* q_terms_dev, const int32_t* q_
     rp.cnt = cnt;
     rp.ckey = ckey;
     rp.cidx = cidx;
+    if (f_off_dev) {
+      rp.f_off = f_off_dev + b0;
+      rp.f_field = f_field_dev;
+      rp.f_code = f_code_dev;
+      memcpy(rp.tags, ix.tags, sizeof(rp.tags));
+    }
     rp.ranges_per_cta = ranges_per_cta(ctx, nq, n_ranges);   // the sample pass ignores it: one range per CTA
     const int n_chunks = (int)((n_ranges + rp.ranges_per_cta - 1) / rp.ranges_per_cta);
     {
@@ -729,6 +778,8 @@ static void bm25_index_free(Bm25Index& ix) {
   if (ix.idf) cudaFree(ix.idf);
   if (ix.dense_of_term) cudaFree(ix.dense_of_term);
   if (ix.dense_ratio) cudaFree(ix.dense_ratio);
+  for (int f = 0; f < SB_MAX_TAG_FIELDS; ++f)
+    if (ix.tags[f]) cudaFree(ix.tags[f]);
   ix = Bm25Index();
 }
 
@@ -821,6 +872,115 @@ int bm25_install_device_csr(sb_ctx* ctx, int64_t* indptr_dev, int32_t* post_doc_
   return SB_OK;
 }
 
+// Checks a host CSR of conditions before anything is launched: f_off[0] == 0 and non-decreasing, every field in range
+// (SB_ERR_ARG) with a BM25 column loaded and, for the hybrid path, dense slot 0's column too (SB_ERR_STATE).
+int bm25_check_conditions(sb_ctx* ctx, const char* who, int B, const int32_t* f_off, const int32_t* f_field,
+                          bool dense_too) {
+  SB_REQUIRE(f_off[0] == 0, SB_ERR_ARG, "%s: f_off[0] must be 0", who);
+  for (int b = 0; b < B; ++b)
+    SB_REQUIRE(f_off[b + 1] >= f_off[b], SB_ERR_ARG, "%s: f_off is not non-decreasing at %d", who, b);
+  for (int i = 0; i < f_off[B]; ++i) {
+    const int f = f_field[i];
+    SB_REQUIRE(f >= 0 && f < SB_MAX_TAG_FIELDS, SB_ERR_ARG, "%s: field %d out of range", who, f);
+    SB_REQUIRE(ctx->bm25.tags[f] != nullptr, SB_ERR_STATE, "%s: field %d has no BM25 tag column loaded", who, f);
+    SB_REQUIRE(!dense_too || ctx->dense[0].tags[f] != nullptr, SB_ERR_STATE,
+               "%s: field %d has no tag column loaded in dense slot 0", who, f);
+  }
+  return SB_OK;
+}
+
+namespace {
+
+int bm25_topk_dev_call(sb_ctx* ctx, const char* who, const int32_t* q_terms_dev, const int32_t* q_off_dev, int32_t B,
+                       int32_t n_q_terms, int32_t max_q_len, int32_t k, const int32_t* f_off_dev, int32_t n_conds,
+                       const int32_t* f_field_dev, const int32_t* f_code_dev, int64_t* out_ids_dev,
+                       double* out_scores_dev, int32_t* out_counts_dev, void* stream) {
+  SB_REQUIRE(ctx != nullptr, SB_ERR_ARG, "%s: ctx is NULL", who);
+  SB_REQUIRE(B >= 0 && k > 0 && max_q_len >= 0 && n_q_terms >= 0 && n_conds >= 0, SB_ERR_ARG, "%s: bad sizes", who);
+  if (B == 0) return SB_OK;
+  SB_REQUIRE(q_off_dev && out_ids_dev && out_scores_dev && out_counts_dev, SB_ERR_ARG, "%s: NULL buffer", who);
+  SB_REQUIRE(n_conds == 0 || (f_off_dev && f_field_dev && f_code_dev), SB_ERR_ARG, "%s: NULL conditions", who);
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  DeviceGuard g(ctx->device);
+  cudaStream_t st = pick_stream(ctx, stream);
+  if (ctx->bm25.n_docs == 0 || ctx->bm25.indptr == nullptr) {
+    bm25_fill_empty_kernel<<<(B * k + 255) / 256, 256, 0, st>>>(out_ids_dev, out_scores_dev, out_counts_dev, B, k);
+    SB_CUDA(cudaGetLastError());
+    return SB_OK;
+  }
+  // no condition in the batch: exactly the unfiltered path
+  return bm25_topk_enqueue(ctx, q_terms_dev, q_off_dev, B, max_q_len, k, out_ids_dev, out_scores_dev, out_counts_dev,
+                           st, n_conds ? f_off_dev : nullptr, f_field_dev, f_code_dev);
+}
+
+// Host form of the (filtered) top-k: one H2D of the query terms (and the conditions), the search, one D2H.  f_off ==
+// nullptr or no condition in the batch: exactly the unfiltered staging and path.
+int bm25_topk_host(sb_ctx* ctx, const char* who, const int32_t* q_terms, const int32_t* q_off, int32_t B, int32_t k,
+                   const int32_t* f_off, const int32_t* f_field, const int32_t* f_code, int64_t* out_ids,
+                   double* out_scores, int32_t* out_counts) {
+  SB_REQUIRE(ctx != nullptr, SB_ERR_ARG, "%s: ctx is NULL", who);
+  SB_REQUIRE(B >= 0 && k > 0, SB_ERR_ARG, "%s: bad B=%d k=%d", who, B, k);
+  if (B == 0) return SB_OK;
+  SB_REQUIRE(q_off && out_ids && out_scores && out_counts, SB_ERR_ARG, "%s: NULL buffer", who);
+  const int n_terms_q = q_off[B];
+  SB_REQUIRE(n_terms_q >= 0 && (n_terms_q == 0 || q_terms), SB_ERR_ARG, "%s: bad query term buffers", who);
+  int max_len = 0;
+  for (int b = 0; b < B; ++b) {
+    SB_REQUIRE(q_off[b + 1] >= q_off[b], SB_ERR_ARG, "%s: q_off must be non-decreasing", who);
+    max_len = std::max(max_len, q_off[b + 1] - q_off[b]);
+  }
+  std::unique_lock<std::mutex> lk(ctx->mu);
+  const int n_conds = f_off ? f_off[B] : 0;
+  if (f_off) {
+    int rc;
+    if ((rc = bm25_check_conditions(ctx, who, B, f_off, f_field, false))) return rc;
+  }
+  DeviceGuard g(ctx->device);
+  cudaStream_t st = ctx->stream;
+  if (ctx->bm25.n_docs == 0 || ctx->bm25.indptr == nullptr) {
+    for (int i = 0; i < B * k; ++i) { out_ids[i] = -1; out_scores[i] = 0.0; }
+    for (int i = 0; i < B; ++i) out_counts[i] = 0;
+    return SB_OK;
+  }
+  int rc;
+  const size_t tb = (size_t)std::max(n_terms_q, 1) * 4, ob = (size_t)(B + 1) * 4;
+  const size_t cb = n_conds ? ob + (size_t)n_conds * 8 : 0;   // f_off | f_field | f_code
+  if ((rc = ctx->pin_in.reserve(tb + ob + cb))) return rc;
+  if ((rc = ctx->q_dev.reserve(tb + ob + cb))) return rc;
+  uint8_t* pi = ctx->pin_in.as<uint8_t>();
+  if (n_terms_q) memcpy(pi, q_terms, (size_t)n_terms_q * 4);
+  memcpy(pi + tb, q_off, ob);
+  if (n_conds) {
+    memcpy(pi + tb + ob, f_off, ob);
+    memcpy(pi + tb + 2 * ob, f_field, (size_t)n_conds * 4);
+    memcpy(pi + tb + 2 * ob + (size_t)n_conds * 4, f_code, (size_t)n_conds * 4);
+  }
+  SB_CUDA(cudaMemcpyAsync(ctx->q_dev.p, pi, tb + ob + cb, cudaMemcpyHostToDevice, st));
+  const int32_t* qt_dev = ctx->q_dev.as<int32_t>();
+  const int32_t* qo_dev = reinterpret_cast<const int32_t*>(ctx->q_dev.as<uint8_t>() + tb);
+  const int32_t* fo_dev = n_conds ? qo_dev + (B + 1) : nullptr;
+  const size_t nid = (size_t)B * k;
+  if ((rc = ctx->out_ids_dev.reserve(nid * 8))) return rc;
+  if ((rc = ctx->out_sc_dev.reserve(nid * 8))) return rc;
+  if ((rc = ctx->out_cnt_dev.reserve((size_t)B * 4))) return rc;
+  if ((rc = bm25_topk_enqueue(ctx, qt_dev, qo_dev, B, max_len, k, ctx->out_ids_dev.as<int64_t>(),
+                              ctx->out_sc_dev.as<double>(), ctx->out_cnt_dev.as<int32_t>(), st, fo_dev,
+                              n_conds ? fo_dev + (B + 1) : nullptr, n_conds ? fo_dev + (B + 1) + n_conds : nullptr)))
+    return rc;
+  if ((rc = ctx->pin_out.reserve(nid * 16 + (size_t)B * 4))) return rc;
+  uint8_t* po = ctx->pin_out.as<uint8_t>();
+  SB_CUDA(cudaMemcpyAsync(po, ctx->out_ids_dev.p, nid * 8, cudaMemcpyDeviceToHost, st));
+  SB_CUDA(cudaMemcpyAsync(po + nid * 8, ctx->out_sc_dev.p, nid * 8, cudaMemcpyDeviceToHost, st));
+  SB_CUDA(cudaMemcpyAsync(po + nid * 16, ctx->out_cnt_dev.p, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
+  SB_CUDA(cudaStreamSynchronize(st));
+  memcpy(out_ids, po, nid * 8);
+  memcpy(out_scores, po + nid * 8, nid * 8);
+  memcpy(out_counts, po + nid * 16, (size_t)B * 4);
+  return SB_OK;
+}
+
+}  // namespace
+
 extern "C" {
 
 int sb_bm25_load(sb_ctx* ctx, const int64_t* indptr, const int32_t* post_doc, const uint16_t* post_tf,
@@ -865,73 +1025,59 @@ int sb_bm25_load(sb_ctx* ctx, const int64_t* indptr, const int32_t* post_doc, co
 
 int64_t sb_bm25_count(sb_ctx* ctx) { return ctx ? ctx->bm25.n_docs : -1; }
 
+int sb_bm25_tags_load(sb_ctx* ctx, int32_t field, const int32_t* codes, int64_t n) {
+  SB_REQUIRE(ctx != nullptr, SB_ERR_ARG, "sb_bm25_tags_load: ctx is NULL");
+  SB_REQUIRE(field >= 0 && field < SB_MAX_TAG_FIELDS, SB_ERR_ARG, "sb_bm25_tags_load: field %d out of range [0,%d)", field,
+             SB_MAX_TAG_FIELDS);
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  DeviceGuard g(ctx->device);
+  Bm25Index& ix = ctx->bm25;
+  SB_REQUIRE(ix.indptr != nullptr, SB_ERR_STATE, "sb_bm25_tags_load: no BM25 index loaded");
+  SB_REQUIRE(n == ix.n_docs, SB_ERR_ARG, "sb_bm25_tags_load: %lld codes for %lld docs", (long long)n,
+             (long long)ix.n_docs);
+  SB_REQUIRE(n == 0 || codes != nullptr, SB_ERR_ARG, "sb_bm25_tags_load: codes is NULL");
+  for (int64_t i = 0; i < n; ++i)
+    SB_REQUIRE(codes[i] >= -1, SB_ERR_ARG, "sb_bm25_tags_load: code %d at doc %lld (must be >= -1)", codes[i],
+               (long long)i);
+  SB_CUDA(cudaStreamSynchronize(ctx->stream));   // a search enqueued earlier may still read the old column
+  if (ix.tags[field]) cudaFree(ix.tags[field]);
+  ix.tags[field] = nullptr;
+  SB_CUDA(cudaMalloc(&ix.tags[field], (size_t)std::max<int64_t>(n, 1) * 4));
+  if (n) SB_CUDA(cudaMemcpy(ix.tags[field], codes, (size_t)n * 4, cudaMemcpyHostToDevice));
+  return SB_OK;
+}
+
 int sb_bm25_topk_dev(sb_ctx* ctx, const int32_t* q_terms_dev, const int32_t* q_off_dev, int32_t B, int32_t n_q_terms,
                      int32_t max_q_len, int32_t k, int64_t* out_ids_dev, double* out_scores_dev,
                      int32_t* out_counts_dev, void* stream) {
-  SB_REQUIRE(ctx != nullptr, SB_ERR_ARG, "sb_bm25_topk_dev: ctx is NULL");
-  SB_REQUIRE(B >= 0 && k > 0 && max_q_len >= 0 && n_q_terms >= 0, SB_ERR_ARG, "sb_bm25_topk_dev: bad sizes");
-  if (B == 0) return SB_OK;
-  SB_REQUIRE(q_off_dev && out_ids_dev && out_scores_dev && out_counts_dev, SB_ERR_ARG, "sb_bm25_topk_dev: NULL buffer");
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  DeviceGuard g(ctx->device);
-  cudaStream_t st = pick_stream(ctx, stream);
-  if (ctx->bm25.n_docs == 0 || ctx->bm25.indptr == nullptr) {
-    bm25_fill_empty_kernel<<<(B * k + 255) / 256, 256, 0, st>>>(out_ids_dev, out_scores_dev, out_counts_dev, B, k);
-    SB_CUDA(cudaGetLastError());
-    return SB_OK;
-  }
-  return bm25_topk_enqueue(ctx, q_terms_dev, q_off_dev, B, max_q_len, k, out_ids_dev, out_scores_dev, out_counts_dev,
-                           st);
+  return bm25_topk_dev_call(ctx, "sb_bm25_topk_dev", q_terms_dev, q_off_dev, B, n_q_terms, max_q_len, k, nullptr, 0,
+                            nullptr, nullptr, out_ids_dev, out_scores_dev, out_counts_dev, stream);
+}
+
+// The conditions stay on the device (a pure enqueue): a field out of range or without a column matches no doc here,
+// where the host forms reject it.
+int sb_bm25_topk_filtered_dev(sb_ctx* ctx, const int32_t* q_terms_dev, const int32_t* q_off_dev, int32_t B,
+                              int32_t n_q_terms, int32_t max_q_len, int32_t k, const int32_t* f_off_dev, int32_t n_conds,
+                              const int32_t* f_field_dev, const int32_t* f_code_dev, int64_t* out_ids_dev,
+                              double* out_scores_dev, int32_t* out_counts_dev, void* stream) {
+  return bm25_topk_dev_call(ctx, "sb_bm25_topk_filtered_dev", q_terms_dev, q_off_dev, B, n_q_terms, max_q_len, k,
+                            f_off_dev, n_conds, f_field_dev, f_code_dev, out_ids_dev, out_scores_dev, out_counts_dev,
+                            stream);
 }
 
 int sb_bm25_topk(sb_ctx* ctx, const int32_t* q_terms, const int32_t* q_off, int32_t B, int32_t k, int64_t* out_ids,
                  double* out_scores, int32_t* out_counts) {
-  SB_REQUIRE(ctx != nullptr, SB_ERR_ARG, "sb_bm25_topk: ctx is NULL");
-  SB_REQUIRE(B >= 0 && k > 0, SB_ERR_ARG, "sb_bm25_topk: bad B=%d k=%d", B, k);
-  if (B == 0) return SB_OK;
-  SB_REQUIRE(q_off && out_ids && out_scores && out_counts, SB_ERR_ARG, "sb_bm25_topk: NULL buffer");
-  const int n_terms_q = q_off[B];
-  SB_REQUIRE(n_terms_q >= 0 && (n_terms_q == 0 || q_terms), SB_ERR_ARG, "sb_bm25_topk: bad query term buffers");
-  int max_len = 0;
-  for (int b = 0; b < B; ++b) {
-    SB_REQUIRE(q_off[b + 1] >= q_off[b], SB_ERR_ARG, "sb_bm25_topk: q_off must be non-decreasing");
-    max_len = std::max(max_len, q_off[b + 1] - q_off[b]);
-  }
-  std::unique_lock<std::mutex> lk(ctx->mu);
-  DeviceGuard g(ctx->device);
-  cudaStream_t st = ctx->stream;
-  if (ctx->bm25.n_docs == 0 || ctx->bm25.indptr == nullptr) {
-    for (int i = 0; i < B * k; ++i) { out_ids[i] = -1; out_scores[i] = 0.0; }
-    for (int i = 0; i < B; ++i) out_counts[i] = 0;
-    return SB_OK;
-  }
-  int rc;
-  const size_t tb = (size_t)std::max(n_terms_q, 1) * 4, ob = (size_t)(B + 1) * 4;
-  if ((rc = ctx->pin_in.reserve(tb + ob))) return rc;
-  if ((rc = ctx->q_dev.reserve(tb + ob))) return rc;
-  uint8_t* pi = ctx->pin_in.as<uint8_t>();
-  if (n_terms_q) memcpy(pi, q_terms, (size_t)n_terms_q * 4);
-  memcpy(pi + tb, q_off, ob);
-  SB_CUDA(cudaMemcpyAsync(ctx->q_dev.p, pi, tb + ob, cudaMemcpyHostToDevice, st));
-  const int32_t* qt_dev = ctx->q_dev.as<int32_t>();
-  const int32_t* qo_dev = reinterpret_cast<const int32_t*>(ctx->q_dev.as<uint8_t>() + tb);
-  const size_t nid = (size_t)B * k;
-  if ((rc = ctx->out_ids_dev.reserve(nid * 8))) return rc;
-  if ((rc = ctx->out_sc_dev.reserve(nid * 8))) return rc;
-  if ((rc = ctx->out_cnt_dev.reserve((size_t)B * 4))) return rc;
-  if ((rc = bm25_topk_enqueue(ctx, qt_dev, qo_dev, B, max_len, k, ctx->out_ids_dev.as<int64_t>(),
-                              ctx->out_sc_dev.as<double>(), ctx->out_cnt_dev.as<int32_t>(), st)))
-    return rc;
-  if ((rc = ctx->pin_out.reserve(nid * 16 + (size_t)B * 4))) return rc;
-  uint8_t* po = ctx->pin_out.as<uint8_t>();
-  SB_CUDA(cudaMemcpyAsync(po, ctx->out_ids_dev.p, nid * 8, cudaMemcpyDeviceToHost, st));
-  SB_CUDA(cudaMemcpyAsync(po + nid * 8, ctx->out_sc_dev.p, nid * 8, cudaMemcpyDeviceToHost, st));
-  SB_CUDA(cudaMemcpyAsync(po + nid * 16, ctx->out_cnt_dev.p, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
-  SB_CUDA(cudaStreamSynchronize(st));
-  memcpy(out_ids, po, nid * 8);
-  memcpy(out_scores, po + nid * 8, nid * 8);
-  memcpy(out_counts, po + nid * 16, (size_t)B * 4);
-  return SB_OK;
+  return bm25_topk_host(ctx, "sb_bm25_topk", q_terms, q_off, B, k, nullptr, nullptr, nullptr, out_ids, out_scores,
+                        out_counts);
+}
+
+int sb_bm25_topk_filtered(sb_ctx* ctx, const int32_t* q_terms, const int32_t* q_off, int32_t B, int32_t k,
+                          const int32_t* f_off, const int32_t* f_field, const int32_t* f_code, int64_t* out_ids,
+                          double* out_scores, int32_t* out_counts) {
+  SB_REQUIRE(B <= 0 || f_off != nullptr, SB_ERR_ARG, "sb_bm25_topk_filtered: f_off is NULL");
+  SB_REQUIRE(B <= 0 || f_off[B] == 0 || (f_field && f_code), SB_ERR_ARG, "sb_bm25_topk_filtered: NULL conditions");
+  return bm25_topk_host(ctx, "sb_bm25_topk_filtered", q_terms, q_off, B, k, f_off, f_field, f_code, out_ids, out_scores,
+                        out_counts);
 }
 
 int sb_bm25_scores(sb_ctx* ctx, const int32_t* q_terms, int32_t n_q, double* out_scores) {

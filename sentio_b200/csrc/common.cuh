@@ -133,6 +133,9 @@ struct Bm25Index {
   int32_t n_dense = 0;
   int32_t* dense_of_term = nullptr;  // [V]
   double* dense_ratio = nullptr;     // [n_dense][n_docs]
+  // payload index for filtered BM25 (sb_bm25_tags_load): tags[f][doc] = dictionary code of field f, -1 = key absent;
+  // nullptr = field f not loaded.  They belong to the installed index: installing another one frees them
+  int32_t* tags[SB_MAX_TAG_FIELDS] = {};
 };
 
 struct CeModel;      // cross_encoder.cu

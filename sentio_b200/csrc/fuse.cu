@@ -531,6 +531,9 @@ int sb_select_dev(sb_ctx* ctx, const int64_t* cand_ids_dev, const void* cand_sco
 
 }  // extern "C"
 
+int bm25_check_conditions(sb_ctx* ctx, const char* who, int B, const int32_t* f_off, const int32_t* f_field,
+                          bool dense_too);   // bm25.cu
+
 namespace {
 
 // Host-buffer form of the whole path for one batch (single shard): pinned staging + ONE H2D of the queries / term ids
@@ -546,9 +549,12 @@ struct RerankArgs {
   int32_t* out_counts;    // [B]
 };
 
+// Filtered (f_off != nullptr): one CSR of conditions per query, checked against both signals' columns before anything is
+// enqueued and uploaded with the inputs; a batch without conditions takes the unfiltered calls.
 int hybrid_host_call(sb_ctx* ctx, const char* who, const float* q, const int32_t* q_terms, const int32_t* q_off, int32_t B,
                      int32_t k, int32_t method, double rrf_k, double w_dense, double w_sparse, int64_t* out_ids,
-                     double* out_scores, int32_t* out_src, int32_t* out_counts, const RerankArgs* rr) {
+                     double* out_scores, int32_t* out_src, int32_t* out_counts, const RerankArgs* rr,
+                     const int32_t* f_off = nullptr, const int32_t* f_field = nullptr, const int32_t* f_code = nullptr) {
   SB_REQUIRE(ctx != nullptr, SB_ERR_ARG, "%s: ctx is NULL", who);
   SB_REQUIRE(B >= 0 && k > 0, SB_ERR_ARG, "%s: bad B=%d k=%d", who, B, k);
   if (B == 0) return SB_OK;
@@ -565,7 +571,9 @@ int hybrid_host_call(sb_ctx* ctx, const char* who, const float* q, const int32_t
   SB_REQUIRE(ctx->dense[0].rows != nullptr && d > 0, SB_ERR_STATE, "%s: no dense index loaded in slot 0", who);
   const size_t qb = (size_t)B * d * 4, tb = (size_t)std::max(n_terms_q, 1) * 4, ob = (size_t)(B + 1) * 4;
   const size_t rb = rr ? (size_t)B * rr->lq * 4 + (size_t)B * 4 : 0;   // query word pieces + lengths
-  const size_t in_bytes = qb + tb + ob + rb;
+  const int n_conds = f_off ? f_off[B] : 0;
+  const size_t cb = n_conds ? ob + (size_t)n_conds * 8 : 0;            // conditions: f_off | f_field | f_code
+  const size_t in_bytes = qb + tb + ob + rb + cb;
   const size_t nid = (size_t)B * k;
   // device layout: inputs | dense ids sc cnt | sparse ids sc cnt | fused ids sc src cnt | reranked ids sc cnt
   const size_t cnt_b = ((size_t)B * 4 + 7) / 8 * 8;
@@ -579,6 +587,7 @@ int hybrid_host_call(sb_ctx* ctx, const char* who, const float* q, const int32_t
     std::lock_guard<std::mutex> lk(ctx->mu);
     DeviceGuard g(ctx->device);
     int rc;
+    if (f_off && (rc = bm25_check_conditions(ctx, who, B, f_off, f_field, true))) return rc;
     if ((rc = ctx->hyb_pin.reserve(std::max(in_bytes, std::max(fused_bytes, rr_bytes)) + 64))) return rc;
     if ((rc = ctx->hyb_dev.reserve((in_bytes + 7) / 8 * 8 + work_bytes + fused_bytes + rr_bytes + 64))) return rc;
     pi = ctx->hyb_pin.as<uint8_t>();
@@ -590,6 +599,12 @@ int hybrid_host_call(sb_ctx* ctx, const char* who, const float* q, const int32_t
       memcpy(pi + qb + tb + ob, rr->q_tok, (size_t)B * rr->lq * 4);
       memcpy(pi + qb + tb + ob + (size_t)B * rr->lq * 4, rr->q_len, (size_t)B * 4);
     }
+    if (n_conds) {
+      uint8_t* pc = pi + qb + tb + ob + rb;
+      memcpy(pc, f_off, ob);
+      memcpy(pc + ob, f_field, (size_t)n_conds * 4);
+      memcpy(pc + ob + (size_t)n_conds * 4, f_code, (size_t)n_conds * 4);
+    }
     SB_CUDA(cudaMemcpyAsync(dv, pi, in_bytes, cudaMemcpyHostToDevice, st));
   }
   const float* q_dev = reinterpret_cast<const float*>(dv);
@@ -597,6 +612,9 @@ int hybrid_host_call(sb_ctx* ctx, const char* who, const float* q, const int32_t
   const int32_t* o_dev = reinterpret_cast<const int32_t*>(dv + qb + tb);
   const int32_t* qt_dev = reinterpret_cast<const int32_t*>(dv + qb + tb + ob);
   const int32_t* ql_dev = rr ? qt_dev + (size_t)B * rr->lq : nullptr;
+  const int32_t* fo_dev = reinterpret_cast<const int32_t*>(dv + qb + tb + ob + rb);   // valid when n_conds > 0
+  const int32_t* ff_dev = fo_dev + (B + 1);
+  const int32_t* fc_dev = ff_dev + n_conds;
   uint8_t* w = dv + (in_bytes + 7) / 8 * 8;
   int64_t* d_ids = reinterpret_cast<int64_t*>(w);
   double* d_sc = reinterpret_cast<double*>(w + nid * 8);
@@ -615,8 +633,16 @@ int hybrid_host_call(sb_ctx* ctx, const char* who, const float* q, const int32_t
   float* r_sc = reinterpret_cast<float*>(w4 + nrr * 8);
   int32_t* r_cnt = reinterpret_cast<int32_t*>(w4 + nrr * 12);
   int rc;
-  if ((rc = sb_dense_topk_dev(ctx, 0, q_dev, B, k, d_ids, d_sc, d_cnt, st))) return rc;
-  if ((rc = sb_bm25_topk_dev(ctx, t_dev, o_dev, B, n_terms_q, max_len, k, s_ids, s_sc, s_cnt, st))) return rc;
+  if (n_conds) {
+    if ((rc = sb_dense_topk_filtered_dev(ctx, 0, q_dev, B, k, fo_dev, n_conds, ff_dev, fc_dev, d_ids, d_sc, d_cnt, st)))
+      return rc;
+    if ((rc = sb_bm25_topk_filtered_dev(ctx, t_dev, o_dev, B, n_terms_q, max_len, k, fo_dev, n_conds, ff_dev, fc_dev, s_ids,
+                                        s_sc, s_cnt, st)))
+      return rc;
+  } else {
+    if ((rc = sb_dense_topk_dev(ctx, 0, q_dev, B, k, d_ids, d_sc, d_cnt, st))) return rc;
+    if ((rc = sb_bm25_topk_dev(ctx, t_dev, o_dev, B, n_terms_q, max_len, k, s_ids, s_sc, s_cnt, st))) return rc;
+  }
   if ((rc = sb_fuse_dev(ctx, method, rrf_k, w_dense, w_sparse, B, d_ids, d_sc, d_cnt, k, s_ids, s_sc, s_cnt, k, nullptr,
                         nullptr, nullptr, 0, nullptr, 0, 0, k, f_ids, f_sc, f_src, f_cnt, st)))
     return rc;
@@ -654,6 +680,18 @@ int sb_hybrid_topk(sb_ctx* ctx, const float* q, const int32_t* q_terms, const in
   SB_REQUIRE(B == 0 || (out_ids && out_scores && out_src && out_counts), SB_ERR_ARG, "sb_hybrid_topk: NULL output buffer");
   return hybrid_host_call(ctx, "sb_hybrid_topk", q, q_terms, q_off, B, k, method, rrf_k, w_dense, w_sparse, out_ids,
                           out_scores, out_src, out_counts, nullptr);
+}
+
+int sb_hybrid_topk_filtered(sb_ctx* ctx, const float* q, const int32_t* q_terms, const int32_t* q_off, int32_t B,
+                            int32_t k, const int32_t* f_off, const int32_t* f_field, const int32_t* f_code,
+                            int32_t method, double rrf_k, double w_dense, double w_sparse, int64_t* out_ids,
+                            double* out_scores, int32_t* out_src, int32_t* out_counts) {
+  SB_REQUIRE(B <= 0 || (out_ids && out_scores && out_src && out_counts), SB_ERR_ARG,
+             "sb_hybrid_topk_filtered: NULL output buffer");
+  SB_REQUIRE(B <= 0 || f_off != nullptr, SB_ERR_ARG, "sb_hybrid_topk_filtered: f_off is NULL");
+  SB_REQUIRE(B <= 0 || f_off[B] == 0 || (f_field && f_code), SB_ERR_ARG, "sb_hybrid_topk_filtered: NULL conditions");
+  return hybrid_host_call(ctx, "sb_hybrid_topk_filtered", q, q_terms, q_off, B, k, method, rrf_k, w_dense, w_sparse,
+                          out_ids, out_scores, out_src, out_counts, nullptr, f_off, f_field, f_code);
 }
 
 int sb_hybrid_rerank_topk(sb_ctx* ctx, const float* q, const int32_t* q_terms, const int32_t* q_off, const int32_t* q_tok,

@@ -375,17 +375,43 @@ class B200Engine:
         flat = np.concatenate([np.asarray(t, dtype=np.int32) for t in term_id_lists])
         return flat, off
 
-    def bm25_topk(self, term_id_lists: Sequence[Sequence[int]], k: int):
+    def load_bm25_tags(self, field: int, codes: np.ndarray) -> None:
+        """Payload index column ``field`` (< 16) of the installed BM25 index: one int32 code per doc, -1 = key absent.
+        Installing another BM25 index drops the columns."""
+        c = np.ascontiguousarray(codes, dtype=np.int32).reshape(-1)
+        check(self._lib.sb_bm25_tags_load(self._h, int(field), _ptr(c), len(c)), "sb_bm25_tags_load")
+
+    def bm25_count(self) -> int:
+        """Docs of the installed BM25 index (0 when none is installed)."""
+        return max(0, int(self._lib.sb_bm25_count(self._h)))
+
+    @staticmethod
+    def _host_filters(filters, B: int):
+        off, fld, code = (np.ascontiguousarray(a, dtype=np.int32).reshape(-1) for a in filters)
+        if len(off) != B + 1 or len(fld) != len(code) or int(off[-1]) != len(fld):
+            raise ValueError("filters must be CSR (f_off [B+1], f_field [n], f_code [n]) with f_off[B] == n")
+        return off, fld, code
+
+    def bm25_topk(self, term_id_lists: Sequence[Sequence[int]], k: int, filters=None):
+        """``filters`` = CSR conditions as ``dense_topk``: the top-k of the docs matching each query's conditions
+        (``sb_bm25_topk_filtered``); None = unfiltered."""
         B = len(term_id_lists)
         flat, off = self.pack_queries(term_id_lists)
         ids = np.empty((B, k), dtype=np.int64)
         sc = np.empty((B, k), dtype=np.float64)
         cnt = np.empty(B, dtype=np.int32)
+        if filters is not None:
+            f_off, fld, code = self._host_filters(filters, B)
+            check(self._lib.sb_bm25_topk_filtered(self._h, _ptr(flat), _ptr(off), B, k, _ptr(f_off), _ptr(fld), _ptr(code),
+                                                  _ptr(ids), _ptr(sc), _ptr(cnt)), "sb_bm25_topk_filtered")
+            return ids, sc, cnt
         check(self._lib.sb_bm25_topk(self._h, _ptr(flat), _ptr(off), B, k, _ptr(ids), _ptr(sc), _ptr(cnt)),
               "sb_bm25_topk")
         return ids, sc, cnt
 
-    def bm25_topk_dev(self, terms_t, off_t, B: int, n_terms: int, max_len: int, k: int, out=None):
+    def bm25_topk_dev(self, terms_t, off_t, B: int, n_terms: int, max_len: int, k: int, out=None, filters=None):
+        """``filters`` = (f_off [B+1], f_field, f_code) int32 CUDA tensors, or None (unfiltered).  A pure enqueue: the
+        conditions are not read on the host, so a field out of range or without a BM25 column matches no doc."""
         import torch
 
         if out is None:
@@ -393,8 +419,18 @@ class B200Engine:
             out = (torch.empty((B, k), dtype=torch.int64, device=dev), torch.empty((B, k), dtype=torch.float64, device=dev),
                    torch.empty((B,), dtype=torch.int32, device=dev))
         ids, sc, cnt = out
-        check(self._lib.sb_bm25_topk_dev(self._h, _tptr(terms_t), _tptr(off_t), B, n_terms, max_len, k, _tptr(ids),
-                                         _tptr(sc), _tptr(cnt), self._stream()), "sb_bm25_topk_dev")
+        if filters is None:
+            check(self._lib.sb_bm25_topk_dev(self._h, _tptr(terms_t), _tptr(off_t), B, n_terms, max_len, k, _tptr(ids),
+                                             _tptr(sc), _tptr(cnt), self._stream()), "sb_bm25_topk_dev")
+            return ids, sc, cnt
+        f_off, fld, code = filters
+        for t in (f_off, fld, code):
+            assert t.is_cuda and t.dtype == torch.int32 and t.is_contiguous()
+        if f_off.numel() != B + 1 or fld.numel() != code.numel():
+            raise ValueError("filters must be CSR (f_off [B+1], f_field [n], f_code [n])")
+        check(self._lib.sb_bm25_topk_filtered_dev(self._h, _tptr(terms_t), _tptr(off_t), B, n_terms, max_len, k,
+                                                  _tptr(f_off), int(fld.numel()), _tptr(fld), _tptr(code), _tptr(ids),
+                                                  _tptr(sc), _tptr(cnt), self._stream()), "sb_bm25_topk_filtered_dev")
         return ids, sc, cnt
 
     def bm25_scores(self, term_ids: Sequence[int]) -> np.ndarray:
@@ -461,8 +497,10 @@ class B200Engine:
         return ids, sc, src, cnt
 
     def hybrid_topk(self, q: np.ndarray, flat_terms: np.ndarray, off: np.ndarray, k: int, method: str = "rrf",
-                    rrf_k: float = 60, w_dense: float = 0.5, w_sparse: float = 0.5):
-        """Whole retrieve -> fuse path from host buffers (sb_hybrid_topk): (ids, scores, src, counts) NumPy arrays."""
+                    rrf_k: float = 60, w_dense: float = 0.5, w_sparse: float = 0.5, filters=None):
+        """Whole retrieve -> fuse path from host buffers (sb_hybrid_topk): (ids, scores, src, counts) NumPy arrays.
+        ``filters`` = CSR conditions as ``dense_topk``, applied to both signals (``sb_hybrid_topk_filtered``; field f
+        must be loaded in dense slot 0 and in BM25); None = unfiltered."""
         q = np.ascontiguousarray(q, dtype=np.float32)
         flat = np.ascontiguousarray(flat_terms, dtype=np.int32)
         off = np.ascontiguousarray(off, dtype=np.int32)
@@ -471,6 +509,13 @@ class B200Engine:
         sc = np.empty((B, k), dtype=np.float64)
         src = np.empty((B, k), dtype=np.int32)
         cnt = np.empty(B, dtype=np.int32)
+        if filters is not None:
+            f_off, fld, code = self._host_filters(filters, B)
+            check(self._lib.sb_hybrid_topk_filtered(self._h, _ptr(q), _ptr(flat), _ptr(off), B, int(k), _ptr(f_off),
+                                                    _ptr(fld), _ptr(code), FUSION_METHODS[method], float(rrf_k),
+                                                    float(w_dense), float(w_sparse), _ptr(ids), _ptr(sc), _ptr(src),
+                                                    _ptr(cnt)), "sb_hybrid_topk_filtered")
+            return ids, sc, src, cnt
         check(self._lib.sb_hybrid_topk(self._h, _ptr(q), _ptr(flat), _ptr(off), B, int(k), FUSION_METHODS[method],
                                        float(rrf_k), float(w_dense), float(w_sparse), _ptr(ids), _ptr(sc), _ptr(src),
                                        _ptr(cnt)), "sb_hybrid_topk")

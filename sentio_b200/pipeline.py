@@ -102,6 +102,22 @@ class HybridPipeline:
         data.extras["shard_local"] = True   # postings / doc_len cover THIS rank's doc range only
         return data
 
+    def load_tags(self, field: int, codes: np.ndarray) -> None:
+        """Payload index column ``field`` (< 16) for filtered search.  ``codes`` is the corpus-global column: one int32
+        code per global doc id from one dictionary for the whole corpus (-1 = key absent); this rank loads its own slice
+        into dense slot 0 and into BM25 (whichever are loaded).  Call it after loading the indexes: installing a BM25
+        index drops its columns."""
+        c = np.ascontiguousarray(codes, dtype=np.int32).reshape(-1)
+        n_dense = self.engine.dense_count.get(0)
+        has_bm25 = self.engine.bm25 is not None
+        if n_dense is None and not has_bm25:
+            raise ValueError("load_tags: load the dense or BM25 index first")
+        if n_dense is not None:
+            self.engine.load_dense_tags(field, c[self.id_base:self.id_base + n_dense], slot=0)
+        if has_bm25:
+            base = self.engine.bm25_id_base
+            self.engine.load_bm25_tags(field, c[base:base + self.engine.bm25_count()])
+
     def load_cross_encoder(self, weights) -> None:
         """weights: sentio_b200.cross_encoder.CrossEncoderWeights"""
         self.engine.ce_load(weights.blob(), weights.config)
@@ -151,6 +167,15 @@ class HybridPipeline:
             outs.append(pin)
         self.torch.cuda.current_stream().synchronize()
         return tuple(p.numpy().copy() for p in outs)
+
+    def _filters_to_dev(self, filters):
+        """host CSR conditions (f_off, f_field, f_code) -> int32 device tensors; None stays None"""
+        if filters is None:
+            return None
+        off, fld, code = (np.ascontiguousarray(a, dtype=np.int32).reshape(-1) for a in filters)
+        if len(fld) != len(code) or int(off[-1]) != len(fld):
+            raise ValueError("filters must be CSR (f_off [B+1], f_field [n], f_code [n]) with f_off[B] == n")
+        return self._to_dev(off, "f_off"), self._to_dev(fld, "f_field"), self._to_dev(code, "f_code")
 
     def _record_layout(self, B: int, k: int, signals: int):
         """Byte layout of one rank's all-gather record: per signal ids[B,k] i64 | scores[B,k] f64 | counts[B] i32."""
@@ -208,18 +233,20 @@ class HybridPipeline:
         return out
 
     # ------------------------------------------------------------------ device-resident path
-    def dense_dev(self, q_t, k: int):
-        """q_t [B,d] fp32 cuda -> global (ids, scores, counts) on this rank."""
+    def dense_dev(self, q_t, k: int, filters=None):
+        """q_t [B,d] fp32 cuda -> global (ids, scores, counts) on this rank.  ``filters``: CSR conditions as int32 device
+        tensors (f_off [B+1], f_field, f_code), applied on every shard before the merge; None = unfiltered."""
         t = self.torch
         B = q_t.shape[0]
+        fkw = {} if filters is None else {"filters": filters}
         if self.world == 1:
             out = (self._buf("d_ids", (B, k), t.int64), self._buf("d_sc", (B, k), t.float64),
                    self._buf("d_cnt", (B,), t.int32))
-            return self.engine.dense_topk_dev(q_t, k, out=out)
+            return self.engine.dense_topk_dev(q_t, k, out=out, **fkw)
         _, nbytes = self._record_layout(B, k, 1)
         rec = self._buf("rec1", (nbytes,), t.uint8)
         with self._stage("local_dense_topk_us"):
-            self.engine.dense_topk_dev(q_t, k, out=self._views(rec, B, k, 0))
+            self.engine.dense_topk_dev(q_t, k, out=self._views(rec, B, k, 0), **fkw)
         g = self._gather(rec)
         ids0, sc0, cnt0 = self._views(g[0], B, k, 0)
         out = (self._buf("d_ids", (B, k), t.int64), self._buf("d_sc", (B, k), t.float64),
@@ -228,16 +255,19 @@ class HybridPipeline:
             return self.engine.merge_shards_dev(ids0, sc0, cnt0, nbytes, self.world, out=out)
 
     def hybrid_dev(self, q_t, terms_t, off_t, n_terms: int, max_len: int, k: int, method: str = "rrf",
-                   rrf_k: float = 60, w_dense: float = 0.5, w_sparse: float = 0.5):
-        """Dense + BM25 + fusion for a batch; returns fused (ids, scores, src, counts) device tensors."""
+                   rrf_k: float = 60, w_dense: float = 0.5, w_sparse: float = 0.5, filters=None):
+        """Dense + BM25 + fusion for a batch; returns fused (ids, scores, src, counts) device tensors.  ``filters``: CSR
+        conditions as int32 device tensors, applied to both signals on every shard (fusion then sees only matching
+        docs); None = unfiltered."""
         t = self.torch
         B = q_t.shape[0]
+        fkw = {} if filters is None else {"filters": filters}
         per, nbytes = self._record_layout(B, k, 2)
         rec = self._buf("rec2", (nbytes,), t.uint8)
         dv = self._views(rec, B, k, 0)
         sv = self._views(rec, B, k, 1)
-        self.engine.dense_topk_dev(q_t, k, out=dv)
-        self.engine.bm25_topk_dev(terms_t, off_t, B, n_terms, max_len, k, out=sv)
+        self.engine.dense_topk_dev(q_t, k, out=dv, **fkw)
+        self.engine.bm25_topk_dev(terms_t, off_t, B, n_terms, max_len, k, out=sv, **fkw)
         if self.world > 1:
             g = self._gather(rec)
             d0 = self._views(g[0], B, k, 0)
@@ -256,14 +286,17 @@ class HybridPipeline:
 
     def hybrid_rerank_dev(self, q_t, terms_t, off_t, n_terms: int, max_len: int, q_tok_t, q_len_t, k: int, k_out: int,
                           seq_len: int = 128, method: str = "rrf", rrf_k: float = 60, w_dense: float = 0.5,
-                          w_sparse: float = 0.5):
-        """retrieve (dense + BM25 + fusion, top k) -> cross-encoder rerank (top k_out), all on the device.
+                          w_sparse: float = 0.5, filters=None):
+        """retrieve (dense + BM25 + fusion, top k) -> cross-encoder rerank (top k_out), all on the device.  ``filters`` as
+        ``hybrid_dev``: every candidate the reranker sees matches its query's conditions.
 
         Sharded runs: after the all-gather + merge every rank holds the fused candidates of ALL queries; the rerank (the
         expensive stage) is then split by query -- rank r scores queries ``rerank_slice(B)`` and returns only those rows
         (no second collective; the caller owns the per-rank result slices)."""
         t = self.torch
-        ids, sc, src, cnt = self.hybrid_dev(q_t, terms_t, off_t, n_terms, max_len, k, method, rrf_k, w_dense, w_sparse)
+        fkw = {} if filters is None else {"filters": filters}
+        ids, sc, src, cnt = self.hybrid_dev(q_t, terms_t, off_t, n_terms, max_len, k, method, rrf_k, w_dense, w_sparse,
+                                            **fkw)
         lo, hi = self.rerank_slice(q_t.shape[0])
         B = hi - lo
         out = (self._buf("r_ids", (B, k_out), t.int64), self._buf("r_sc", (B, k_out), t.float32),
@@ -280,9 +313,15 @@ class HybridPipeline:
         return min(B, self.rank * per), min(B, (self.rank + 1) * per)
 
     # ------------------------------------------------------------------ host (e2e) path
-    def search_dense(self, q: np.ndarray, k: int, out=None):
+    def search_dense(self, q: np.ndarray, k: int, out=None, filters=None):
         """Host in / host out.  world == 1: straight through the C-ABI host entry point (``out``: arrays to fill in
-        place -- page-locked ones from ``engine.pinned_empty`` skip the staging copies)."""
+        place -- page-locked ones from ``engine.pinned_empty`` skip the staging copies).  ``filters``: host CSR
+        conditions (f_off [B+1], f_field, f_code) int32 arrays, or None (unfiltered)."""
+        if filters is not None:
+            if self.world == 1:
+                return self.engine.dense_topk(q, k, filters=filters)
+            q_t = self._to_dev(np.ascontiguousarray(q, dtype=np.float32), "q")
+            return self._to_host(self.dense_dev(q_t, k, filters=self._filters_to_dev(filters)), "dense")
         if self.world == 1:
             return self.engine.dense_topk(q, k, out=out) if out is not None else self.engine.dense_topk(q, k)
         t = self.torch
@@ -290,7 +329,9 @@ class HybridPipeline:
         return self._to_host(self.dense_dev(q_t, k), "dense")
 
     def search_hybrid(self, q: np.ndarray, term_lists: Sequence[Sequence[int]], k: int, method: str = "rrf",
-                      rrf_k: float = 60, w_dense: float = 0.5, w_sparse: float = 0.5):
+                      rrf_k: float = 60, w_dense: float = 0.5, w_sparse: float = 0.5, filters=None):
+        """Host in / host out.  ``filters``: host CSR conditions (f_off [B+1], f_field, f_code) int32 arrays applied to
+        both signals (field f must be loaded for dense and BM25, see ``load_tags``), or None (unfiltered)."""
         import os
         import time
 
@@ -299,14 +340,17 @@ class HybridPipeline:
         flat, off = B200Engine.pack_queries(term_lists)
         if self.world == 1 and self.device is not None:
             # single shard: straight through the C ABI's host entry point (its own pinned staging, no framework on the path)
+            if filters is not None:
+                return self.engine.hybrid_topk(q, flat, off, k, method, rrf_k, w_dense, w_sparse, filters=filters)
             return self.engine.hybrid_topk(q, flat, off, k, method, rrf_k, w_dense, w_sparse)
         max_len = int(np.diff(off).max()) if len(off) > 1 else 0
         t1 = time.perf_counter()
         q_t = self._to_dev(np.ascontiguousarray(q, dtype=np.float32), "q")
         terms_t = self._to_dev(flat, "terms")
         off_t = self._to_dev(off, "off")
+        fkw = {} if filters is None else {"filters": self._filters_to_dev(filters)}
         t2 = time.perf_counter()
-        dev = self.hybrid_dev(q_t, terms_t, off_t, int(off[-1]), max_len, k, method, rrf_k, w_dense, w_sparse)
+        dev = self.hybrid_dev(q_t, terms_t, off_t, int(off[-1]), max_len, k, method, rrf_k, w_dense, w_sparse, **fkw)
         t3 = time.perf_counter()
         out = self._to_host(dev, "hybrid")
         if trace:
@@ -317,9 +361,10 @@ class HybridPipeline:
 
     def search_hybrid_rerank(self, q: np.ndarray, term_lists, q_tok: np.ndarray, q_len: np.ndarray, k: int, k_out: int,
                              seq_len: int = 128, method: str = "rrf", rrf_k: float = 60, w_dense: float = 0.5,
-                             w_sparse: float = 0.5):
+                             w_sparse: float = 0.5, filters=None):
+        """``filters`` as ``search_hybrid``; a filtered call reranks through ``hybrid_rerank_dev``."""
         flat, off = B200Engine.pack_queries(term_lists)
-        if self.world == 1 and self.device is not None:  # single shard: the C ABI's own host entry point
+        if self.world == 1 and self.device is not None and filters is None:  # one shard: the C ABI host entry point
             return self.engine.hybrid_rerank_topk(q, flat, off, q_tok, q_len, k, k_out, seq_len, method, rrf_k, w_dense,
                                                   w_sparse)
         max_len = int(np.diff(off).max()) if len(off) > 1 else 0
@@ -327,5 +372,6 @@ class HybridPipeline:
         terms_t, off_t = self._to_dev(flat, "terms"), self._to_dev(off, "off")
         qt_t = self._to_dev(np.ascontiguousarray(q_tok, dtype=np.int32), "qtok")
         ql_t = self._to_dev(np.ascontiguousarray(q_len, dtype=np.int32), "qlen")
+        fkw = {} if filters is None else {"filters": self._filters_to_dev(filters)}
         return self._to_host(self.hybrid_rerank_dev(q_t, terms_t, off_t, int(off[-1]), max_len, qt_t, ql_t, k, k_out,
-                                                    seq_len, method, rrf_k, w_dense, w_sparse), "rerank")
+                                                    seq_len, method, rrf_k, w_dense, w_sparse, **fkw), "rerank")
