@@ -7,10 +7,12 @@
 //   * dense_scan_mma_kernel<QBN>   N = QBN = 16 / 32 / 64 / 128 / 256 queries (m64nQBNk16).
 // A ring stage holds one corpus box (16 KB) and the matching box of the query block (QBN x 128 B), so shared memory does
 // not grow with d: at QBN = 256 four 48 KB stages fit the 227 KB a block may use.
-// At QBN = 256 a 16 KB corpus box feeds 8 MMAs of 64 x 256 x 16: the pass is bound by the tensor pipe, not by HBM.
+// At QBN = 256 a 16 KB corpus box feeds 8 MMAs of 64 x 256 x 16.
 //
-// Every CTA loads the query boxes itself (512 KB per tile from L2 at d = 1024): sharing them across a 2-CTA cluster by
-// TMA multicast was measured slower on the H100 (DESIGN.md K1b).
+// Every CTA loads the query boxes itself (512 KB per tile from L2 at d = 1024).  Those L2 reads do not bound the pass,
+// and sharing them across a 2-CTA cluster by TMA multicast measured no faster on the H100.  The serial epilogue does
+// bound it: skipping it takes a 256-query pass from 1.07 to 0.79 ms (DESIGN.md K1b).  So the epilogue keeps global loads
+// off its critical path: a tile's row scales are loaded before its MMAs, and the thresholds once per column pair.
 //
 // Exactness (dense_common.cuh, DESIGN.md "K1: exactness"):
 //   * queries are L2-normalised before the fp16 rounding (cosine is scale invariant; the caller's scale never reaches
@@ -63,6 +65,21 @@ __device__ __forceinline__ void tma_prefetch_l2_2d(const CUtensorMap* map, int c
   asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global [%0, {%1, %2}];" ::"l"(map), "r"(c0), "r"(c1) : "memory");
 }
 
+// *ptr if `live`, else 0, through the read-only path.  volatile: the load is issued where it is written (ahead of a
+// tile's MMAs) instead of being moved to its first use.
+__device__ __forceinline__ float ldg_early(const float* ptr, bool live) {
+  float v = 0.f;
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.u32 p, %2, 0;\n"
+      "@p ld.global.nc.f32 %0, [%1];\n"
+      "}\n"
+      : "+f"(v)
+      : "l"(ptr), "r"((uint32_t)live));
+  return v;
+}
+
 struct MmaScanParams {
   const float* inv_norm;
   const float* thr_init;        // [QBN] safe initial thresholds (NULL = -inf: sampling pass)
@@ -95,8 +112,9 @@ dense_scan_mma_kernel(const __grid_constant__ CUtensorMap tm_rows, const __grid_
   constexpr uint32_t kStageBytes = kATileBytes + kQBoxBytes;  // corpus box, then query box
   uint64_t* bars = reinterpret_cast<uint64_t*>(sm + (size_t)p.stages * kStageBytes);
   const uint32_t bar_full = smem_u32(bars), bar_empty = smem_u32(bars + p.stages);
-  volatile float* thr = reinterpret_cast<volatile float*>(bars + 2 * p.stages);   // [QBN]
-  int* cnt = reinterpret_cast<int*>(const_cast<float*>(thr) + QBN);              // [QBN]
+  float* thr = reinterpret_cast<float*>(bars + 2 * p.stages);   // [QBN], 8-byte aligned
+  const uint32_t thr_s = smem_u32(thr);                         // read-only once the block has synchronised
+  int* cnt = reinterpret_cast<int*>(thr + QBN);                 // [QBN]
   float* rq_s = reinterpret_cast<float*>(cnt + QBN);                             // [QBN] EUCLID only
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -152,6 +170,16 @@ dense_scan_mma_kernel(const __grid_constant__ CUtensorMap tm_rows, const __grid_
     const size_t q_stride = (size_t)grid * p.capg;
     int it = 0;
     for (int t = 0; t < my_tiles; ++t) {
+      // this thread's accumulator rows: row0 and row0 + 8; columns 8 j + 2 (lane % 4) + {0, 1}.  Their per-row scales are
+      // loaded before the MMAs, so the epilogue does not start with a global-memory round trip.
+      const int64_t row0 = (int64_t)tile_row(t) + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+      const bool live0 = row0 < p.n, live1 = row0 + 8 < p.n;
+      const float invn0 = ldg_early(p.inv_norm + row0, live0), invn1 = ldg_early(p.inv_norm + row0 + 8, live1);
+      float h0 = 0.f, h1 = 0.f;
+      if constexpr (EUCLID) {
+        h0 = ldg_early(p.hh + row0, live0);
+        h1 = ldg_early(p.hh + row0 + 8, live1);
+      }
       float acc[QBN / 2];
       for (int kb = 0; kb < p.kb_count; ++kb, ++it) {
         const int s = it % p.stages;
@@ -172,16 +200,6 @@ dense_scan_mma_kernel(const __grid_constant__ CUtensorMap tm_rows, const __grid_
       wgmma_wait<0>();
       __syncwarp();
       if (lane == 0) mbar_arrive(bar_empty + 8 * ((it - 1) % p.stages));
-      // this thread's accumulator rows: row0 and row0 + 8; columns 8 j + 2 (lane % 4) + {0, 1}
-      const int64_t row0 = (int64_t)tile_row(t) + wg * 64 + (warp & 3) * 16 + (lane >> 2);
-      const bool live0 = row0 < p.n, live1 = row0 + 8 < p.n;
-      const float invn0 = live0 ? __ldg(p.inv_norm + row0) : 0.f;
-      const float invn1 = live1 ? __ldg(p.inv_norm + row0 + 8) : 0.f;
-      float h0 = 0.f, h1 = 0.f;
-      if constexpr (EUCLID) {
-        h0 = live0 ? __ldg(p.hh + row0) : 0.f;
-        h1 = live1 ? __ldg(p.hh + row0 + 8) : 0.f;
-      }
       auto key = [&](float a, float invn, float h, int col) {
         float s = a * invn;
         if constexpr (EUCLID) s = __fsub_rn(__fmul_rn(rq_s[col], s), h);
@@ -225,6 +243,11 @@ dense_scan_mma_kernel(const __grid_constant__ CUtensorMap tm_rows, const __grid_
         for (int j = 0; j < QBN / 4; j += 2) {   // acc[2 j .. 2 j + 3]: columns 4 j .. 4 j + 7
           uint2 mw = make_uint2(0u, 0u);
           if constexpr (FILTER) mw = __ldg(reinterpret_cast<const uint2*>(mrow + 4 * j));
+          // the thresholds of this thread's two columns: one 8-byte shared load serves all four scores of the step
+          float2 tc;
+          asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];"   // volatile: issued here, not hoisted into live registers
+                       : "=f"(tc.x), "=f"(tc.y)
+                       : "r"(thr_s + 4u * (4 * j + 2 * (lane & 3))));
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             if (!(h ? live1 : live0)) continue;
@@ -237,7 +260,7 @@ dense_scan_mma_kernel(const __grid_constant__ CUtensorMap tm_rows, const __grid_
               const float score = key(acc[2 * j + 2 * h + e], invn, hrow, col);
               bool match = true;
               if constexpr (FILTER) match = ((e ? mw.y : mw.x) >> (h ? sh1 : sh0)) & 1u;
-              if (score >= thr[col] && match) {
+              if (score >= (e ? tc.y : tc.x) && match) {
                 const int pos = atomicAdd(&cnt[col], 1);
                 if (pos < p.capg) my_cand[(size_t)col * q_stride + pos] = make_key32(score, (uint32_t)row);
               }
