@@ -195,6 +195,53 @@ int sb_dense_topk_filtered_dev(sb_ctx* ctx, int slot, const float* q_dev, int32_
                                int32_t* out_counts_dev, void* stream);
 int64_t sb_dense_fallback_count(sb_ctx* ctx);
 /*
+ * Boolean payload filters -- Qdrant's `query_points(query_filter=)` with must / should / must_not / min_should, nested
+ * filters, MatchValue, MatchAny and Range (DESIGN.md K1h).  The host compiles each query's filter into a postfix program
+ * of predicates over the slot's tag columns (dictionary codes, sb_dense_tags_load) and value columns (below).
+ *
+ * sb_dense_values_load: numeric payload column `field` (< SB_MAX_VALUE_FIELDS) of dense slot `slot`: vals[n] holds one
+ * fp64 per row, NaN = the row has no numeric value at the key.  n must equal sb_dense_count.  sb_dense_load drops every
+ * value column; reserve grows them, upsert sets them to NaN on the written rows, delete moves them with the rows.
+ * sb_dense_values_write: vals[i] -> value column `field` (loaded) at rows[i] (distinct, < count).
+ *
+ * sb_pred: one program step.  Leaves push one bit per row, combinators pop `a` bits and push one:
+ *   SB_PRED_EQ       tags[field][row] == a (a >= 0)
+ *   SB_PRED_IN       tags[field][row] is one of pool[a, a + b) (ascending, distinct codes >= 0; b = 0 matches nothing)
+ *   SB_PRED_RANGE    vals[field][row] >= lo (lo_incl) or > lo, and <= hi (hi_incl) or < hi, compared in fp64; NaN
+ *                    matches nothing; -inf / +inf inclusive bounds leave a side open
+ *   SB_PRED_PRESENT  tags[field][row] >= 0
+ *   SB_PRED_AND / SB_PRED_OR / SB_PRED_NOR   all / at least one / none of the top `a` bits (AND of 0 bits is true)
+ *   SB_PRED_ATLEAST  at least b of the top `a` bits
+ * sb_dense_topk_where: as sb_dense_topk_filtered, over the rows on which query b's program prog[p_off[b], p_off[b+1])
+ * leaves a 1.  An empty program is unfiltered; a batch of empty programs is exactly sb_dense_topk.  A program must leave
+ * exactly one bit, hold at most SB_MAX_PRED_STACK bits at any step and have at most SB_MAX_PRED steps; every field named
+ * must be loaded (SB_ERR_STATE); everything is validated before the first launch (SB_ERR_ARG).  Results: the EXACT top-k
+ * of the matching rows, same order, scores, out_counts and all-zero-query behaviour as sb_dense_topk_filtered.
+ */
+#define SB_MAX_VALUE_FIELDS 16
+#define SB_MAX_PRED 1024
+#define SB_MAX_PRED_STACK 64
+#define SB_PRED_EQ 1
+#define SB_PRED_IN 2
+#define SB_PRED_RANGE 3
+#define SB_PRED_PRESENT 4
+#define SB_PRED_AND 5
+#define SB_PRED_OR 6
+#define SB_PRED_NOR 7
+#define SB_PRED_ATLEAST 8
+typedef struct sb_pred {
+  int32_t op;       /* SB_PRED_* */
+  int32_t field;    /* tag field (EQ, IN, PRESENT) or value field (RANGE); ignored by combinators */
+  int32_t a, b;     /* see above */
+  double lo, hi;    /* RANGE bounds */
+  int32_t lo_incl, hi_incl;
+} sb_pred;
+int sb_dense_values_load(sb_ctx* ctx, int slot, int32_t field, const double* vals, int64_t n);
+int sb_dense_values_write(sb_ctx* ctx, int slot, int32_t field, const int64_t* rows, const double* vals, int64_t n);
+int sb_dense_topk_where(sb_ctx* ctx, int slot, const float* q, int32_t B, int32_t k, const int32_t* p_off,
+                        const sb_pred* prog, const int32_t* pool, int32_t n_pool, int64_t* out_ids, double* out_scores,
+                        int32_t* out_counts);
+/*
  * Grouped dense search -- Qdrant's `search_groups(group_by=, limit=L, group_size=G, query_filter=)`: one answer per
  * document, not per chunk (the reference stamps every chunk with metadata.parent_id, text_splitter.py:143).
  *

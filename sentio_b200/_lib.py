@@ -61,6 +61,10 @@ SIGNATURES = {
                                              C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                              C.c_void_p]),
     "sb_dense_fallback_count": (C.c_int64, [C.c_void_p]),
+    "sb_dense_values_load": (C.c_int, [C.c_void_p, C.c_int, C.c_int32, C.c_void_p, C.c_int64]),
+    "sb_dense_values_write": (C.c_int, [C.c_void_p, C.c_int, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64]),
+    "sb_dense_topk_where": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                      C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "sb_dense_groups": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "sb_dense_group_rounds": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32]),

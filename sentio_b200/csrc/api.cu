@@ -70,6 +70,8 @@ void sb_destroy(sb_ctx* ctx) {
     if (ctx->dense[s].rows32) cudaFree(ctx->dense[s].rows32);
     for (int f = 0; f < SB_MAX_TAG_FIELDS; ++f)
       if (ctx->dense[s].tags[f]) cudaFree(ctx->dense[s].tags[f]);
+    for (int f = 0; f < SB_MAX_VALUE_FIELDS; ++f)
+      if (ctx->dense[s].vals[f]) cudaFree(ctx->dense[s].vals[f]);
   }
   Bm25Index& b = ctx->bm25;
   if (b.indptr) cudaFree(b.indptr);

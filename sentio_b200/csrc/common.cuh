@@ -116,6 +116,9 @@ struct DenseIndex {
   // payload index for filtered search (sb_dense_tags_load): tags[f][row] = dictionary code of field f, -1 = key absent;
   // nullptr = field f not loaded.  Dropped by sb_dense_load.
   int32_t* tags[SB_MAX_TAG_FIELDS] = {};
+  // numeric payload columns for range filters (sb_dense_values_load): vals[f][row] = the fp64 value, NaN = none;
+  // nullptr = not loaded.  Same capacity and mutation rules as the tag columns.  Dropped by sb_dense_load.
+  double* vals[SB_MAX_VALUE_FIELDS] = {};
 };
 
 struct Bm25Index {
@@ -170,8 +173,8 @@ struct sb_ctx {
   DevBuf qaux_dev;   // dense: per-query eps [B] fp32 | fallback flags [B] i32
   DevBuf fb_count_dev;   // dense: [1] u64, queries answered by the exact fallback kernel (sb_dense_fallback_count)
   DevBuf sigma_dev;      // dense float32 storage: [1] u64, bits of the largest sigma of the rows one load / upsert stores
-  DevBuf filt_dev;       // filtered dense: match mask | per-query counts / state | conditions (CSR)
-  PinBuf filt_pin;       // filtered dense: host copies of the conditions and the per-query match counts
+  DevBuf filt_dev;       // filtered dense: per-query counts / state | one chunk's filter programs | match mask
+  PinBuf filt_pin;       // filtered dense: host copies of the per-query counts / state and the programs
   // grouped dense search (sb_dense_groups): result [B][L][G] | one round's prefixes | replicated queries | completions
   DevBuf grp_res_dev, grp_round_dev, grp_q_dev, grp_cmp_dev;
   std::vector<int64_t> grp_rounds;   // [r]: grouped queries answered in r + 1 rounds (sb_dense_group_rounds)

@@ -20,6 +20,8 @@
 #include <string.h>
 #include <algorithm>
 #include <cmath>
+#include <string>
+#include <unordered_map>
 
 #include "dense_common.cuh"
 #include "dense_mma.cuh"
@@ -127,7 +129,8 @@ __global__ void dense_store_rows32_kernel(const TIn* __restrict__ in, int64_t n_
 
 // ------------------------------------------------------------------------------------------------ mutation kernels
 // sb_dense_delete's compaction: one warp per move from[m] -> to[m] (sources >= n - |D| > destinations, so one launch
-// has no read/write hazard): the fp16 row in 16-byte copies, its inverse norm and its code in every loaded tag column.
+// has no read/write hazard): the fp16 row in 16-byte copies, its inverse norm, its code in every loaded tag column and
+// its value in every loaded value column.
 struct MoveParams {
   __half* rows;
   float* inv_norm;
@@ -135,6 +138,7 @@ struct MoveParams {
   float* hh;                          // Euclid, else nullptr
   float* rows32;                      // float32 storage, else nullptr
   int32_t* tags[SB_MAX_TAG_FIELDS];   // nullptr = field not loaded
+  double* vals[SB_MAX_VALUE_FIELDS];  // likewise
   const int64_t* from;
   const int64_t* to;
   int64_t n_moves;
@@ -162,6 +166,9 @@ __global__ void __launch_bounds__(256) dense_move_rows_kernel(const MoveParams p
 #pragma unroll
   for (int f = 0; f < SB_MAX_TAG_FIELDS; ++f)
     if (lane == f + 1 && p.tags[f] != nullptr) p.tags[f][t] = p.tags[f][s];
+#pragma unroll
+  for (int f = 0; f < SB_MAX_VALUE_FIELDS; ++f)
+    if (lane == f + 16 && p.vals[f] != nullptr) p.vals[f][t] = p.vals[f][s];
 }
 
 // codes[i] -> col[rows[i]]; codes == nullptr writes -1 (an upserted row's payload is unknown until its codes arrive)
@@ -170,6 +177,14 @@ __global__ void __launch_bounds__(256) dense_tags_scatter_kernel(int32_t* __rest
                                                                  const int32_t* __restrict__ codes, int64_t n) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) col[rows[i]] = codes ? codes[i] : -1;
+}
+
+// vals[i] -> col[rows[i]]; vals == nullptr writes NaN (all bits set, the pattern of unused capacity)
+__global__ void __launch_bounds__(256) dense_values_scatter_kernel(double* __restrict__ col,
+                                                                   const int64_t* __restrict__ rows,
+                                                                   const double* __restrict__ vals, int64_t n) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) col[rows[i]] = vals ? vals[i] : __longlong_as_double(-1ll);
 }
 
 // ------------------------------------------------------------------------------------------------ scan kernel
@@ -914,78 +929,137 @@ __global__ void __launch_bounds__(kFbThreads, 1) dense_exact_fallback_kernel(con
 
 // ------------------------------------------------------------------------------------------------ filtered search
 // Match mask of a chunk of <= 256 queries: bit (row % 32) of mask[(row / 32) * qs + q] is set iff row < n satisfies
-// every condition of query q (no conditions: every row).  Each warp owns 32-row words (lane = row) and, per block of
-// 32 queries, ballots every query's predicate; lane j keeps query j's word, so a block of 32 query columns is one
-// 128-byte store.  counts[q] += popcount of its words.  Columns nq .. qs-1 are written as zero.
+// query q's program (sb_pred, DESIGN.md K1h; an empty program matches every row).  Legacy conjunctions and grouped
+// search's exclusion mode arrive here as programs too (dense_topk_filtered_enqueue).  One launch serves a group of the
+// chunk's DISTINCT programs, staged in shared memory with their code pools: each warp owns 32-row words (lane = row),
+// loads each column the chunk references once per row into its own shared-memory slot, evaluates every distinct program
+// once (boolean stack in a 64-bit register), ballots it, and writes the word to every query column that shares the
+// program, so a block of 32 query columns is one 128-byte store.  counts[q] += popcount of its words.
 constexpr int kGatherMax = 2048;   // queries with at most this many matching rows skip the scans (= winner buffer)
+constexpr int kWhereThreads = 256;
+constexpr int kWhereWarps = kWhereThreads / 32;
+constexpr int kWhereMaxPreds = 1536;          // program steps of one launch (staged: 60 KB)
+constexpr int kWhereMaxPoolStaged = 8192;     // codes of one launch's pools staged in shared memory; beyond: read from L2
 
-struct MaskParams {
-  const int32_t* const* tags;   // [SB_MAX_TAG_FIELDS] device pointers of the slot's tag columns
-  const int32_t* f_off;         // [nq + 1] (absolute offsets into f_field / f_code)
-  const int32_t* f_field;
-  const int32_t* f_code;
+struct WhereParams {
+  const int32_t* tag[SB_MAX_TAG_FIELDS];      // the columns the chunk references; program fields index these
+  const double* val[SB_MAX_VALUE_FIELDS];
+  int32_t n_tag, n_val;
+  const sb_pred* prog;                        // the launch's distinct programs, back to back
+  const int32_t* u_off;                       // [n_u + 1] program u is prog[u_off[u], u_off[u+1])
+  const int32_t* q_u;                         // [qs] query column -> program; -1 = zero column, -2 = another launch's
+  const int32_t* pool;                        // IN codes (offsets relative to this pointer)
+  int32_t n_preds, n_u, n_pool, pool_staged;
   int64_t n, n_words;
-  int32_t nq, qs;
-  uint32_t* mask;               // [n_words][qs]
-  int32_t* counts;              // [nq], zeroed by the caller
-  // exclusion mode (grouped search, K1f): x_field >= 0 also requires tags[x_field][row] >= 0 and absent from the query's
-  // codes [x_off[q], x_off[q+1]) of x_code, sorted ascending.  x_field = -1: off.
-  int32_t x_field;
-  const int32_t* x_off;         // [nq + 1] (absolute offsets into x_code)
-  const int32_t* x_code;
+  int32_t qs;
+  uint32_t* mask;                             // [n_words][qs]
+  int32_t* counts;                            // [qs], zeroed by the caller
 };
 
-// true iff v is one of the n ascending codes at a
-__device__ __forceinline__ bool sorted_codes_contain(const int32_t* __restrict__ a, int n, int32_t v) {
+// true iff v is one of the n ascending codes at a (shared or global memory)
+__device__ __forceinline__ bool sorted_codes_contain(const int32_t* a, int n, int32_t v) {
   int lo = 0, len = n;
   while (len > 0) {
     const int h = len >> 1;
-    if (__ldg(a + lo + h) < v) {
+    if (a[lo + h] < v) {
       lo += h + 1;
       len -= h + 1;
     } else {
       len = h;
     }
   }
-  return lo < n && __ldg(a + lo) == v;
+  return lo < n && a[lo] == v;
 }
 
-__global__ void __launch_bounds__(256) dense_filter_mask_kernel(const MaskParams p) {
-  const int lane = threadIdx.x & 31;
-  const int64_t warp0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-  int cnt[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // lane's query in block qb: qb * 32 + lane
+// One program on this thread's row: tg / vl point at the thread's slot of column 0 (column c is c * kWhereThreads on).
+// Bit 0 of st is the top of the stack; validation guarantees depth <= 64, so no bit is ever shifted out.
+__device__ __forceinline__ bool where_eval(const sb_pred* pr, int len, const int32_t* pool, const int32_t* tg,
+                                           const double* vl) {
+  uint64_t st = 0ull;
+  for (int i = 0; i < len; ++i) {
+    const sb_pred& p = pr[i];
+    const int op = p.op;
+    bool r;
+    if (op >= SB_PRED_AND) {
+      const int na = p.a;
+      const uint64_t m = na >= 64 ? ~0ull : (1ull << na) - 1ull;
+      const uint64_t x = st & m;
+      r = op == SB_PRED_AND ? x == m : op == SB_PRED_OR ? x != 0ull : op == SB_PRED_NOR ? x == 0ull : __popcll(x) >= p.b;
+      st = na >= 64 ? 0ull : st >> na;
+    } else if (op == SB_PRED_RANGE) {
+      const double v = vl[p.field * kWhereThreads];
+      r = (p.lo_incl ? v >= p.lo : v > p.lo) && (p.hi_incl ? v <= p.hi : v < p.hi);   // NaN: false
+    } else {
+      const int32_t t = tg[p.field * kWhereThreads];
+      r = op == SB_PRED_EQ ? t == p.a : op == SB_PRED_PRESENT ? t >= 0 : sorted_codes_contain(pool + p.a, p.b, t);
+    }
+    st = (st << 1) | (r ? 1ull : 0ull);
+  }
+  return len == 0 || (st & 1ull) != 0ull;
+}
+
+// dynamic shared memory of one launch: values [n_val][256] | programs | tags [n_tag][256] | u_off | bits [8][n_u] | pool
+__host__ __device__ inline size_t where_smem_bytes(int n_val, int n_preds, int n_tag, int n_u, int n_pool_staged) {
+  return (size_t)n_val * kWhereThreads * 8 + (size_t)n_preds * sizeof(sb_pred) + (size_t)n_tag * kWhereThreads * 4 +
+         (size_t)(n_u + 1) * 4 + (size_t)kWhereWarps * n_u * 4 + (size_t)n_pool_staged * 4;
+}
+
+__global__ void __launch_bounds__(kWhereThreads) dense_where_mask_kernel(const WhereParams p) {
+  extern __shared__ __align__(16) uint8_t wsm[];
+  double* s_val = reinterpret_cast<double*>(wsm);
+  sb_pred* s_prog = reinterpret_cast<sb_pred*>(s_val + (size_t)p.n_val * kWhereThreads);
+  int32_t* s_tag = reinterpret_cast<int32_t*>(s_prog + p.n_preds);
+  int32_t* s_uoff = s_tag + (size_t)p.n_tag * kWhereThreads;
+  uint32_t* s_bits = reinterpret_cast<uint32_t*>(s_uoff + p.n_u + 1);
+  int32_t* s_pool = reinterpret_cast<int32_t*>(s_bits + kWhereWarps * p.n_u);
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  {
+    const unsigned long long* src = reinterpret_cast<const unsigned long long*>(p.prog);
+    unsigned long long* dst = reinterpret_cast<unsigned long long*>(s_prog);
+    const int words = p.n_preds * (int)(sizeof(sb_pred) / 8);
+    for (int i = tid; i < words; i += kWhereThreads) dst[i] = __ldg(src + i);
+    for (int i = tid; i <= p.n_u; i += kWhereThreads) s_uoff[i] = __ldg(p.u_off + i);
+    if (p.pool_staged)
+      for (int i = tid; i < p.n_pool; i += kWhereThreads) s_pool[i] = __ldg(p.pool + i);
+  }
+  __syncthreads();
+  const int32_t* pool = p.pool_staged ? s_pool : p.pool;
+  int qu[8], cnt[8];
+#pragma unroll
+  for (int qb = 0; qb < 8; ++qb) {
+    qu[qb] = qb * 32 < p.qs ? __ldg(p.q_u + qb * 32 + lane) : -2;
+    cnt[qb] = 0;
+  }
+  uint32_t* bits = s_bits + warp * p.n_u;
+  int32_t* my_tag = s_tag + tid;
+  double* my_val = s_val + tid;
+  const int64_t warp0 = ((int64_t)blockIdx.x * kWhereThreads + tid) >> 5;
+  const int64_t nwarps = ((int64_t)gridDim.x * kWhereThreads) >> 5;
   for (int64_t w = warp0; w < p.n_words; w += nwarps) {
     const int64_t row = w * 32 + lane;
     const bool live = row < p.n;
+    // each thread reads back only its own slots: no barrier between these stores and where_eval's loads
+    for (int c = 0; c < p.n_tag; ++c) my_tag[c * kWhereThreads] = live ? __ldg(p.tag[c] + row) : -1;
+    for (int c = 0; c < p.n_val; ++c) my_val[c * kWhereThreads] = live ? __ldg(p.val[c] + row) : __longlong_as_double(-1ll);
+    for (int u = 0; u < p.n_u; ++u) {
+      const int b0 = s_uoff[u];
+      const bool m = live && where_eval(s_prog + b0, s_uoff[u + 1] - b0, pool, my_tag, my_val);
+      const uint32_t b = __ballot_sync(0xffffffffu, m);
+      if (lane == 0) bits[u] = b;
+    }
+    __syncwarp();
 #pragma unroll
     for (int qb = 0; qb < 8; ++qb) {
-      if (qb * 32 >= p.qs) break;
-      uint32_t mine = 0u;
-      for (int j = 0; j < 32; ++j) {
-        const int q = qb * 32 + j;
-        if (q >= p.nq) break;
-        bool m = live;
-        const int e = __ldg(p.f_off + q + 1);
-        for (int i = __ldg(p.f_off + q); i < e && m; ++i) {
-          const int32_t code = __ldg(p.f_code + i);
-          m = code >= 0 && __ldg(p.tags[__ldg(p.f_field + i)] + row) == code;
-        }
-        if (m && p.x_field >= 0) {
-          const int32_t g = __ldg(p.tags[p.x_field] + row);
-          const int x0 = __ldg(p.x_off + q);
-          m = g >= 0 && !sorted_codes_contain(p.x_code + x0, __ldg(p.x_off + q + 1) - x0, g);
-        }
-        const uint32_t bits = __ballot_sync(0xffffffffu, m);
-        if (lane == j) mine = bits;
-      }
+      if (qu[qb] == -2) continue;
+      const uint32_t mine = qu[qb] >= 0 ? bits[qu[qb]] : 0u;
       p.mask[(size_t)w * p.qs + qb * 32 + lane] = mine;
       cnt[qb] += __popc(mine);
     }
+    __syncwarp();   // bits[] is rewritten for the next word
   }
 #pragma unroll
   for (int qb = 0; qb < 8; ++qb)
-    if (qb * 32 + lane < p.nq && cnt[qb] > 0) atomicAdd(p.counts + qb * 32 + lane, cnt[qb]);
+    if (qu[qb] >= 0 && cnt[qb] > 0) atomicAdd(p.counts + qb * 32 + lane, cnt[qb]);
 }
 
 // Exact path of a low-cardinality query (<= kGatherMax matching rows): one CTA compacts the query's matching rows out
@@ -1504,41 +1578,193 @@ int dense_fallback_enqueue(sb_ctx* ctx, const DenseIndex& ix, const float* q_pad
 
 namespace {
 
-// Filtered top-k of B queries (q_pad on the device; conditions as host CSR arrays) in chunks of <= 256 queries: per
-// chunk the match mask + match counts, one wait for the counts, then the gather path for low-cardinality queries and
-// the masked scans for the rest.  x_field >= 0 adds the exclusion mode of the mask (MaskParams; host CSR x_off / x_code):
-// every query is then filtered.
-int dense_topk_filtered_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int B, int k, const int32_t* f_off,
-                                const int32_t* f_field, const int32_t* f_code, int64_t* out_ids, double* out_scores,
-                                int32_t* out_counts, cudaStream_t st, int x_field = -1, const int32_t* x_off = nullptr,
-                                const int32_t* x_code = nullptr) {
-  SB_REQUIRE(k <= kDenseMaxK, SB_ERR_UNSUPPORTED, "dense: top_k %d too large (max %d per call)", k, kDenseMaxK);
-  SB_REQUIRE(f_off[0] == 0, SB_ERR_ARG, "sb_dense_topk_filtered: f_off[0] must be 0");
-  for (int b = 0; b < B; ++b)
-    SB_REQUIRE(f_off[b + 1] >= f_off[b], SB_ERR_ARG, "sb_dense_topk_filtered: f_off is not non-decreasing at %d", b);
-  const int n_conds = f_off[B];
-  for (int i = 0; i < n_conds; ++i) {
-    const int f = f_field[i];
-    SB_REQUIRE(f >= 0 && f < SB_MAX_TAG_FIELDS, SB_ERR_ARG, "sb_dense_topk_filtered: field %d out of range", f);
-    SB_REQUIRE(ix.tags[f] != nullptr, SB_ERR_STATE, "sb_dense_topk_filtered: field %d has no tag column loaded", f);
+size_t align16(size_t v) { return (v + 15) / 16 * 16; }
+
+// The public program input, checked before anything is launched: offsets, op codes, loaded fields, pool ranges in bounds
+// and ascending, a well-formed stack, the limits (include/sentio_b200.h, sb_dense_topk_where).
+int where_validate(const char* who, const DenseIndex& ix, int B, const int32_t* p_off, const sb_pred* prog,
+                   const int32_t* pool, int32_t n_pool) {
+  SB_REQUIRE(p_off[0] == 0, SB_ERR_ARG, "%s: p_off[0] must be 0", who);
+  SB_REQUIRE(n_pool >= 0 && (n_pool == 0 || pool != nullptr), SB_ERR_ARG, "%s: bad pool (n_pool=%d)", who, n_pool);
+  for (int b = 0; b < B; ++b) {
+    const int32_t p0 = p_off[b], p1 = p_off[b + 1];
+    SB_REQUIRE(p1 >= p0, SB_ERR_ARG, "%s: p_off is not non-decreasing at %d", who, b);
+    SB_REQUIRE(p1 - p0 <= SB_MAX_PRED, SB_ERR_ARG, "%s: query %d has %d program steps (max %d)", who, b, p1 - p0,
+               SB_MAX_PRED);
+    int depth = 0;
+    for (int32_t i = p0; i < p1; ++i) {
+      const sb_pred& e = prog[i];
+      SB_REQUIRE(e.op >= SB_PRED_EQ && e.op <= SB_PRED_ATLEAST, SB_ERR_ARG, "%s: step %d has op %d", who, i, e.op);
+      if (e.op == SB_PRED_RANGE) {
+        SB_REQUIRE(e.field >= 0 && e.field < SB_MAX_VALUE_FIELDS, SB_ERR_ARG, "%s: step %d: value field %d out of range",
+                   who, i, e.field);
+        SB_REQUIRE(ix.vals[e.field] != nullptr, SB_ERR_STATE, "%s: value field %d has no column loaded", who, e.field);
+        SB_REQUIRE(!std::isnan(e.lo) && !std::isnan(e.hi), SB_ERR_ARG, "%s: step %d: NaN range bound", who, i);
+        SB_REQUIRE((e.lo_incl == 0 || e.lo_incl == 1) && (e.hi_incl == 0 || e.hi_incl == 1), SB_ERR_ARG,
+                   "%s: step %d: inclusive flags must be 0 or 1", who, i);
+      } else if (e.op <= SB_PRED_PRESENT) {
+        SB_REQUIRE(e.field >= 0 && e.field < SB_MAX_TAG_FIELDS, SB_ERR_ARG, "%s: step %d: tag field %d out of range", who,
+                   i, e.field);
+        SB_REQUIRE(ix.tags[e.field] != nullptr, SB_ERR_STATE, "%s: field %d has no tag column loaded", who, e.field);
+        SB_REQUIRE(e.op != SB_PRED_EQ || e.a >= 0, SB_ERR_ARG, "%s: step %d: EQ code %d (must be >= 0)", who, i, e.a);
+        if (e.op == SB_PRED_IN) {
+          SB_REQUIRE(e.a >= 0 && e.b >= 0 && (int64_t)e.a + e.b <= n_pool, SB_ERR_ARG,
+                     "%s: step %d: pool range [%d, %d + %d) outside [0, %d)", who, i, e.a, e.a, e.b, n_pool);
+          for (int32_t j = e.a; j < e.a + e.b; ++j)
+            SB_REQUIRE(pool[j] >= 0 && (j == e.a || pool[j] > pool[j - 1]), SB_ERR_ARG,
+                       "%s: step %d: pool codes must be >= 0 and strictly ascending (pool[%d] = %d)", who, i, j, pool[j]);
+        }
+      }
+      if (e.op <= SB_PRED_PRESENT) {
+        depth += 1;
+      } else {
+        SB_REQUIRE(e.a >= 0 && e.a <= depth, SB_ERR_ARG, "%s: step %d pops %d of %d stack entries", who, i, e.a, depth);
+        depth += 1 - e.a;
+      }
+      SB_REQUIRE(depth <= SB_MAX_PRED_STACK, SB_ERR_ARG, "%s: query %d's program needs more than %d stack entries", who,
+                 b, SB_MAX_PRED_STACK);
+    }
+    SB_REQUIRE(p1 == p0 || depth == 1, SB_ERR_ARG, "%s: query %d's program leaves %d stack entries (must be 1)", who, b,
+               depth);
   }
-  const bool excl = x_field >= 0;
-  if (n_conds == 0 && !excl)   // no query has a condition: exactly the unfiltered search
+  return SB_OK;
+}
+
+// One mask launch of a chunk: a group of its distinct programs (staged at the given offsets of the chunk's bytes)
+struct WhereLaunch {
+  size_t o_prog, o_uoff, o_qu, o_pool;
+  int n_preds, n_u, n_pool;
+};
+
+// The host side of one chunk's mask: its distinct programs in launch groups, fields remapped to the chunk's columns
+struct WhereChunk {
+  std::vector<uint8_t> bytes;
+  std::vector<WhereLaunch> launches;
+  int n_tag = 0, n_val = 0;
+  int tag_f[SB_MAX_TAG_FIELDS], val_f[SB_MAX_VALUE_FIELDS];
+};
+
+template <typename T>
+size_t put(std::vector<uint8_t>& v, const T* src, size_t n) {
+  const size_t o = (v.size() + 15) / 16 * 16;
+  v.resize(o + n * sizeof(T));
+  if (n) memcpy(v.data() + o, src, n * sizeof(T));
+  return o;
+}
+
+void where_plan_chunk(const int32_t* p_off, const sb_pred* prog, const int32_t* pool, int c0, int nq, int qs,
+                      WhereChunk& ch) {
+  int slot_t[SB_MAX_TAG_FIELDS], slot_v[SB_MAX_VALUE_FIELDS];
+  std::fill(slot_t, slot_t + SB_MAX_TAG_FIELDS, -1);
+  std::fill(slot_v, slot_v + SB_MAX_VALUE_FIELDS, -1);
+  // distinct programs by content (an IN leaf by its codes, not by where they sit in the pool)
+  std::unordered_map<std::string, int> seen;
+  std::vector<int> uq(nq), rep;
+  for (int q = 0; q < nq; ++q) {
+    std::string key;
+    for (int32_t i = p_off[c0 + q]; i < p_off[c0 + q + 1]; ++i) {
+      const sb_pred& e = prog[i];
+      key.append(reinterpret_cast<const char*>(&e.op), 8);   // op, field
+      if (e.op == SB_PRED_IN) {
+        key.append(reinterpret_cast<const char*>(&e.b), 4);
+        key.append(reinterpret_cast<const char*>(pool + e.a), (size_t)e.b * 4);
+      } else {
+        key.append(reinterpret_cast<const char*>(&e.a), sizeof(sb_pred) - 8);
+      }
+    }
+    auto it = seen.emplace(key, (int)rep.size());
+    if (it.second) rep.push_back(q);
+    uq[q] = it.first->second;
+  }
+  // launch groups of consecutive distinct programs, each within the staged-program budget (SB_MAX_PRED <= the budget)
+  std::vector<int> group_of(rep.size()), local(rep.size());
+  std::vector<int> g_first;
+  int cur = 0;
+  for (size_t u = 0; u < rep.size(); ++u) {
+    const int len = p_off[c0 + rep[u] + 1] - p_off[c0 + rep[u]];
+    if (g_first.empty() || cur + len > kWhereMaxPreds) {
+      g_first.push_back((int)u);
+      cur = 0;
+    }
+    group_of[u] = (int)g_first.size() - 1;
+    local[u] = (int)u - g_first.back();
+    cur += len;
+  }
+  for (size_t g = 0; g < g_first.size(); ++g) {
+    const size_t u1 = g + 1 < g_first.size() ? (size_t)g_first[g + 1] : rep.size();
+    std::vector<sb_pred> gp;
+    std::vector<int32_t> uoff(1, 0), gpool, qu(qs);
+    for (size_t u = g_first[g]; u < u1; ++u) {
+      const int q = rep[u];
+      for (int32_t i = p_off[c0 + q]; i < p_off[c0 + q + 1]; ++i) {
+        sb_pred e = prog[i];
+        if (e.op == SB_PRED_RANGE) {
+          if (slot_v[e.field] < 0) {
+            slot_v[e.field] = ch.n_val;
+            ch.val_f[ch.n_val++] = e.field;
+          }
+          e.field = slot_v[e.field];
+        } else if (e.op <= SB_PRED_PRESENT) {
+          if (slot_t[e.field] < 0) {
+            slot_t[e.field] = ch.n_tag;
+            ch.tag_f[ch.n_tag++] = e.field;
+          }
+          e.field = slot_t[e.field];
+          if (e.op == SB_PRED_IN) {
+            const int32_t a = (int32_t)gpool.size();
+            gpool.insert(gpool.end(), pool + e.a, pool + e.a + e.b);
+            e.a = a;
+          }
+        } else {
+          e.field = 0;
+        }
+        gp.push_back(e);
+      }
+      uoff.push_back((int32_t)gp.size());
+    }
+    for (int q = 0; q < qs; ++q)
+      qu[q] = q >= nq ? (g == 0 ? -1 : -2) : group_of[uq[q]] == (int)g ? local[uq[q]] : -2;
+    WhereLaunch L;
+    L.n_preds = (int)gp.size();
+    L.n_u = (int)(u1 - g_first[g]);
+    L.n_pool = (int)gpool.size();
+    L.o_prog = put(ch.bytes, gp.data(), gp.size());
+    L.o_uoff = put(ch.bytes, uoff.data(), uoff.size());
+    L.o_qu = put(ch.bytes, qu.data(), qu.size());
+    L.o_pool = put(ch.bytes, gpool.data(), gpool.size());
+    ch.launches.push_back(L);
+  }
+}
+
+// Filtered top-k of B queries (q_pad on the device; one validated program per query, host arrays) in chunks of <= 256
+// queries: per chunk the match mask + match counts, one wait for the counts, then the gather path for low-cardinality
+// queries and the masked scans for the rest.  A batch of empty programs is the unfiltered search.
+int dense_topk_where_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int B, int k, const int32_t* p_off,
+                             const sb_pred* prog, const int32_t* pool, int64_t* out_ids, double* out_scores,
+                             int32_t* out_counts, cudaStream_t st) {
+  SB_REQUIRE(k <= kDenseMaxK, SB_ERR_UNSUPPORTED, "dense: top_k %d too large (max %d per call)", k, kDenseMaxK);
+  if (p_off[B] == 0)   // no query has a program: exactly the unfiltered search
     return dense_topk_enqueue(ctx, ix, q_pad, B, k, out_ids, out_scores, out_counts, st);
-  const int n_x = excl ? x_off[B] : 0;
 
   const int64_t n_words = ix.n_pad / 32;
   int qchunk = 256;   // queries per mask; the mask (n_pad * qchunk / 8 bytes) is kept under 1 GB
   while (qchunk > 32 && (size_t)n_words * 4 * qchunk > (1ull << 30)) qchunk >>= 1;
-  // device: tag pointers | f_off | f_field | f_code | x_off | x_code | counts [qchunk] | state [qchunk] | qlist [qchunk] |
-  // mask
-  const size_t o_off = 128, o_field = o_off + ((size_t)(B + 1) * 4 + 15) / 16 * 16;
-  const size_t o_code = o_field + ((size_t)n_conds * 4 + 15) / 16 * 16;
-  const size_t o_xoff = o_code + ((size_t)n_conds * 4 + 15) / 16 * 16;
-  const size_t o_xcode = o_xoff + (excl ? ((size_t)(B + 1) * 4 + 15) / 16 * 16 : 0);
-  const size_t o_cnt = o_xcode + ((size_t)n_x * 4 + 15) / 16 * 16;
-  const size_t o_state = o_cnt + (size_t)qchunk * 4, o_qlist = o_state + (size_t)qchunk * 4;
-  const size_t o_mask = (o_qlist + (size_t)qchunk * 4 + 255) / 256 * 256;
+  std::vector<WhereChunk> chunks((B + qchunk - 1) / qchunk);
+  size_t stage_bytes = 0, smem_max = 0;
+  for (size_t c = 0; c < chunks.size(); ++c) {
+    const int c0 = (int)c * qchunk, nq = std::min(qchunk, B - c0);
+    WhereChunk& ch = chunks[c];
+    where_plan_chunk(p_off, prog, pool, c0, nq, std::max(32, next_pow2(nq)), ch);
+    stage_bytes = std::max(stage_bytes, ch.bytes.size());
+    for (const WhereLaunch& L : ch.launches) {
+      const int staged = L.n_pool <= kWhereMaxPoolStaged ? L.n_pool : 0;
+      smem_max = std::max(smem_max, where_smem_bytes(ch.n_val, L.n_preds, ch.n_tag, L.n_u, staged));
+    }
+  }
+  // device: counts [qchunk] | state [qchunk] | qlist [qchunk] | one chunk's programs | mask
+  const size_t o_cnt = 0, o_state = (size_t)qchunk * 4, o_qlist = o_state + (size_t)qchunk * 4;
+  const size_t o_stage = align16(o_qlist + (size_t)qchunk * 4);
+  const size_t o_mask = (o_stage + stage_bytes + 255) / 256 * 256;
   const size_t dev_bytes = o_mask + (size_t)n_words * qchunk * 4;
   int rc;
   if ((rc = ctx->filt_dev.reserve(dev_bytes))) return rc;
@@ -1546,15 +1772,6 @@ int dense_topk_filtered_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad,
   uint8_t* dv = ctx->filt_dev.as<uint8_t>();
   uint8_t* hp = ctx->filt_pin.as<uint8_t>();
   SB_CUDA(cudaStreamSynchronize(st));   // the pinned staging may still feed an earlier call's copies
-  memcpy(hp, ix.tags, sizeof(ix.tags));
-  memcpy(hp + o_off, f_off, (size_t)(B + 1) * 4);
-  memcpy(hp + o_field, f_field, (size_t)n_conds * 4);
-  memcpy(hp + o_code, f_code, (size_t)n_conds * 4);
-  if (excl) {
-    memcpy(hp + o_xoff, x_off, (size_t)(B + 1) * 4);
-    memcpy(hp + o_xcode, x_code, (size_t)n_x * 4);
-  }
-  SB_CUDA(cudaMemcpyAsync(dv, hp, o_cnt, cudaMemcpyHostToDevice, st));
   int32_t* cnt_h = reinterpret_cast<int32_t*>(hp + o_cnt);
   int32_t* state_h = reinterpret_cast<int32_t*>(hp + o_state);
   int32_t* qlist_h = reinterpret_cast<int32_t*>(hp + o_qlist);
@@ -1562,41 +1779,53 @@ int dense_topk_filtered_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad,
   int32_t* state_d = reinterpret_cast<int32_t*>(dv + o_state);
   int32_t* qlist_d = reinterpret_cast<int32_t*>(dv + o_qlist);
   uint32_t* mask = reinterpret_cast<uint32_t*>(dv + o_mask);
+  SB_REQUIRE(smem_max <= ctx->smem_optin, SB_ERR_UNSUPPORTED, "dense: filter programs need %zu bytes of shared memory",
+             smem_max);
+  SB_CUDA(cudaFuncSetAttribute(dense_where_mask_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max));
   const size_t gather_smem = (size_t)kGatherMax * 20 + (size_t)ix.d_pad * 4 + 64;
   auto gather_kern = ix.rows32 ? dense_filter_gather_kernel<true> : dense_filter_gather_kernel<false>;
   SB_CUDA(cudaFuncSetAttribute(gather_kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gather_smem));
   for (int c0 = 0; c0 < B; c0 += qchunk) {
     const int nq = std::min(qchunk, B - c0);
     const int qs = std::max(32, next_pow2(nq));   // >= the widest wgmma group of the chunk
-    SB_CUDA(cudaMemsetAsync(cnt_d, 0, (size_t)nq * 4, st));
-    MaskParams mk;
-    mk.tags = reinterpret_cast<const int32_t* const*>(dv);
-    mk.f_off = reinterpret_cast<const int32_t*>(dv + o_off) + c0;
-    mk.f_field = reinterpret_cast<const int32_t*>(dv + o_field);
-    mk.f_code = reinterpret_cast<const int32_t*>(dv + o_code);
-    mk.n = ix.n;
-    mk.n_words = n_words;
-    mk.nq = nq;
-    mk.qs = qs;
-    mk.mask = mask;
-    mk.counts = cnt_d;
-    mk.x_field = x_field;
-    mk.x_off = excl ? reinterpret_cast<const int32_t*>(dv + o_xoff) + c0 : nullptr;
-    mk.x_code = excl ? reinterpret_cast<const int32_t*>(dv + o_xcode) : nullptr;
-    const int64_t blocks = std::min<int64_t>((n_words + 7) / 8, (int64_t)ctx->num_sms * 8);
-    {
+    const WhereChunk& ch = chunks[c0 / qchunk];
+    memcpy(hp + o_stage, ch.bytes.data(), ch.bytes.size());
+    SB_CUDA(cudaMemcpyAsync(dv + o_stage, hp + o_stage, ch.bytes.size(), cudaMemcpyHostToDevice, st));
+    SB_CUDA(cudaMemsetAsync(cnt_d, 0, (size_t)qs * 4, st));
+    WhereParams wp;
+    for (int c = 0; c < ch.n_tag; ++c) wp.tag[c] = ix.tags[ch.tag_f[c]];
+    for (int c = 0; c < ch.n_val; ++c) wp.val[c] = ix.vals[ch.val_f[c]];
+    wp.n_tag = ch.n_tag;
+    wp.n_val = ch.n_val;
+    wp.n = ix.n;
+    wp.n_words = n_words;
+    wp.qs = qs;
+    wp.mask = mask;
+    wp.counts = cnt_d;
+    const uint8_t* sd = dv + o_stage;
+    for (const WhereLaunch& L : ch.launches) {
+      wp.prog = reinterpret_cast<const sb_pred*>(sd + L.o_prog);
+      wp.u_off = reinterpret_cast<const int32_t*>(sd + L.o_uoff);
+      wp.q_u = reinterpret_cast<const int32_t*>(sd + L.o_qu);
+      wp.pool = reinterpret_cast<const int32_t*>(sd + L.o_pool);
+      wp.n_preds = L.n_preds;
+      wp.n_u = L.n_u;
+      wp.n_pool = L.n_pool;
+      wp.pool_staged = L.n_pool <= kWhereMaxPoolStaged ? 1 : 0;
+      const size_t smem = where_smem_bytes(ch.n_val, L.n_preds, ch.n_tag, L.n_u, wp.pool_staged ? L.n_pool : 0);
+      const int64_t blocks = std::min<int64_t>((n_words + kWhereWarps - 1) / kWhereWarps, (int64_t)ctx->num_sms * 8);
       ProfScope ps(ctx, SB_PROF_DENSE_FILTER, st);
-      dense_filter_mask_kernel<<<(unsigned)blocks, 256, 0, st>>>(mk);
+      dense_where_mask_kernel<<<(unsigned)blocks, kWhereThreads, smem, st>>>(wp);
     }
     SB_CUDA(cudaGetLastError());
     SB_CUDA(cudaMemcpyAsync(cnt_h, cnt_d, (size_t)nq * 4, cudaMemcpyDeviceToHost, st));
     SB_CUDA(cudaStreamSynchronize(st));
     // route: a filtered query with <= kGatherMax matching rows is answered exactly from its matches; the others are
-    // scanned with the mask (a query without conditions matches every row)
+    // scanned with the mask (a query without a program matches every row)
     int n_gather = 0;
     int64_t c_min = ix.n;
     for (int q = 0; q < nq; ++q) {
-      const bool filtered = excl || f_off[c0 + q + 1] > f_off[c0 + q];
+      const bool filtered = p_off[c0 + q + 1] > p_off[c0 + q];
       const bool gather = filtered && cnt_h[q] <= kGatherMax;
       state_h[q] = gather ? 1 : 0;
       if (gather) qlist_h[n_gather++] = q;
@@ -1642,7 +1871,67 @@ int dense_topk_filtered_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad,
   return SB_OK;
 }
 
-size_t align16(size_t v) { return (v + 15) / 16 * 16; }
+
+// Legacy conditions (CSR f_off / f_field / f_code, conjunctions of "tag == code") and grouped search's exclusion mode
+// (x_field >= 0: the row's code at x_field must be present and absent from the query's ascending x_code range) as
+// programs: per query the conjunction reduced to one EQ leaf per field (a negative code, or two codes on one field,
+// match nothing: one empty IN leaf), then PRESENT(x) AND NOR(IN(x, codes)), under one AND.  Every query is filtered in
+// exclusion mode; without it a query without conditions gets the empty program (unfiltered).
+int dense_topk_filtered_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int B, int k, const int32_t* f_off,
+                                const int32_t* f_field, const int32_t* f_code, int64_t* out_ids, double* out_scores,
+                                int32_t* out_counts, cudaStream_t st, int x_field = -1, const int32_t* x_off = nullptr,
+                                const int32_t* x_code = nullptr) {
+  SB_REQUIRE(f_off[0] == 0, SB_ERR_ARG, "sb_dense_topk_filtered: f_off[0] must be 0");
+  for (int b = 0; b < B; ++b)
+    SB_REQUIRE(f_off[b + 1] >= f_off[b], SB_ERR_ARG, "sb_dense_topk_filtered: f_off is not non-decreasing at %d", b);
+  const int n_conds = f_off[B];
+  for (int i = 0; i < n_conds; ++i) {
+    const int f = f_field[i];
+    SB_REQUIRE(f >= 0 && f < SB_MAX_TAG_FIELDS, SB_ERR_ARG, "sb_dense_topk_filtered: field %d out of range", f);
+    SB_REQUIRE(ix.tags[f] != nullptr, SB_ERR_STATE, "sb_dense_topk_filtered: field %d has no tag column loaded", f);
+  }
+  std::vector<int32_t> p_off(B + 1, 0), pool;
+  std::vector<sb_pred> prog;
+  auto leaf = [&](int op, int field, int a, int b) {
+    sb_pred e = {};
+    e.op = op;
+    e.field = field;
+    e.a = a;
+    e.b = b;
+    prog.push_back(e);
+  };
+  for (int b = 0; b < B; ++b) {
+    int32_t code_of[SB_MAX_TAG_FIELDS];
+    std::fill(code_of, code_of + SB_MAX_TAG_FIELDS, -2);
+    bool none = false;
+    for (int i = f_off[b]; i < f_off[b + 1]; ++i) {
+      const int f = f_field[i], c = f_code[i];
+      none |= c < 0 || (code_of[f] != -2 && code_of[f] != c);
+      code_of[f] = c;
+    }
+    if (none) {
+      leaf(SB_PRED_IN, f_field[f_off[b]], 0, 0);
+    } else {
+      int n = 0;
+      for (int f = 0; f < SB_MAX_TAG_FIELDS; ++f)
+        if (code_of[f] >= 0) {
+          leaf(SB_PRED_EQ, f, code_of[f], 0);
+          ++n;
+        }
+      if (x_field >= 0) {
+        leaf(SB_PRED_PRESENT, x_field, 0, 0);
+        leaf(SB_PRED_IN, x_field, (int32_t)pool.size(), x_off[b + 1] - x_off[b]);
+        pool.insert(pool.end(), x_code + x_off[b], x_code + x_off[b + 1]);
+        leaf(SB_PRED_NOR, 0, 1, 0);
+        n += 2;
+      }
+      if (n > 1) leaf(SB_PRED_AND, 0, n, 0);
+    }
+    p_off[b + 1] = (int32_t)prog.size();
+  }
+  return dense_topk_where_enqueue(ctx, ix, q_pad, B, k, p_off.data(), prog.data(), pool.data(), out_ids, out_scores,
+                                  out_counts, st);
+}
 
 // Grouped search of B padded queries (DESIGN.md K1f) into ctx->grp_res_dev, laid out n_groups [B] | g_code [B][L] |
 // g_hits [B][L] | h_ids [B][L][G] | h_scores [B][L][G] (offsets in *o).  Every step consumes an exact ordered prefix:
@@ -1880,8 +2169,8 @@ int dense_store_staged(sb_ctx* ctx, DenseIndex& ix, const void* vecs, int64_t n,
   return SB_OK;
 }
 
-// Reallocate rows / inv_norm / cfac / hh / every loaded tag column to n_cap rows (> ix.n_cap): the [0, n_pad) prefix is
-// copied device to device, the rest is zero (tags -1).  Old and new buffers coexist during the copy.
+// Reallocate rows / inv_norm / cfac / hh / every loaded tag and value column to n_cap rows (> ix.n_cap): the [0, n_pad)
+// prefix is copied device to device, the rest is zero (tags -1, values NaN).  Old and new buffers coexist during the copy.
 int dense_grow(sb_ctx* ctx, DenseIndex& ix, int64_t n_cap) {
   const size_t rb = (size_t)ix.d_pad * sizeof(__half);
   __half* rows = nullptr;
@@ -1891,6 +2180,7 @@ int dense_grow(sb_ctx* ctx, DenseIndex& ix, int64_t n_cap) {
   float* rows32 = nullptr;
   const size_t rb32 = (size_t)ix.d_pad * sizeof(float);
   int32_t* tags[SB_MAX_TAG_FIELDS] = {};
+  double* vals[SB_MAX_VALUE_FIELDS] = {};
   cudaError_t e = cudaMalloc(&rows, (size_t)n_cap * rb);
   if (e == cudaSuccess) e = cudaMalloc(&inv, (size_t)n_cap * sizeof(float));
   if (e == cudaSuccess && ix.metric != SB_METRIC_COSINE) e = cudaMalloc(&cfac, (size_t)n_cap * sizeof(double));
@@ -1898,6 +2188,8 @@ int dense_grow(sb_ctx* ctx, DenseIndex& ix, int64_t n_cap) {
   if (e == cudaSuccess && ix.storage == SB_STORAGE_F32) e = cudaMalloc(&rows32, (size_t)n_cap * rb32);
   for (int f = 0; f < SB_MAX_TAG_FIELDS && e == cudaSuccess; ++f)
     if (ix.tags[f]) e = cudaMalloc(&tags[f], (size_t)n_cap * 4);
+  for (int f = 0; f < SB_MAX_VALUE_FIELDS && e == cudaSuccess; ++f)
+    if (ix.vals[f]) e = cudaMalloc(&vals[f], (size_t)n_cap * 8);
   const int64_t keep = ix.n_pad;
   cudaStream_t st = ctx->stream;
   if (e == cudaSuccess && keep) e = cudaMemcpyAsync(rows, ix.rows, (size_t)keep * rb, cudaMemcpyDeviceToDevice, st);
@@ -1923,6 +2215,11 @@ int dense_grow(sb_ctx* ctx, DenseIndex& ix, int64_t n_cap) {
     if (keep) e = cudaMemcpyAsync(tags[f], ix.tags[f], (size_t)keep * 4, cudaMemcpyDeviceToDevice, st);
     if (e == cudaSuccess) e = cudaMemsetAsync(tags[f] + keep, 0xff, (size_t)(n_cap - keep) * 4, st);
   }
+  for (int f = 0; f < SB_MAX_VALUE_FIELDS && e == cudaSuccess; ++f) {
+    if (!vals[f]) continue;
+    if (keep) e = cudaMemcpyAsync(vals[f], ix.vals[f], (size_t)keep * 8, cudaMemcpyDeviceToDevice, st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(vals[f] + keep, 0xff, (size_t)(n_cap - keep) * 8, st);
+  }
   if (e == cudaSuccess) e = cudaStreamSynchronize(st);
   if (e != cudaSuccess) {   // the slot keeps its old buffers; the new ones are released on every failure
     cudaStreamSynchronize(st);
@@ -1932,6 +2229,7 @@ int dense_grow(sb_ctx* ctx, DenseIndex& ix, int64_t n_cap) {
     cudaFree(hh);
     cudaFree(rows32);
     for (int f = 0; f < SB_MAX_TAG_FIELDS; ++f) cudaFree(tags[f]);
+    for (int f = 0; f < SB_MAX_VALUE_FIELDS; ++f) cudaFree(vals[f]);
     sb_set_error("dense: growing slot to %lld rows failed: %s", (long long)n_cap, cudaGetErrorString(e));
     return SB_ERR_CUDA;
   }
@@ -1949,6 +2247,11 @@ int dense_grow(sb_ctx* ctx, DenseIndex& ix, int64_t n_cap) {
     if (ix.tags[f]) {
       cudaFree(ix.tags[f]);
       ix.tags[f] = tags[f];
+    }
+  for (int f = 0; f < SB_MAX_VALUE_FIELDS; ++f)
+    if (ix.vals[f]) {
+      cudaFree(ix.vals[f]);
+      ix.vals[f] = vals[f];
     }
   ix.n_cap = n_cap;
   return SB_OK;
@@ -2045,6 +2348,8 @@ int sb_dense_load_storage(sb_ctx* ctx, int slot, const void* vecs, int64_t n, in
   if (ix.rows32) cudaFree(ix.rows32);
   for (int f = 0; f < SB_MAX_TAG_FIELDS; ++f)
     if (ix.tags[f]) cudaFree(ix.tags[f]);
+  for (int f = 0; f < SB_MAX_VALUE_FIELDS; ++f)
+    if (ix.vals[f]) cudaFree(ix.vals[f]);
   ix = DenseIndex();
   ix.n = n;
   ix.d = d;
@@ -2146,6 +2451,9 @@ int sb_dense_upsert(sb_ctx* ctx, int slot, const int64_t* rows, const void* vecs
   for (int f = 0; f < SB_MAX_TAG_FIELDS; ++f)
     if (ix.tags[f])
       dense_tags_scatter_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(ix.tags[f], dst, nullptr, n);
+  for (int f = 0; f < SB_MAX_VALUE_FIELDS; ++f)
+    if (ix.vals[f])
+      dense_values_scatter_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(ix.vals[f], dst, nullptr, n);
   SB_CUDA(cudaGetLastError());
   SB_CUDA(cudaStreamSynchronize(ctx->stream));
   ix.n = n_new;
@@ -2228,6 +2536,7 @@ int sb_dense_delete(sb_ctx* ctx, int slot, const int64_t* rows, int64_t n, int64
     mp.hh = ix.hh;
     mp.rows32 = ix.rows32;
     memcpy(mp.tags, ix.tags, sizeof(mp.tags));
+    memcpy(mp.vals, ix.vals, sizeof(mp.vals));
     mp.from = f_dev;
     mp.to = f_dev + mv;
     mp.n_moves = mv;
@@ -2244,6 +2553,8 @@ int sb_dense_delete(sb_ctx* ctx, int slot, const int64_t* rows, int64_t n, int64
     SB_CUDA(cudaMemsetAsync(ix.rows32 + (size_t)keep * ix.d_pad, 0, (size_t)n * ix.d_pad * sizeof(float), ctx->stream));
   for (int f = 0; f < SB_MAX_TAG_FIELDS; ++f)
     if (ix.tags[f]) SB_CUDA(cudaMemsetAsync(ix.tags[f] + keep, 0xff, (size_t)n * 4, ctx->stream));
+  for (int f = 0; f < SB_MAX_VALUE_FIELDS; ++f)
+    if (ix.vals[f]) SB_CUDA(cudaMemsetAsync(ix.vals[f] + keep, 0xff, (size_t)n * 8, ctx->stream));
   SB_CUDA(cudaStreamSynchronize(ctx->stream));
   ix.n = keep;
   ix.n_pad = round_rows(keep);
@@ -2466,6 +2777,99 @@ int sb_dense_topk_filtered(sb_ctx* ctx, int slot, const float* q, int32_t B, int
   if ((rc = ctx->out_cnt_dev.reserve((size_t)B * 4))) return rc;
   if ((rc = dense_topk_filtered_enqueue(ctx, ix, q_pad, B, k, f_off, f_field, f_code, ctx->out_ids_dev.as<int64_t>(),
                                         ctx->out_sc_dev.as<double>(), ctx->out_cnt_dev.as<int32_t>(), st)))
+    return rc;
+  SB_CUDA(cudaMemcpyAsync(out_ids, ctx->out_ids_dev.p, nid * 8, cudaMemcpyDeviceToHost, st));
+  SB_CUDA(cudaMemcpyAsync(out_scores, ctx->out_sc_dev.p, nid * 8, cudaMemcpyDeviceToHost, st));
+  SB_CUDA(cudaMemcpyAsync(out_counts, ctx->out_cnt_dev.p, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
+  SB_CUDA(cudaStreamSynchronize(st));
+  return SB_OK;
+}
+
+int sb_dense_values_load(sb_ctx* ctx, int slot, int32_t field, const double* vals, int64_t n) {
+  SB_REQUIRE(ctx != nullptr, SB_ERR_ARG, "sb_dense_values_load: ctx is NULL");
+  SB_REQUIRE(slot >= 0 && slot < SB_MAX_DENSE_SLOTS, SB_ERR_ARG, "sb_dense_values_load: bad slot %d", slot);
+  SB_REQUIRE(field >= 0 && field < SB_MAX_VALUE_FIELDS, SB_ERR_ARG,
+             "sb_dense_values_load: field %d out of range [0,%d)", field, SB_MAX_VALUE_FIELDS);
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  DeviceGuard g(ctx->device);
+  DenseIndex& ix = ctx->dense[slot];
+  SB_REQUIRE(ix.d > 0, SB_ERR_STATE, "sb_dense_values_load: dense slot %d has no index loaded", slot);
+  SB_REQUIRE(n == ix.n, SB_ERR_ARG, "sb_dense_values_load: %lld values for %lld rows", (long long)n, (long long)ix.n);
+  SB_REQUIRE(n == 0 || vals != nullptr, SB_ERR_ARG, "sb_dense_values_load: vals is NULL");
+  SB_CUDA(cudaStreamSynchronize(ctx->stream));
+  if (ix.vals[field]) cudaFree(ix.vals[field]);
+  ix.vals[field] = nullptr;
+  // a column spans the slot's capacity: NaN on the rows past n, so upserts and deletes never reallocate it alone
+  const int64_t cap = std::max<int64_t>(ix.n_cap, 1);
+  SB_CUDA(cudaMalloc(&ix.vals[field], (size_t)cap * 8));
+  SB_CUDA(cudaMemset(ix.vals[field], 0xff, (size_t)cap * 8));
+  if (n) SB_CUDA(cudaMemcpy(ix.vals[field], vals, (size_t)n * 8, cudaMemcpyHostToDevice));
+  return SB_OK;
+}
+
+int sb_dense_values_write(sb_ctx* ctx, int slot, int32_t field, const int64_t* rows, const double* vals, int64_t n) {
+  SB_REQUIRE(ctx != nullptr, SB_ERR_ARG, "sb_dense_values_write: ctx is NULL");
+  SB_REQUIRE(slot >= 0 && slot < SB_MAX_DENSE_SLOTS, SB_ERR_ARG, "sb_dense_values_write: bad slot %d", slot);
+  SB_REQUIRE(field >= 0 && field < SB_MAX_VALUE_FIELDS, SB_ERR_ARG,
+             "sb_dense_values_write: field %d out of range [0,%d)", field, SB_MAX_VALUE_FIELDS);
+  SB_REQUIRE(n >= 0, SB_ERR_ARG, "sb_dense_values_write: bad n=%lld", (long long)n);
+  SB_REQUIRE(n == 0 || (rows != nullptr && vals != nullptr), SB_ERR_ARG, "sb_dense_values_write: NULL buffer");
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  DeviceGuard g(ctx->device);
+  DenseIndex& ix = ctx->dense[slot];
+  SB_REQUIRE(ix.d > 0, SB_ERR_STATE, "sb_dense_values_write: dense slot %d has no index loaded", slot);
+  SB_REQUIRE(ix.vals[field] != nullptr, SB_ERR_STATE, "sb_dense_values_write: field %d has no value column loaded",
+             field);
+  std::vector<int64_t> sorted;
+  int rc = check_rows("sb_dense_values_write", rows, n, ix.n, sorted);
+  if (rc) return rc;
+  if (n == 0) return SB_OK;
+  SB_CUDA(cudaDeviceSynchronize());
+  if ((rc = ctx->misc2_dev.reserve((size_t)n * 16))) return rc;
+  int64_t* r_dev = ctx->misc2_dev.as<int64_t>();
+  double* v_dev = reinterpret_cast<double*>(r_dev + n);
+  SB_CUDA(cudaMemcpyAsync(r_dev, rows, (size_t)n * 8, cudaMemcpyHostToDevice, ctx->stream));
+  SB_CUDA(cudaMemcpyAsync(v_dev, vals, (size_t)n * 8, cudaMemcpyHostToDevice, ctx->stream));
+  dense_values_scatter_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(ix.vals[field], r_dev, v_dev, n);
+  SB_CUDA(cudaGetLastError());
+  SB_CUDA(cudaStreamSynchronize(ctx->stream));
+  return SB_OK;
+}
+
+int sb_dense_topk_where(sb_ctx* ctx, int slot, const float* q, int32_t B, int32_t k, const int32_t* p_off,
+                        const sb_pred* prog, const int32_t* pool, int32_t n_pool, int64_t* out_ids, double* out_scores,
+                        int32_t* out_counts) {
+  SB_REQUIRE(ctx != nullptr, SB_ERR_ARG, "sb_dense_topk_where: ctx is NULL");
+  SB_REQUIRE(slot >= 0 && slot < SB_MAX_DENSE_SLOTS, SB_ERR_ARG, "sb_dense_topk_where: bad slot %d", slot);
+  SB_REQUIRE(B >= 0 && k > 0, SB_ERR_ARG, "sb_dense_topk_where: bad B=%d k=%d", B, k);
+  if (B == 0) return SB_OK;
+  SB_REQUIRE(q && p_off && out_ids && out_scores && out_counts, SB_ERR_ARG, "sb_dense_topk_where: NULL buffer");
+  SB_REQUIRE(p_off[B] == 0 || prog != nullptr, SB_ERR_ARG, "sb_dense_topk_where: NULL program");
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  DeviceGuard g(ctx->device);
+  cudaStream_t st = ctx->stream;
+  DenseIndex& ix = ctx->dense[slot];
+  SB_REQUIRE(ix.d > 0, SB_ERR_STATE, "sb_dense_topk_where: dense slot %d has no index loaded", slot);
+  int rc = where_validate("sb_dense_topk_where", ix, B, p_off, prog, pool, n_pool);
+  if (rc) return rc;
+  SB_REQUIRE(k <= kDenseMaxK, SB_ERR_UNSUPPORTED, "dense: top_k %d too large (max %d per call)", k, kDenseMaxK);
+  if (ix.n == 0) {
+    for (int i = 0; i < B * k; ++i) { out_ids[i] = -1; out_scores[i] = 0.0; }
+    for (int i = 0; i < B; ++i) out_counts[i] = 0;
+    return SB_OK;
+  }
+  const size_t qbytes = (size_t)B * ix.d * sizeof(float);
+  const size_t nid = (size_t)B * k;
+  if ((rc = ctx->pin_in.reserve(qbytes))) return rc;
+  SB_CUDA(cudaStreamSynchronize(st));
+  memcpy(ctx->pin_in.p, q, qbytes);
+  float* q_pad = nullptr;
+  if ((rc = sb_dense_pad_queries(ctx, ix, ctx->pin_in.as<float>(), B, false, &q_pad, st))) return rc;
+  if ((rc = ctx->out_ids_dev.reserve(nid * 8))) return rc;
+  if ((rc = ctx->out_sc_dev.reserve(nid * 8))) return rc;
+  if ((rc = ctx->out_cnt_dev.reserve((size_t)B * 4))) return rc;
+  if ((rc = dense_topk_where_enqueue(ctx, ix, q_pad, B, k, p_off, prog, pool, ctx->out_ids_dev.as<int64_t>(),
+                                     ctx->out_sc_dev.as<double>(), ctx->out_cnt_dev.as<int32_t>(), st)))
     return rc;
   SB_CUDA(cudaMemcpyAsync(out_ids, ctx->out_ids_dev.p, nid * 8, cudaMemcpyDeviceToHost, st));
   SB_CUDA(cudaMemcpyAsync(out_scores, ctx->out_sc_dev.p, nid * 8, cudaMemcpyDeviceToHost, st));

@@ -160,6 +160,12 @@ class B200Engine:
         c = np.ascontiguousarray(codes, dtype=np.int32).reshape(-1)
         check(self._lib.sb_dense_tags_load(self._h, slot, int(field), _ptr(c), len(c)), "sb_dense_tags_load")
 
+    def load_dense_values(self, field: int, vals: np.ndarray, slot: int = 0) -> None:
+        """Numeric payload column ``field`` (< 16) of dense slot ``slot`` for range filters: one fp64 per row, NaN = the
+        row has no numeric value at the key."""
+        v = np.ascontiguousarray(vals, dtype=np.float64).reshape(-1)
+        check(self._lib.sb_dense_values_load(self._h, slot, int(field), _ptr(v), len(v)), "sb_dense_values_load")
+
     # ------------------------------------------------------------------ K1d dense mutation (upsert / delete in place)
     def dense_reserve(self, n_cap: int, slot: int = 0) -> None:
         """Grow slot ``slot``'s row capacity to at least ``n_cap`` (never shrinks), so later appends do not reallocate."""
@@ -185,6 +191,15 @@ class B200Engine:
         if len(r) != len(c):
             raise ValueError("rows and codes must have the same length")
         check(self._lib.sb_dense_tags_write(self._h, slot, int(field), _ptr(r), _ptr(c), len(r)), "sb_dense_tags_write")
+
+    def dense_values_write(self, field: int, rows, vals, slot: int = 0) -> None:
+        """``vals[i]`` -> value column ``field`` at row ``rows[i]`` (NaN = no value)."""
+        r = np.ascontiguousarray(rows, dtype=np.int64).reshape(-1)
+        v = np.ascontiguousarray(vals, dtype=np.float64).reshape(-1)
+        if len(r) != len(v):
+            raise ValueError("rows and vals must have the same length")
+        check(self._lib.sb_dense_values_write(self._h, slot, int(field), _ptr(r), _ptr(v), len(r)),
+              "sb_dense_values_write")
 
     def dense_delete(self, rows, slot: int = 0):
         """Delete rows by swap-compaction; returns the moves (moved_from, moved_to) int64 arrays: the row that held
@@ -242,6 +257,34 @@ class B200Engine:
         cnt = np.empty(B, dtype=np.int32)
         check(self._lib.sb_dense_topk_filtered(self._h, slot, _ptr(q), B, k, _ptr(off), _ptr(fld), _ptr(code), _ptr(ids),
                                                _ptr(sc), _ptr(cnt)), "sb_dense_topk_filtered")
+        return ids, sc, cnt
+
+    def dense_topk_where(self, q: np.ndarray, k: int, programs, slot: int = 0):
+        """Exact top-k of the rows on which each query's filter program holds (``sb_dense_topk_where``, DESIGN.md K1h).
+        ``programs`` = (p_off int32 [B+1], prog ``payload_filter.PRED_DTYPE`` [n], pool int32), as
+        ``PayloadIndex.compile_programs`` returns them; an empty program is unfiltered.  Returns (ids [B,k] int64,
+        scores [B,k] float64, counts [B] int32) like ``dense_topk``."""
+        from .payload_filter import PRED_DTYPE
+
+        q = np.ascontiguousarray(np.atleast_2d(q), dtype=np.float32)
+        B, d = q.shape
+        if slot not in self.dense_dim:
+            raise SentioB200Error(f"dense slot {slot} has no index loaded")
+        if d != self.dense_dim[slot]:
+            raise ValueError(f"query dimension {d} != index dimension {self.dense_dim[slot]}")
+        off, prog, pool = programs
+        off = np.ascontiguousarray(off, dtype=np.int32).reshape(-1)
+        prog = np.ascontiguousarray(prog).reshape(-1)
+        pool = np.ascontiguousarray(pool, dtype=np.int32).reshape(-1)
+        if prog.dtype != PRED_DTYPE:
+            raise ValueError("programs: prog must be a payload_filter.PRED_DTYPE array")
+        if len(off) != B + 1 or int(off[-1]) != len(prog):
+            raise ValueError("programs must be (p_off [B+1], prog [n], pool) with p_off[B] == n")
+        ids = np.empty((B, k), dtype=np.int64)
+        sc = np.empty((B, k), dtype=np.float64)
+        cnt = np.empty(B, dtype=np.int32)
+        check(self._lib.sb_dense_topk_where(self._h, slot, _ptr(q), B, k, _ptr(off), _ptr(prog), _ptr(pool), len(pool),
+                                            _ptr(ids), _ptr(sc), _ptr(cnt)), "sb_dense_topk_where")
         return ids, sc, cnt
 
     def dense_groups(self, q: np.ndarray, field: int, limit: int, group_size: int, filters=None, slot: int = 0):

@@ -20,6 +20,7 @@ from __future__ import annotations
 
 import enum
 import threading
+from types import SimpleNamespace
 from dataclasses import dataclass, field
 from typing import Any, Sequence
 
@@ -29,7 +30,7 @@ from .engine import B200Engine
 from .payload_filter import PayloadIndex
 
 __all__ = ["B200VectorStore", "ScoredPoint", "Record", "UpdateResult", "CollectionInfo", "Distance", "Datatype",
-           "PointGroup", "GroupsResult"]
+           "PointGroup", "GroupsResult", "QueryResponse"]
 
 
 @dataclass
@@ -57,6 +58,11 @@ class PointGroup:
 @dataclass
 class GroupsResult:
     groups: list = field(default_factory=list)
+
+
+@dataclass
+class QueryResponse:
+    points: list = field(default_factory=list)   # ScoredPoints, best first
 
 
 @dataclass
@@ -166,8 +172,39 @@ class _Collection:
         if self._payload_index is None:
             self._payload_index = PayloadIndex(self.payloads,
                                                lambda f, codes: self.engine.load_dense_tags(f, codes, slot=0),
-                                               lambda f, rows, codes: self.engine.dense_tags_write(f, rows, codes, slot=0))
+                                               lambda f, rows, codes: self.engine.dense_tags_write(f, rows, codes, slot=0),
+                                               lambda f, vals: self.engine.load_dense_values(f, vals, slot=0),
+                                               lambda f, rows, vals: self.engine.dense_values_write(f, rows, vals, slot=0))
         return self._payload_index
+
+
+_QUERY_KINDS = ("recommend", "discover", "context", "fusion", "order_by", "formula", "sample", "rrf")
+MAX_QUERY_DEPTH = 1024   # offset + limit of one query_points request (the engine's top-k bound)
+
+
+def _query_vector(query, where: str) -> np.ndarray:
+    """The vector of a ``query_points`` query: a plain vector or a ``NearestQuery``-shaped object (``.nearest``).  A point
+    id, the other query kinds, named or sparse vectors raise ``ValueError``."""
+    if query is None:
+        raise ValueError(f"{where}: a query vector is required")
+    for kind in _QUERY_KINDS:
+        if getattr(query, kind, None) is not None:
+            raise ValueError(f"{where}: {type(query).__name__} queries are not supported (only nearest-vector queries)")
+    if hasattr(query, "nearest"):
+        if getattr(query, "mmr", None) is not None:
+            raise ValueError(f"{where}: NearestQuery with mmr is not supported (plain nearest-vector queries only)")
+        query = query.nearest
+    if isinstance(query, (str, int)) or hasattr(query, "hex"):
+        raise ValueError(f"{where}: a point id as the query is not supported (give the vector)")
+    if isinstance(query, dict) or hasattr(query, "indices"):
+        raise ValueError(f"{where}: named, sparse and multi-vector queries are not supported (one dense vector)")
+    try:
+        q = np.asarray(query, dtype=np.float32)
+    except (TypeError, ValueError) as e:
+        raise ValueError(f"{where}: the query must be a numeric vector ({e})") from None
+    if q.ndim != 1:
+        raise ValueError(f"{where}: the query must be one vector, got shape {q.shape}")
+    return q
 
 
 def _points_columns(points):
@@ -472,6 +509,81 @@ class B200VectorStore:
         """CSR conditions for the engine, or None when no query has a condition (the unfiltered search)."""
         off, fld, code = col.payload_index().compile(filters)
         return (off, fld, code) if len(fld) else None
+
+    def query_points(self, collection_name: str, query, query_filter=None, limit: int = 10, offset: int | None = None,
+                     score_threshold: float | None = None, with_payload: bool = True, with_vectors: bool = False,
+                     using=None, search_params=None, prefetch=None, lookup_from=None, **_ignored) -> QueryResponse:
+        """Qdrant ``query_points`` with a nearest-vector query: the exact best points after skipping ``offset``, at most
+        ``limit`` of them, over the points matching ``query_filter``.  The filter may use must / should / must_not /
+        min_should, nested filters, MatchValue, MatchAny and Range (INTEGRATION.md has the semantics and the refusals).
+        ``score_threshold`` keeps scores >= it (Cosine, Dot) or distances <= it (Euclid).  ``with_vectors`` returns
+        what ``retrieve`` returns.  ``search_params`` tunes approximate search and is accepted: every search here is
+        exact.  A point-id query, other query kinds, ``prefetch``, ``lookup_from``, ``using`` and offset + limit > 1024
+        raise ``ValueError``."""
+        req = SimpleNamespace(query=query, filter=query_filter, limit=limit, offset=offset,
+                              score_threshold=score_threshold, with_payload=with_payload, with_vector=with_vectors,
+                              using=using, prefetch=prefetch, lookup_from=lookup_from)
+        return self._query(collection_name, [req], "query_points")[0]
+
+    def query_batch_points(self, collection_name: str, requests: Sequence) -> list[QueryResponse]:
+        """Qdrant ``query_batch_points``: one ``query_points`` per request (``.query``, ``.filter``, ``.limit``, ``.offset``,
+        ``.score_threshold``, ``.with_payload``, ``.with_vector``), answered in ONE device batch of depth max(offset +
+        limit).  Each answer is a cut of its query's exact order, so it equals the request run alone."""
+        return self._query(collection_name, list(requests), "query_batch_points")
+
+    def _query(self, collection_name: str, reqs: list, where: str) -> list[QueryResponse]:
+        col = self._get(collection_name)
+        if not reqs:
+            return []
+        qs, cuts = [], []
+        for r in reqs:
+            for attr in ("prefetch", "lookup_from", "using"):
+                if getattr(r, attr, None) is not None:
+                    raise ValueError(f"{where}: {attr} is not supported")
+            qs.append(_query_vector(getattr(r, "query", None), where))
+            limit = getattr(r, "limit", None)
+            limit = 10 if limit is None else limit
+            offset = getattr(r, "offset", None) or 0
+            if not all(isinstance(v, int) and not isinstance(v, bool) for v in (limit, offset)) or limit < 1 \
+                    or offset < 0:
+                raise ValueError(f"{where}: limit must be an int >= 1 and offset an int >= 0")
+            if offset + limit > MAX_QUERY_DEPTH:
+                raise ValueError(f"{where}: offset + limit = {offset + limit} exceeds {MAX_QUERY_DEPTH}")
+            # Qdrant's QueryRequest leaves both flags None by default, which it reads as False
+            flags = [getattr(r, "with_payload", True), getattr(r, "with_vector", getattr(r, "with_vectors", False))]
+            flags = [False if f is None else f for f in flags]
+            if not all(isinstance(f, bool) for f in flags):
+                raise ValueError(f"{where}: with_payload / with_vector must be True or False (selectors are not "
+                                 "supported)")
+            t = getattr(r, "score_threshold", None)
+            if t is not None and (isinstance(t, bool) or not isinstance(t, (int, float))):
+                raise ValueError(f"{where}: score_threshold must be a number")
+            cuts.append((offset, limit, t, *flags))
+        if len({len(q) for q in qs}) != 1 or len(qs[0]) != col.dim:
+            raise ValueError(f"{where}: query vectors must have dimension {col.dim}")
+        q = np.stack(qs)
+        filters = [getattr(r, "filter", None) for r in reqs]
+        with col.lock:
+            k = max(1, min(max(o + lim for o, lim, *_ in cuts), max(len(col.ids), 1)))
+            if any(f is not None for f in filters):
+                programs = col.payload_index().compile_programs(filters)
+                ids, scores, counts = col.engine.dense_topk_where(q, k, programs)
+            else:
+                ids, scores, counts = col.engine.dense_topk(q, k)
+            euclid = col.distance is Distance.EUCLID
+            out = []
+            for b, (offset, limit, t, wp, wv) in enumerate(cuts):
+                rows = [int(r) for r in ids[b, offset:min(int(counts[b]), offset + limit)]]
+                sc = [float(x) for x in scores[b, offset:offset + len(rows)]]
+                if t is not None:   # the order is best first, so the points kept are a prefix
+                    keep = sum(1 for x in sc if (x <= t if euclid else x >= t))
+                    rows, sc = rows[:keep], sc[:keep]
+                vecs = col.engine.dense_fetch(rows, slot=0) if wv and rows else None
+                out.append(QueryResponse(points=[
+                    ScoredPoint(id=col.ids[r], score=s_, payload=col.payloads[r] if wp else None,
+                                vector=vecs[j].tolist() if vecs is not None else None)
+                    for j, (r, s_) in enumerate(zip(rows, sc))]))
+            return out
 
     def search_batch_arrays(self, collection_name: str, query_vectors: np.ndarray, limit: int):
         """Batched extension: (rows [B,k] int64, scores [B,k] float64, counts [B]) without Python objects."""
