@@ -37,9 +37,10 @@ typedef struct sb_ctx sb_ctx;
 #define SB_ERR_STATE (-3)
 #define SB_ERR_UNSUPPORTED (-4)
 
-/* dtypes accepted by sb_dense_load */
+/* dtypes accepted by sb_dense_load (SB_U8: uint8 slots only, SB_STORAGE_U8 below) */
 #define SB_F32 0
 #define SB_F16 1
+#define SB_U8 2
 
 /* BM25 variants (rank_bm25 0.2.2 class names; reference src/core/retrievers/sparse.py:91-97) */
 #define SB_BM25_OKAPI 0
@@ -127,11 +128,21 @@ int32_t sb_dense_metric(sb_ctx* ctx, int slot);
  * sb_dense_fetch returns x bit for bit (Cosine: fl32(x / ||x||), Qdrant's normalised vector); upsert, delete, reserve,
  * tags, filtered and grouped search follow the slot's storage.  A float32 slot rejects rows with a non-finite fp64 norm
  * (every metric).
+ * SB_STORAGE_U8 (Qdrant's Datatype.UINT8) keeps only the caller's rows x, one byte per dimension (rows padded with zeros
+ * to a multiple of 64 bytes), and no fp16 rows: 1 byte per dimension per row in HBM.  Every component must be an integer
+ * in [0, 255]: SB_U8 input is taken as is; SB_F32 / SB_F16 input must hold integral values in that range, and any other
+ * value (fractional, negative, above 255, NaN, inf) is rejected with SB_ERR_ARG before the slot changes.  Scores are the
+ * float32 formulas above, exact fp64 on the integer x and the caller's fp32 query.  Unlike a float32 slot,
+ * sb_dense_fetch returns x itself (as fp32) for every metric, Cosine included: a normalised uint8 vector does not exist.
+ * Every query on a uint8 slot takes the wgmma batched scan (DESIGN.md K1i), whatever the batch size, row count or
+ * sb_dense_set_mode: mode 1 does not apply to uint8 slots.  Upsert, delete, reserve, tags, filtered and grouped search,
+ * the _dev entry points and the scorers with a vector source follow the slot's storage.
  * sb_dense_load_storage: sb_dense_load_metric with a storage datatype; sb_dense_load / sb_dense_load_metric mean
- * SB_STORAGE_F16.  sb_dense_storage: the slot's storage, -1 for a bad slot.
+ * SB_STORAGE_F16.  SB_U8 input is accepted by uint8 slots only.  sb_dense_storage: the slot's storage, -1 for a bad slot.
  */
 #define SB_STORAGE_F16 0
 #define SB_STORAGE_F32 1
+#define SB_STORAGE_U8 2
 int sb_dense_load_storage(sb_ctx* ctx, int slot, const void* vecs, int64_t n, int32_t d, int32_t dtype, int64_t id_base,
                           int32_t metric, int32_t storage);
 int32_t sb_dense_storage(sb_ctx* ctx, int slot);
@@ -274,7 +285,8 @@ int sb_dense_group_rounds(sb_ctx* ctx, int64_t* hist, int32_t n);
  *
  * sb_dense_reserve: grow the slot's capacity to at least n_cap rows (never shrinks).  Without it, an upsert that
  * outgrows the capacity reallocates to max(needed, 1.5 x capacity) rows, with old and new buffers alive during the copy.
- * sb_dense_upsert: stores vecs[i] (n rows of sb_dense_dim values, dtype as sb_dense_load, same conversion) at row
+ * sb_dense_upsert: stores vecs[i] (n rows of sb_dense_dim values, dtype as sb_dense_load, same conversion and the same
+ * uint8 rules: SB_U8 on uint8 slots only, SB_ERR_ARG elsewhere) at row
  * rows[i].  rows[i] < count overwrites; rows >= count must be exactly count .. count+m-1 (any order); no row twice; the
  * count stays under 2^31.  Every loaded tag column is set to -1 on the written rows (sb_dense_tags_write sets codes).
  * sb_dense_tags_write: codes[i] (>= -1) -> tag column `field` (loaded) at rows[i] (distinct, < count).

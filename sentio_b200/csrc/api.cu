@@ -68,6 +68,7 @@ void sb_destroy(sb_ctx* ctx) {
     if (ctx->dense[s].cfac) cudaFree(ctx->dense[s].cfac);
     if (ctx->dense[s].hh) cudaFree(ctx->dense[s].hh);
     if (ctx->dense[s].rows32) cudaFree(ctx->dense[s].rows32);
+    if (ctx->dense[s].rows8) cudaFree(ctx->dense[s].rows8);
     for (int f = 0; f < SB_MAX_TAG_FIELDS; ++f)
       if (ctx->dense[s].tags[f]) cudaFree(ctx->dense[s].tags[f]);
     for (int f = 0; f < SB_MAX_VALUE_FIELDS; ++f)

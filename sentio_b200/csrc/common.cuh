@@ -108,8 +108,12 @@ struct DenseIndex {
   int32_t storage = SB_STORAGE_F16;
   float* rows32 = nullptr;   // [n_cap][d_pad] fp32, zero padded; nullptr for float16 storage
   double sigma_max = 0.0;
-  // cached CUtensorMap (128 bytes, 64-byte aligned) over rows[0, n_pad) for the wgmma batched scan; valid iff
-  // tm_rows_ptr == rows and tm_n_pad == n_pad (an append within capacity keeps `rows` but widens n_pad)
+  // uint8 storage (DESIGN.md K1i): the caller's integer rows x, one byte per dimension, INSTEAD of `rows` (which stays
+  // nullptr); d_pad = round_up(d, 64).  inv_norm is the scan scale (Cosine fl32(1/||x||), Dot / Euclid 1), hh = ||x||^2 / 2
+  // rounded up (Euclid), cfac is not allocated and sigma_max stays 0: the scan reads the vector it scores.
+  uint8_t* rows8 = nullptr;  // [n_cap][d_pad]
+  // cached CUtensorMap (128 bytes, 64-byte aligned) over rows[0, n_pad) (uint8: rows8) for the wgmma batched scan;
+  // valid iff tm_rows_ptr == rows (rows8) and tm_n_pad == n_pad (an append within capacity keeps `rows` but widens n_pad)
   alignas(64) unsigned char tm_rows[128] = {0};
   const void* tm_rows_ptr = nullptr;
   int64_t tm_n_pad = 0;

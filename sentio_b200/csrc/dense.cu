@@ -127,6 +127,34 @@ __global__ void dense_store_rows32_kernel(const TIn* __restrict__ in, int64_t n_
   atomicMax(sigma_bits, (unsigned long long)__double_as_longlong(sig));
 }
 
+// Uint8 storage (DESIGN.md K1i): one warp per row writes rows8 = x (zero padded to d_pad bytes), the scan scale inv_norm
+// (Cosine fl32(1/||x||), 0 for a zero row; Dot / Euclid 1: the scan reads x itself), for Euclid hh = ||x||^2 / 2 rounded
+// up to fp32, and folds the row's ||x||^2 (an integer below 2^28) into *xx_max.  The host has checked that every input
+// value is an integer in [0, 255].
+template <typename TIn>
+__global__ void dense_store_rows8_kernel(const TIn* __restrict__ in, int64_t n_rows, int32_t d, int32_t d_pad,
+                                         uint8_t* __restrict__ rows8, float* __restrict__ inv_norm, int64_t row0,
+                                         const int64_t* __restrict__ dst_rows, bool cosine, float* __restrict__ hh,
+                                         unsigned long long* __restrict__ xx_max) {
+  const int64_t r = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (r >= n_rows) return;
+  const int64_t out_row = dst_rows ? dst_rows[r] : row0 + r;
+  const TIn* src = in + r * (int64_t)d;
+  uint8_t* dst = rows8 + out_row * (int64_t)d_pad;
+  uint32_t ss = 0;
+  for (int i = lane; i < d_pad; i += 32) {
+    const uint32_t v = i < d ? (uint32_t)(float)src[i] : 0u;
+    dst[i] = (uint8_t)v;
+    ss += v * v;
+  }
+  for (int o = 16; o; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
+  if (lane != 0) return;
+  inv_norm[out_row] = cosine ? (ss ? (float)(1.0 / sqrt((double)ss)) : 0.f) : 1.f;
+  if (hh) hh[out_row] = __double2float_ru(0.5 * (double)ss);
+  atomicMax(xx_max, (unsigned long long)ss);
+}
+
 // ------------------------------------------------------------------------------------------------ mutation kernels
 // sb_dense_delete's compaction: one warp per move from[m] -> to[m] (sources >= n - |D| > destinations, so one launch
 // has no read/write hazard): the fp16 row in 16-byte copies, its inverse norm, its code in every loaded tag column and
@@ -137,6 +165,7 @@ struct MoveParams {
   double* cfac;                       // Dot / Euclid, else nullptr
   float* hh;                          // Euclid, else nullptr
   float* rows32;                      // float32 storage, else nullptr
+  uint8_t* rows8;                     // uint8 storage (then rows is nullptr), else nullptr
   int32_t* tags[SB_MAX_TAG_FIELDS];   // nullptr = field not loaded
   double* vals[SB_MAX_VALUE_FIELDS];  // likewise
   const int64_t* from;
@@ -150,9 +179,16 @@ __global__ void __launch_bounds__(256) dense_move_rows_kernel(const MoveParams p
   const int lane = threadIdx.x & 31;
   if (m >= p.n_moves) return;
   const int64_t s = p.from[m], t = p.to[m];
-  const uint4* src = reinterpret_cast<const uint4*>(p.rows) + s * p.ch;
-  uint4* dst = reinterpret_cast<uint4*>(p.rows) + t * p.ch;
-  for (int c = lane; c < p.ch; c += 32) dst[c] = src[c];
+  if (p.rows) {
+    const uint4* src = reinterpret_cast<const uint4*>(p.rows) + s * p.ch;
+    uint4* dst = reinterpret_cast<uint4*>(p.rows) + t * p.ch;
+    for (int c = lane; c < p.ch; c += 32) dst[c] = src[c];
+  }
+  if (p.rows8) {   // the uint8 row: d_pad / 16 = ch / 2 16-byte chunks
+    const uint4* src8 = reinterpret_cast<const uint4*>(p.rows8) + s * (p.ch / 2);
+    uint4* dst8 = reinterpret_cast<uint4*>(p.rows8) + t * (p.ch / 2);
+    for (int c = lane; c < p.ch / 2; c += 32) dst8[c] = src8[c];
+  }
   if (p.rows32) {   // the fp32 row: 2 * ch 16-byte chunks
     const uint4* src32 = reinterpret_cast<const uint4*>(p.rows32) + s * 2 * p.ch;
     uint4* dst32 = reinterpret_cast<uint4*>(p.rows32) + t * 2 * p.ch;
@@ -706,7 +742,8 @@ __global__ void __launch_bounds__(kMergeThreads, 1) dense_merge_kernel(const Mer
   ra.metric = p.metric;
   ra.cfac = p.cfac;
   ra.rows32 = p.rows32;
-  rescore_and_emit<F32>(sel, nsel, P, ek, ei, &qq_s, q_s, ra);
+  ra.rows8 = nullptr;
+  rescore_and_emit<F32 ? SB_STORAGE_F32 : SB_STORAGE_F16>(sel, nsel, P, ek, ei, &qq_s, q_s, ra);
 }
 
 // ------------------------------------------------------------------------------------------------ query preparation
@@ -718,6 +755,9 @@ __global__ void __launch_bounds__(kMergeThreads, 1) dense_merge_kernel(const Mer
 // could leave the fp32 range, or whose exact fp64 distances cannot resolve the window, gets its fallback flag fb[r].
 // Float32 storage (DESIGN.md K1g) adds sigma (>= ||y^ - x^|| resp. ||v - x|| over the slot's rows): the key of x differs
 // from the key of v by at most sigma (Cosine, Dot) or (r + rho) sigma (Euclid); sigma = 0 for float16 storage.
+// Uint8 storage (DESIGN.md K1i): the scan reads x itself, so sigma = 0 and rho, hmax bound ||x|| and ||x||^2 / 2.  q16 is
+// written with its columns permuted inside every 64-column block (u8_query_column), so that the 16 bytes a scan thread
+// reads from a corpus row are its wgmma A fragments for the block's four k16 steps.
 struct PrepMetric {
   int32_t metric;
   double rho, hmax, sigma;
@@ -725,7 +765,7 @@ struct PrepMetric {
   int32_t* fb;    // [rows]
 };
 
-template <bool F32>
+template <int ST>
 __global__ void __launch_bounds__(256) dense_prep_queries_kernel(const float* __restrict__ q_pad, int nq, int d_pad,
                                                                  float* __restrict__ qn, __half* __restrict__ q16,
                                                                  float* __restrict__ eps, int mma, const PrepMetric pm) {
@@ -758,7 +798,8 @@ __global__ void __launch_bounds__(256) dense_prep_queries_kernel(const float* __
     if (qn) qn[(size_t)r * d_pad + i] = v;
     if (q16) {
       const __half h = __float2half_rn(v);
-      q16[(size_t)r * d_pad + i] = h;
+      if constexpr (ST == SB_STORAGE_U8) q16[(size_t)r * d_pad + (i & ~63) + u8_query_column(i & 63)] = h;
+      else q16[(size_t)r * d_pad + i] = h;
       const double e = (double)__half2float(h) - (double)v;
       dd += e * e;
     }
@@ -774,14 +815,14 @@ __global__ void __launch_bounds__(256) dense_prep_queries_kernel(const float* __
     float e = 0.f;
     if (!zero) e = mma ? (float)(sqrt(t) * 1.0001) + dense_eps_mma_acc(d_pad) : dense_eps_fp32(d_pad);
     // float32 storage (DESIGN.md K1g): + sigma (Cosine, Dot), + (r + rho) sigma (Euclid), the first through r * ed
-    if constexpr (F32)
+    if constexpr (ST == SB_STORAGE_F32)
       if (pm.metric == SB_METRIC_COSINE && !zero) e = __double2float_ru((double)e + pm.sigma);
     if (pm.metric != SB_METRIC_COSINE) {
       // Dot: |acc * (float)c - <qn, v>| <= c (e + 2^-22) with c <= rho (1 + 2^-10); the zero query keeps eps 0 (every key
       // is exactly 0).  Euclid: key = r * (acc * s) - h; r * eps_dot + r rho 2^-22 (r and its product) + hmax 2^-22 (h
       // rounded up) + (r rho + hmax) 2^-24 (the subtraction), all inside (r rho + hmax) 2^-20.
       double ed = ((double)e + 0x1p-20) * pm.rho * 1.001;
-      if constexpr (F32) ed += pm.sigma;
+      if constexpr (ST == SB_STORAGE_F32) ed += pm.sigma;
       const bool fits = pm.rho <= 1e36;
       if (pm.metric == SB_METRIC_DOT) {
         e = zero ? 0.f : __double2float_ru(ed);
@@ -789,7 +830,7 @@ __global__ void __launch_bounds__(256) dense_prep_queries_kernel(const float* __
       } else {
         const double rr = zero ? 0.0 : (double)(float)nrm;
         double ee = (rr * ed + (rr * pm.rho + pm.hmax) * 0x1p-20) * 1.001;
-        if constexpr (F32) ee += pm.rho * pm.sigma * 1.001;   // | ||v||^2 - ||x||^2 | / 2 <= (rho + sigma / 2) sigma
+        if constexpr (ST == SB_STORAGE_F32) ee += pm.rho * pm.sigma * 1.001;   // | ||v||^2 - ||x||^2 | / 2 <= (rho + sigma / 2) sigma
         e = __double2float_ru(ee);
         // the fp64 exact stage resolves ||q - v||^2 to (r + rho)^2 2^-41 (d <= 4096 terms); it must stay far below eps
         const double res = (rr + pm.rho) * (rr + pm.rho) * 0x1p-41;
@@ -823,10 +864,11 @@ struct FallbackParams {
   int32_t mask_qs;
   int32_t metric;
   const double* cfac;
-  const float* rows32;           // F32 only
+  const float* rows32;           // float32 storage only
+  const uint8_t* rows8;          // uint8 storage only
 };
 
-template <bool FILTER, bool F32>
+template <bool FILTER, int ST>
 __global__ void __launch_bounds__(kFbThreads, 1) dense_exact_fallback_kernel(const FallbackParams p) {
   const int qi = blockIdx.x;
   if (p.flag[qi] == 0) return;
@@ -898,7 +940,7 @@ __global__ void __launch_bounds__(kFbThreads, 1) dense_exact_fallback_kernel(con
         if (row < p.n) match = (p.mask[(size_t)(row >> 5) * p.mask_qs + qi] >> (row & 31)) & 1u;
       if (row < p.n && match) {
         okey = f64_orderable(
-            exact_key_row<F32>(p.metric, p.rows, p.cfac, p.rows32, (uint32_t)row, q, p.d_pad, p.ch, qn, lane));
+            exact_key_row<ST>(p.metric, p.rows, p.cfac, p.rows32, p.rows8, (uint32_t)row, q, p.d_pad, p.ch, qn, lane));
         if (okey == 0ull) okey = 1ull;
       }
       if (lane == 0) {
@@ -1079,10 +1121,11 @@ struct GatherParams {
   int32_t* out_counts;
   int32_t metric;
   const double* cfac;
-  const float* rows32;       // F32 only
+  const float* rows32;       // float32 storage only
+  const uint8_t* rows8;      // uint8 storage only
 };
 
-template <bool F32>
+template <int ST>
 __global__ void __launch_bounds__(kMergeThreads, 1) dense_filter_gather_kernel(const GatherParams p) {
   extern __shared__ __align__(16) uint8_t gsmem[];
   unsigned long long* sel = reinterpret_cast<unsigned long long*>(gsmem);   // [kGatherMax] (key score field unused)
@@ -1118,7 +1161,8 @@ __global__ void __launch_bounds__(kMergeThreads, 1) dense_filter_gather_kernel(c
   ra.metric = p.metric;
   ra.cfac = p.cfac;
   ra.rows32 = p.rows32;
-  rescore_and_emit<F32>(sel, nsel, P, ek, ei, &qq_s, q_s, ra);
+  ra.rows8 = p.rows8;
+  rescore_and_emit<ST>(sel, nsel, P, ek, ei, &qq_s, q_s, ra);
 }
 
 // ------------------------------------------------------------------------------------------------ grouped search (K1f)
@@ -1370,8 +1414,9 @@ int dense_topk_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int B, i
   ScanPlan pl;
   int rc = make_plan(ctx, ix, k, &pl);
   if (rc) return rc;
-  // batches of >= 16 queries ride the tensor cores: one HBM pass per 64 / 128 queries instead of one per 4
-  if (ctx->dense_mode != 1 && dense_mma_eligible(ctx, ix, B))
+  // batches of >= 16 queries ride the tensor cores: one HBM pass per 64 / 128 queries instead of one per 4.  A uint8 slot
+  // has no fp16 rows for the CUDA-core scan: every batch takes the wgmma scan (DESIGN.md K1i)
+  if (ix.storage == SB_STORAGE_U8 || (ctx->dense_mode != 1 && dense_mma_eligible(ctx, ix, B)))
     return dense_mma_topk_enqueue(ctx, ix, q_pad, B, k, out_ids, out_scores, out_counts, st, flt);
   const int chunk = B < kMergeChunk ? B : kMergeChunk;
   const size_t per_q = (size_t)pl.grid * pl.kprime;
@@ -1507,6 +1552,16 @@ __global__ void __launch_bounds__(128) dense_fetch_f32_kernel(const float* rows3
   }
 }
 
+// uint8 storage: x as fp32 for every metric (a normalised uint8 vector does not exist)
+__global__ void __launch_bounds__(128) dense_fetch_u8_kernel(const uint8_t* rows8, int d, int d_pad, int64_t n,
+                                                             int64_t id_base, const int64_t* ids, int n_ids, float* out) {
+  const int r = blockIdx.x;
+  if (r >= n_ids) return;
+  const int64_t idx = ids[r] - id_base;
+  const bool live = idx >= 0 && idx < n;
+  for (int i = threadIdx.x; i < d; i += blockDim.x) out[(size_t)r * d + i] = live ? (float)rows8[(size_t)idx * d_pad + i] : 0.f;
+}
+
 }  // namespace
 
 // Shared with dense_mma.cu: query preparation (normalised fp32 copy, optional fp16 operand rows, eps, cleared fallback
@@ -1533,8 +1588,12 @@ int dense_prep_queries(sb_ctx* ctx, const DenseIndex& ix, const float* q_pad, in
   }
   SB_CUDA(cudaMemsetAsync(fb, 0, (size_t)rows * 4, st));
   ctx->launches += 1;
-  if (ix.rows32) dense_prep_queries_kernel<true><<<rows, 256, 0, st>>>(q_pad, B, ix.d_pad, qn, q16, eps, mma ? 1 : 0, pm);
-  else dense_prep_queries_kernel<false><<<rows, 256, 0, st>>>(q_pad, B, ix.d_pad, qn, q16, eps, mma ? 1 : 0, pm);
+  if (ix.storage == SB_STORAGE_U8)
+    dense_prep_queries_kernel<SB_STORAGE_U8><<<rows, 256, 0, st>>>(q_pad, B, ix.d_pad, qn, q16, eps, mma ? 1 : 0, pm);
+  else if (ix.rows32)
+    dense_prep_queries_kernel<SB_STORAGE_F32><<<rows, 256, 0, st>>>(q_pad, B, ix.d_pad, qn, q16, eps, mma ? 1 : 0, pm);
+  else
+    dense_prep_queries_kernel<SB_STORAGE_F16><<<rows, 256, 0, st>>>(q_pad, B, ix.d_pad, qn, q16, eps, mma ? 1 : 0, pm);
   SB_CUDA(cudaGetLastError());
   *eps_out = eps;
   *fb_out = fb;
@@ -1567,10 +1626,13 @@ int dense_fallback_enqueue(sb_ctx* ctx, const DenseIndex& ix, const float* q_pad
   fp.metric = ix.metric;
   fp.cfac = ix.cfac;
   fp.rows32 = ix.rows32;
+  fp.rows8 = ix.rows8;
   ctx->launches += 1;
-  const bool f32 = ix.rows32 != nullptr;
-  auto kern = flt ? (f32 ? dense_exact_fallback_kernel<true, true> : dense_exact_fallback_kernel<true, false>)
-                  : (f32 ? dense_exact_fallback_kernel<false, true> : dense_exact_fallback_kernel<false, false>);
+  auto kern = flt ? dense_exact_fallback_kernel<true, SB_STORAGE_F16> : dense_exact_fallback_kernel<false, SB_STORAGE_F16>;
+  if (ix.storage == SB_STORAGE_F32)
+    kern = flt ? dense_exact_fallback_kernel<true, SB_STORAGE_F32> : dense_exact_fallback_kernel<false, SB_STORAGE_F32>;
+  else if (ix.storage == SB_STORAGE_U8)
+    kern = flt ? dense_exact_fallback_kernel<true, SB_STORAGE_U8> : dense_exact_fallback_kernel<false, SB_STORAGE_U8>;
   kern<<<B, kFbThreads, 0, st>>>(fp);
   SB_CUDA(cudaGetLastError());
   return SB_OK;
@@ -1783,7 +1845,9 @@ int dense_topk_where_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, in
              smem_max);
   SB_CUDA(cudaFuncSetAttribute(dense_where_mask_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max));
   const size_t gather_smem = (size_t)kGatherMax * 20 + (size_t)ix.d_pad * 4 + 64;
-  auto gather_kern = ix.rows32 ? dense_filter_gather_kernel<true> : dense_filter_gather_kernel<false>;
+  auto gather_kern = ix.storage == SB_STORAGE_U8    ? dense_filter_gather_kernel<SB_STORAGE_U8>
+                     : ix.storage == SB_STORAGE_F32 ? dense_filter_gather_kernel<SB_STORAGE_F32>
+                                                    : dense_filter_gather_kernel<SB_STORAGE_F16>;
   SB_CUDA(cudaFuncSetAttribute(gather_kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gather_smem));
   for (int c0 = 0; c0 < B; c0 += qchunk) {
     const int nq = std::min(qchunk, B - c0);
@@ -1854,6 +1918,7 @@ int dense_topk_where_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, in
       gp.metric = ix.metric;
       gp.cfac = ix.cfac;
       gp.rows32 = ix.rows32;
+      gp.rows8 = ix.rows8;
       ProfScope ps(ctx, SB_PROF_DENSE_GATHER, st);
       gather_kern<<<n_gather, kMergeThreads, gather_smem, st>>>(gp);
     }
@@ -2118,17 +2183,19 @@ int64_t round_rows(int64_t n) { return (n + kRowPad - 1) / kRowPad * kRowPad; }
 
 // The one store-rows path of sb_dense_load and sb_dense_upsert: n host rows (SB_F32 / SB_F16) through a device staging
 // buffer in chunks, converted by dense_store_rows_kernel into rows row0 + i, or dst_dev[i] (a device list) when given.
-// A float32 slot also gets rows32 from dense_store_rows32_kernel, and *sigma the largest sigma of the stored rows.
-// Returns after the last chunk has been stored.
+// A float32 slot also gets rows32 from dense_store_rows32_kernel, and *sigma the largest sigma of the stored rows.  A
+// uint8 slot is written by dense_store_rows8_kernel alone (SB_U8 / SB_F32 / SB_F16 input, checked by check_u8_rows), and
+// *sigma receives the largest ||x||^2 of the stored rows instead.  Returns after the last chunk has been stored.
 int dense_store_staged(sb_ctx* ctx, DenseIndex& ix, const void* vecs, int64_t n, int32_t dtype, const int64_t* dst_dev,
                        int64_t row0, double* sigma) {
   const int d = ix.d;
-  const size_t esz = dtype == SB_F32 ? 4 : 2;
+  const size_t esz = dtype == SB_F32 ? 4 : dtype == SB_U8 ? 1 : 2;
+  const bool u8 = ix.storage == SB_STORAGE_U8;
   const int64_t chunk_rows = std::max<int64_t>(1, (int64_t)((256ull << 20) / ((size_t)d * esz)));
   int rc = ctx->misc_dev.reserve((size_t)std::min<int64_t>(chunk_rows, n) * d * esz);
   if (rc) return rc;
   unsigned long long* sigma_bits = nullptr;
-  if (ix.rows32) {
+  if (ix.rows32 || u8) {
     if ((rc = ctx->sigma_dev.reserve(8))) return rc;
     sigma_bits = ctx->sigma_dev.as<unsigned long long>();
     SB_CUDA(cudaMemsetAsync(sigma_bits, 0, 8, ctx->stream));
@@ -2140,7 +2207,18 @@ int dense_store_staged(sb_ctx* ctx, DenseIndex& ix, const void* vecs, int64_t n,
     const int wpb = 8;
     const unsigned blocks = (unsigned)((nr + wpb - 1) / wpb);
     const int64_t* dst = dst_dev ? dst_dev + r0 : nullptr;
-    if (dtype == SB_F32)
+    if (u8) {
+      const bool cos = ix.metric == SB_METRIC_COSINE;
+      if (dtype == SB_U8)
+        dense_store_rows8_kernel<uint8_t><<<blocks, wpb * 32, 0, ctx->stream>>>(
+            ctx->misc_dev.as<uint8_t>(), nr, d, ix.d_pad, ix.rows8, ix.inv_norm, row0 + r0, dst, cos, ix.hh, sigma_bits);
+      else if (dtype == SB_F32)
+        dense_store_rows8_kernel<float><<<blocks, wpb * 32, 0, ctx->stream>>>(
+            ctx->misc_dev.as<float>(), nr, d, ix.d_pad, ix.rows8, ix.inv_norm, row0 + r0, dst, cos, ix.hh, sigma_bits);
+      else
+        dense_store_rows8_kernel<__half><<<blocks, wpb * 32, 0, ctx->stream>>>(
+            ctx->misc_dev.as<__half>(), nr, d, ix.d_pad, ix.rows8, ix.inv_norm, row0 + r0, dst, cos, ix.hh, sigma_bits);
+    } else if (dtype == SB_F32)
       dense_store_rows_kernel<float><<<blocks, wpb * 32, 0, ctx->stream>>>(ctx->misc_dev.as<float>(), nr, d, ix.d_pad,
                                                                            ix.rows, ix.inv_norm, row0 + r0, dst, true,
                                                                            ix.cfac, ix.hh);
@@ -2164,7 +2242,8 @@ int dense_store_staged(sb_ctx* ctx, DenseIndex& ix, const void* vecs, int64_t n,
   if (sigma_bits) {
     unsigned long long bits = 0;
     SB_CUDA(cudaMemcpy(&bits, sigma_bits, 8, cudaMemcpyDeviceToHost));
-    memcpy(sigma, &bits, 8);
+    if (u8) *sigma = (double)bits;   // an integer ||x||^2, not fp64 bits
+    else memcpy(sigma, &bits, 8);
   }
   return SB_OK;
 }
@@ -2172,8 +2251,10 @@ int dense_store_staged(sb_ctx* ctx, DenseIndex& ix, const void* vecs, int64_t n,
 // Reallocate rows / inv_norm / cfac / hh / every loaded tag and value column to n_cap rows (> ix.n_cap): the [0, n_pad)
 // prefix is copied device to device, the rest is zero (tags -1, values NaN).  Old and new buffers coexist during the copy.
 int dense_grow(sb_ctx* ctx, DenseIndex& ix, int64_t n_cap) {
-  const size_t rb = (size_t)ix.d_pad * sizeof(__half);
+  const bool u8 = ix.storage == SB_STORAGE_U8;   // rows8 instead of rows
+  const size_t rb = (size_t)ix.d_pad * (u8 ? 1 : sizeof(__half));
   __half* rows = nullptr;
+  uint8_t* rows8 = nullptr;
   float* inv = nullptr;
   double* cfac = nullptr;
   float* hh = nullptr;
@@ -2181,9 +2262,9 @@ int dense_grow(sb_ctx* ctx, DenseIndex& ix, int64_t n_cap) {
   const size_t rb32 = (size_t)ix.d_pad * sizeof(float);
   int32_t* tags[SB_MAX_TAG_FIELDS] = {};
   double* vals[SB_MAX_VALUE_FIELDS] = {};
-  cudaError_t e = cudaMalloc(&rows, (size_t)n_cap * rb);
+  cudaError_t e = u8 ? cudaMalloc(&rows8, (size_t)n_cap * rb) : cudaMalloc(&rows, (size_t)n_cap * rb);
   if (e == cudaSuccess) e = cudaMalloc(&inv, (size_t)n_cap * sizeof(float));
-  if (e == cudaSuccess && ix.metric != SB_METRIC_COSINE) e = cudaMalloc(&cfac, (size_t)n_cap * sizeof(double));
+  if (e == cudaSuccess && ix.metric != SB_METRIC_COSINE && !u8) e = cudaMalloc(&cfac, (size_t)n_cap * sizeof(double));
   if (e == cudaSuccess && ix.metric == SB_METRIC_EUCLID) e = cudaMalloc(&hh, (size_t)n_cap * sizeof(float));
   if (e == cudaSuccess && ix.storage == SB_STORAGE_F32) e = cudaMalloc(&rows32, (size_t)n_cap * rb32);
   for (int f = 0; f < SB_MAX_TAG_FIELDS && e == cudaSuccess; ++f)
@@ -2192,10 +2273,12 @@ int dense_grow(sb_ctx* ctx, DenseIndex& ix, int64_t n_cap) {
     if (ix.vals[f]) e = cudaMalloc(&vals[f], (size_t)n_cap * 8);
   const int64_t keep = ix.n_pad;
   cudaStream_t st = ctx->stream;
-  if (e == cudaSuccess && keep) e = cudaMemcpyAsync(rows, ix.rows, (size_t)keep * rb, cudaMemcpyDeviceToDevice, st);
+  uint8_t* rows_b = u8 ? rows8 : reinterpret_cast<uint8_t*>(rows);   // the row buffer, as bytes
+  const void* old_b = u8 ? (const void*)ix.rows8 : (const void*)ix.rows;
+  if (e == cudaSuccess && keep) e = cudaMemcpyAsync(rows_b, old_b, (size_t)keep * rb, cudaMemcpyDeviceToDevice, st);
   if (e == cudaSuccess && keep)
     e = cudaMemcpyAsync(inv, ix.inv_norm, (size_t)keep * sizeof(float), cudaMemcpyDeviceToDevice, st);
-  if (e == cudaSuccess) e = cudaMemsetAsync(rows + (size_t)keep * ix.d_pad, 0, (size_t)(n_cap - keep) * rb, st);
+  if (e == cudaSuccess) e = cudaMemsetAsync(rows_b + (size_t)keep * rb, 0, (size_t)(n_cap - keep) * rb, st);
   if (e == cudaSuccess) e = cudaMemsetAsync(inv + keep, 0, (size_t)(n_cap - keep) * sizeof(float), st);
   if (cfac) {
     if (e == cudaSuccess && keep)
@@ -2224,6 +2307,7 @@ int dense_grow(sb_ctx* ctx, DenseIndex& ix, int64_t n_cap) {
   if (e != cudaSuccess) {   // the slot keeps its old buffers; the new ones are released on every failure
     cudaStreamSynchronize(st);
     cudaFree(rows);
+    cudaFree(rows8);
     cudaFree(inv);
     cudaFree(cfac);
     cudaFree(hh);
@@ -2234,11 +2318,13 @@ int dense_grow(sb_ctx* ctx, DenseIndex& ix, int64_t n_cap) {
     return SB_ERR_CUDA;
   }
   cudaFree(ix.rows);
+  cudaFree(ix.rows8);
   cudaFree(ix.inv_norm);
   cudaFree(ix.cfac);
   cudaFree(ix.hh);
   cudaFree(ix.rows32);
   ix.rows = rows;
+  ix.rows8 = rows8;
   ix.inv_norm = inv;
   ix.cfac = cfac;
   ix.hh = hh;
@@ -2301,6 +2387,30 @@ int check_metric_rows(const char* who, int metric, const void* vecs, int64_t n, 
   return SB_OK;
 }
 
+// Input rows of a uint8 slot, checked on the host before anything changes: every value an integer in [0, 255].  SB_U8
+// input holds nothing else.
+int check_u8_rows(const char* who, const void* vecs, int64_t n, int d, int32_t dtype) {
+  if (dtype == SB_U8) return SB_OK;
+  for (int64_t r = 0; r < n; ++r)
+    for (int i = 0; i < d; ++i) {
+      const size_t at = (size_t)r * d + i;
+      const float v = dtype == SB_F32 ? reinterpret_cast<const float*>(vecs)[at]
+                                      : __half2float(reinterpret_cast<const __half*>(vecs)[at]);
+      SB_REQUIRE(v >= 0.f && v <= 255.f && v == floorf(v), SB_ERR_ARG,
+                 "%s: row %lld, component %d is %g; a uint8 slot takes integers in [0, 255]", who, (long long)r, i,
+                 (double)v);
+    }
+  return SB_OK;
+}
+
+// rho >= max ||x|| and hmax >= max ||x||^2 / 2 (rounded up to fp32, as hh is) of uint8 rows whose largest ||x||^2 is xx
+void u8_norm_bounds(int metric, double xx, double* rho, double* hmax) {
+  *rho = metric == SB_METRIC_COSINE ? 0.0 : sqrt(xx) * (1.0 + 0x1p-20);
+  float hf = (float)(0.5 * xx);
+  if ((double)hf < 0.5 * xx) hf = nextafterf(hf, INFINITY);
+  *hmax = metric == SB_METRIC_EUCLID ? (double)hf : 0.0;
+}
+
 }  // namespace
 
 // Shared with other translation units (hybrid batch path, scorers).
@@ -2325,14 +2435,19 @@ int sb_dense_load_storage(sb_ctx* ctx, int slot, const void* vecs, int64_t n, in
   SB_REQUIRE(slot >= 0 && slot < SB_MAX_DENSE_SLOTS, SB_ERR_ARG, "sb_dense_load: bad slot %d", slot);
   SB_REQUIRE(n >= 0 && d > 0 && d <= 4096, SB_ERR_ARG, "sb_dense_load: bad shape n=%lld d=%d", (long long)n, d);
   SB_REQUIRE(n < (1ll << 31), SB_ERR_ARG, "sb_dense_load: a shard holds at most 2^31-1 rows");
-  SB_REQUIRE(dtype == SB_F32 || dtype == SB_F16, SB_ERR_ARG, "sb_dense_load: dtype must be SB_F32 or SB_F16");
+  SB_REQUIRE(dtype == SB_F32 || dtype == SB_F16 || (dtype == SB_U8 && storage == SB_STORAGE_U8), SB_ERR_ARG,
+             "sb_dense_load: dtype must be SB_F32 or SB_F16 (or SB_U8 for SB_STORAGE_U8)");
   SB_REQUIRE(n == 0 || vecs != nullptr, SB_ERR_ARG, "sb_dense_load: vecs is NULL");
   SB_REQUIRE(metric == SB_METRIC_COSINE || metric == SB_METRIC_DOT || metric == SB_METRIC_EUCLID, SB_ERR_ARG,
              "sb_dense_load: metric %d is not supported (SB_METRIC_COSINE, SB_METRIC_DOT or SB_METRIC_EUCLID)", metric);
-  SB_REQUIRE(storage == SB_STORAGE_F16 || storage == SB_STORAGE_F32, SB_ERR_ARG,
-             "sb_dense_load: storage %d is not supported (SB_STORAGE_F16 or SB_STORAGE_F32)", storage);
+  SB_REQUIRE(storage == SB_STORAGE_F16 || storage == SB_STORAGE_F32 || storage == SB_STORAGE_U8, SB_ERR_ARG,
+             "sb_dense_load: storage %d is not supported (SB_STORAGE_F16, SB_STORAGE_F32 or SB_STORAGE_U8)", storage);
+  const bool u8 = storage == SB_STORAGE_U8;
   double rho = 0.0, hmax = 0.0;
-  if (metric != SB_METRIC_COSINE || storage == SB_STORAGE_F32) {   // float32 storage: finite norms for every metric
+  if (u8) {   // the norm bounds come from the store kernel
+    int rc = check_u8_rows("sb_dense_load", vecs, n, d, dtype);
+    if (rc) return rc;
+  } else if (metric != SB_METRIC_COSINE || storage == SB_STORAGE_F32) {   // float32 storage: finite norms for every metric
     int rc = check_metric_rows("sb_dense_load", metric, vecs, n, d, dtype, &rho, &hmax);
     if (rc) return rc;
     if (metric == SB_METRIC_COSINE) rho = 0.0;
@@ -2346,6 +2461,7 @@ int sb_dense_load_storage(sb_ctx* ctx, int slot, const void* vecs, int64_t n, in
   if (ix.cfac) cudaFree(ix.cfac);
   if (ix.hh) cudaFree(ix.hh);
   if (ix.rows32) cudaFree(ix.rows32);
+  if (ix.rows8) cudaFree(ix.rows8);
   for (int f = 0; f < SB_MAX_TAG_FIELDS; ++f)
     if (ix.tags[f]) cudaFree(ix.tags[f]);
   for (int f = 0; f < SB_MAX_VALUE_FIELDS; ++f)
@@ -2353,20 +2469,25 @@ int sb_dense_load_storage(sb_ctx* ctx, int slot, const void* vecs, int64_t n, in
   ix = DenseIndex();
   ix.n = n;
   ix.d = d;
-  ix.d_pad = (d + 7) / 8 * 8;
+  ix.d_pad = u8 ? (d + 63) / 64 * 64 : (d + 7) / 8 * 8;   // uint8: 64-byte rows, every slot fits the wgmma scan
   ix.n_pad = round_rows(n);
   ix.id_base = id_base;
   ix.metric = metric;
   ix.storage = storage;
   ix.rho_max = rho;
   ix.h_max = hmax;
-  if (n == 0) return SB_OK;   // an empty float32 slot gets rows32 with its first growth
+  if (n == 0) return SB_OK;   // an empty float32 / uint8 slot gets rows32 / rows8 with its first growth
   ix.n_cap = ix.n_pad;
-  SB_CUDA(cudaMalloc(&ix.rows, (size_t)ix.n_cap * ix.d_pad * sizeof(__half)));
+  if (u8) {
+    SB_CUDA(cudaMalloc(&ix.rows8, (size_t)ix.n_cap * ix.d_pad));
+    SB_CUDA(cudaMemsetAsync(ix.rows8, 0, (size_t)ix.n_cap * ix.d_pad, ctx->stream));
+  } else {
+    SB_CUDA(cudaMalloc(&ix.rows, (size_t)ix.n_cap * ix.d_pad * sizeof(__half)));
+    SB_CUDA(cudaMemsetAsync(ix.rows, 0, (size_t)ix.n_cap * ix.d_pad * sizeof(__half), ctx->stream));
+  }
   SB_CUDA(cudaMalloc(&ix.inv_norm, (size_t)ix.n_cap * sizeof(float)));
-  SB_CUDA(cudaMemsetAsync(ix.rows, 0, (size_t)ix.n_cap * ix.d_pad * sizeof(__half), ctx->stream));
   SB_CUDA(cudaMemsetAsync(ix.inv_norm, 0, (size_t)ix.n_cap * sizeof(float), ctx->stream));
-  if (metric != SB_METRIC_COSINE) {
+  if (metric != SB_METRIC_COSINE && !u8) {
     SB_CUDA(cudaMalloc(&ix.cfac, (size_t)ix.n_cap * sizeof(double)));
     SB_CUDA(cudaMemsetAsync(ix.cfac, 0, (size_t)ix.n_cap * sizeof(double), ctx->stream));
   }
@@ -2377,6 +2498,12 @@ int sb_dense_load_storage(sb_ctx* ctx, int slot, const void* vecs, int64_t n, in
   if (storage == SB_STORAGE_F32) {
     SB_CUDA(cudaMalloc(&ix.rows32, (size_t)ix.n_cap * ix.d_pad * sizeof(float)));
     SB_CUDA(cudaMemsetAsync(ix.rows32, 0, (size_t)ix.n_cap * ix.d_pad * sizeof(float), ctx->stream));
+  }
+  if (u8) {
+    double xx = 0.0;
+    int rc = dense_store_staged(ctx, ix, vecs, n, dtype, nullptr, 0, &xx);
+    u8_norm_bounds(metric, xx, &ix.rho_max, &ix.h_max);
+    return rc;
   }
   return dense_store_staged(ctx, ix, vecs, n, dtype, nullptr, 0, &ix.sigma_max);
 }
@@ -2420,7 +2547,8 @@ int sb_dense_upsert(sb_ctx* ctx, int slot, const int64_t* rows, const void* vecs
   SB_REQUIRE(ctx != nullptr, SB_ERR_ARG, "sb_dense_upsert: ctx is NULL");
   SB_REQUIRE(slot >= 0 && slot < SB_MAX_DENSE_SLOTS, SB_ERR_ARG, "sb_dense_upsert: bad slot %d", slot);
   SB_REQUIRE(n >= 0, SB_ERR_ARG, "sb_dense_upsert: bad n=%lld", (long long)n);
-  SB_REQUIRE(dtype == SB_F32 || dtype == SB_F16, SB_ERR_ARG, "sb_dense_upsert: dtype must be SB_F32 or SB_F16");
+  SB_REQUIRE(dtype == SB_F32 || dtype == SB_F16 || dtype == SB_U8, SB_ERR_ARG,
+             "sb_dense_upsert: dtype must be SB_F32, SB_F16 or SB_U8");
   SB_REQUIRE(n == 0 || (rows != nullptr && vecs != nullptr), SB_ERR_ARG, "sb_dense_upsert: NULL buffer");
   std::lock_guard<std::mutex> lk(ctx->mu);
   DeviceGuard g(ctx->device);
@@ -2435,8 +2563,12 @@ int sb_dense_upsert(sb_ctx* ctx, int slot, const int64_t* rows, const void* vecs
   const int64_t m = sorted.end() - std::lower_bound(sorted.begin(), sorted.end(), ix.n);
   SB_REQUIRE(m == 0 || (sorted[n - m] == ix.n && sorted[n - 1] == ix.n + m - 1), SB_ERR_ARG,
              "sb_dense_upsert: appended rows must be exactly %lld .. %lld", (long long)ix.n, (long long)(ix.n + m - 1));
+  const bool u8 = ix.storage == SB_STORAGE_U8;
+  SB_REQUIRE(dtype != SB_U8 || u8, SB_ERR_ARG, "sb_dense_upsert: SB_U8 rows need a uint8 slot");
   double rho = 0.0, hmax = 0.0, sigma = 0.0;
-  if (ix.metric != SB_METRIC_COSINE || ix.storage == SB_STORAGE_F32) {
+  if (u8) {
+    if ((rc = check_u8_rows("sb_dense_upsert", vecs, n, ix.d, dtype))) return rc;
+  } else if (ix.metric != SB_METRIC_COSINE || ix.storage == SB_STORAGE_F32) {
     if ((rc = check_metric_rows("sb_dense_upsert", ix.metric, vecs, n, ix.d, dtype, &rho, &hmax))) return rc;
     if (ix.metric == SB_METRIC_COSINE) rho = 0.0;
   }
@@ -2448,6 +2580,10 @@ int sb_dense_upsert(sb_ctx* ctx, int slot, const int64_t* rows, const void* vecs
   int64_t* dst = ctx->misc2_dev.as<int64_t>();
   SB_CUDA(cudaMemcpyAsync(dst, rows, (size_t)n * 8, cudaMemcpyHostToDevice, ctx->stream));
   if ((rc = dense_store_staged(ctx, ix, vecs, n, dtype, dst, 0, &sigma))) return rc;
+  if (u8) {   // sigma is the largest ||x||^2 of the rows; a uint8 slot's own sigma stays 0
+    u8_norm_bounds(ix.metric, sigma, &rho, &hmax);
+    sigma = 0.0;
+  }
   for (int f = 0; f < SB_MAX_TAG_FIELDS; ++f)
     if (ix.tags[f])
       dense_tags_scatter_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(ix.tags[f], dst, nullptr, n);
@@ -2535,6 +2671,7 @@ int sb_dense_delete(sb_ctx* ctx, int slot, const int64_t* rows, int64_t n, int64
     mp.cfac = ix.cfac;
     mp.hh = ix.hh;
     mp.rows32 = ix.rows32;
+    mp.rows8 = ix.rows8;
     memcpy(mp.tags, ix.tags, sizeof(mp.tags));
     memcpy(mp.vals, ix.vals, sizeof(mp.vals));
     mp.from = f_dev;
@@ -2545,7 +2682,9 @@ int sb_dense_delete(sb_ctx* ctx, int slot, const int64_t* rows, int64_t n, int64
     SB_CUDA(cudaGetLastError());
   }
   // the vacated tail [keep, n) returns to the zero state of unused capacity
-  SB_CUDA(cudaMemsetAsync(ix.rows + (size_t)keep * ix.d_pad, 0, (size_t)n * ix.d_pad * sizeof(__half), ctx->stream));
+  if (ix.rows)
+    SB_CUDA(cudaMemsetAsync(ix.rows + (size_t)keep * ix.d_pad, 0, (size_t)n * ix.d_pad * sizeof(__half), ctx->stream));
+  if (ix.rows8) SB_CUDA(cudaMemsetAsync(ix.rows8 + (size_t)keep * ix.d_pad, 0, (size_t)n * ix.d_pad, ctx->stream));
   SB_CUDA(cudaMemsetAsync(ix.inv_norm + keep, 0, (size_t)n * sizeof(float), ctx->stream));
   if (ix.cfac) SB_CUDA(cudaMemsetAsync(ix.cfac + keep, 0, (size_t)n * sizeof(double), ctx->stream));
   if (ix.hh) SB_CUDA(cudaMemsetAsync(ix.hh + keep, 0, (size_t)n * sizeof(float), ctx->stream));
@@ -2669,7 +2808,10 @@ int sb_dense_fetch(sb_ctx* ctx, int slot, const int64_t* ids, int32_t n_ids, flo
   if ((rc = ctx->misc2_dev.reserve((size_t)n_ids * 8))) return rc;
   if ((rc = ctx->misc3_dev.reserve((size_t)n_ids * ix.d * 4))) return rc;
   SB_CUDA(cudaMemcpyAsync(ctx->misc2_dev.p, ids, (size_t)n_ids * 8, cudaMemcpyHostToDevice, ctx->stream));
-  if (ix.rows32)
+  if (ix.rows8)
+    dense_fetch_u8_kernel<<<n_ids, 128, 0, ctx->stream>>>(ix.rows8, ix.d, ix.d_pad, ix.n, ix.id_base,
+                                                          ctx->misc2_dev.as<int64_t>(), n_ids, ctx->misc3_dev.as<float>());
+  else if (ix.rows32)
     dense_fetch_f32_kernel<<<n_ids, 128, 0, ctx->stream>>>(ix.rows32, ix.metric == SB_METRIC_COSINE, ix.d, ix.d_pad, ix.n,
                                                            ix.id_base, ctx->misc2_dev.as<int64_t>(), n_ids,
                                                            ctx->misc3_dev.as<float>());

@@ -15,6 +15,7 @@ struct RescoreArgs {
   int32_t metric;       // SB_METRIC_*
   const double* cfac;   // [rows] c of v = c * y (Dot / Euclid)
   const float* rows32;  // float32 storage: [rows][d_pad] the caller's x (read by the F32 instantiations only)
+  const uint8_t* rows8; // uint8 storage: [rows][d_pad] the caller's x (read by the U8 instantiations only)
 };
 
 // ---- approximate -> exact hand-off (DESIGN.md "K1: exactness") --------------------------------------------------------
@@ -32,6 +33,14 @@ struct RescoreArgs {
 __host__ __device__ __forceinline__ float dense_eps_fp32(int d_pad) { return (float)d_pad * 1.1920929e-7f + 1.9073486e-6f; }
 // accumulation part of the wgmma scan's eps: the tensor core's fp32 accumulator may truncate (<= 2 ulp per step)
 __host__ __device__ __forceinline__ float dense_eps_mma_acc(int d_pad) { return (float)d_pad * 2.3841858e-7f + 1.9073486e-6f; }
+
+// uint8 scan (DESIGN.md K1i): natural column c (0..63) of a 64-column block -> its column in the permuted fp16 query block.
+// Byte c = 16 t + 4 s + j of a corpus row is the wgmma A element of k16 step s at k = 2 t + j (j < 2) or 2 t + 8 + j - 2
+// (j >= 2) for the thread with lane % 4 = t, so the query's column c goes to 16 s + that k.
+__host__ __device__ __forceinline__ int u8_query_column(int c) {
+  const int t = c >> 4, s = (c >> 2) & 3, j = c & 3;
+  return 16 * s + 2 * t + (j < 2 ? j : 6 + j);
+}
 
 // lower edge of the window as a composite key (keys >= it are members)
 __device__ __forceinline__ unsigned long long window_lo_key(unsigned long long kth_lb_key, float eps) {
@@ -220,6 +229,61 @@ __device__ __forceinline__ void exact_f32_warp(int metric, const float* rows32, 
   }
 }
 
+// Exact fp64 ordering key of NR uint8-storage rows x (DESIGN.md K1i), one full warp; every lane returns them.  The same
+// formulas and operation order as exact_f32_warp; every product q_i x_i and every x_i^2 is exact in fp64.  Lane l reads
+// the 8 bytes of chunk c = l + 32 j of every row with one 8-byte load (rows are 64-byte aligned).
+template <int NR>
+__device__ __forceinline__ void exact_u8_warp(int metric, const uint8_t* rows8, const uint32_t (&idx)[NR], const float* q,
+                                              int d_pad, int nch, double qn, int lane, double (&out)[NR]) {
+  const bool euclid = metric == SB_METRIC_EUCLID, cosine = metric == SB_METRIC_COSINE;
+  const uint2* r[NR];
+  double acc[NR], xx[NR];
+#pragma unroll
+  for (int i = 0; i < NR; ++i) {
+    r[i] = reinterpret_cast<const uint2*>(rows8 + (size_t)idx[i] * d_pad);
+    acc[i] = 0.0;
+    xx[i] = 0.0;
+  }
+  for (int ch = lane; ch < nch; ch += 32) {
+    const float4 qa = *reinterpret_cast<const float4*>(q + (size_t)ch * 8);
+    const float4 qb = *reinterpret_cast<const float4*>(q + (size_t)ch * 8 + 4);
+    const float qv[8] = {qa.x, qa.y, qa.z, qa.w, qb.x, qb.y, qb.z, qb.w};
+    uint2 raw[NR];
+#pragma unroll
+    for (int i = 0; i < NR; ++i) raw[i] = __ldg(r[i] + ch);
+#pragma unroll
+    for (int i = 0; i < NR; ++i) {
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        const uint32_t w = e < 4 ? raw[i].x : raw[i].y;
+        const double x = (double)((w >> (8 * (e & 3))) & 0xffu), qe = (double)qv[e];
+        if (euclid) {
+          const double t = __dsub_rn(qe, x);
+          acc[i] = __fma_rn(t, t, acc[i]);
+        } else {
+          acc[i] = __fma_rn(x, qe, acc[i]);
+          if (cosine) xx[i] = __fma_rn(x, x, xx[i]);
+        }
+      }
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < NR; ++i) {
+    for (int o = 16; o; o >>= 1) {
+      acc[i] += __shfl_xor_sync(0xffffffffu, acc[i], o);
+      xx[i] += __shfl_xor_sync(0xffffffffu, xx[i], o);
+    }
+    if (euclid) {
+      out[i] = -sqrt(acc[i]);
+    } else if (cosine) {
+      const double den = qn * sqrt(xx[i]);
+      out[i] = den > 0.0 ? acc[i] / den : 0.0;
+    } else {
+      out[i] = acc[i];
+    }
+  }
+}
+
 // exact ordering key of one stored row under the slot's metric (Cosine: the existing cosine path)
 __device__ __forceinline__ double exact_key_warp(int metric, const __half* rows, const double* cfac, uint32_t idx,
                                                  const float* q, int d_pad, int nch, double qn, int lane) {
@@ -230,14 +294,21 @@ __device__ __forceinline__ double exact_key_warp(int metric, const __half* rows,
   return s[0];
 }
 
-// exact ordering key of one row under the slot's storage: F32 scores the caller's x, else the stored fp16 representation
-template <bool F32>
+// exact ordering key of one row under the slot's storage ST (SB_STORAGE_*): float32 and uint8 score the caller's x,
+// float16 the stored fp16 representation
+template <int ST>
 __device__ __forceinline__ double exact_key_row(int metric, const __half* rows, const double* cfac, const float* rows32,
-                                                uint32_t idx, const float* q, int d_pad, int nch, double qn, int lane) {
-  if constexpr (F32) {
+                                                const uint8_t* rows8, uint32_t idx, const float* q, int d_pad, int nch,
+                                                double qn, int lane) {
+  if constexpr (ST == SB_STORAGE_F32) {
     const uint32_t ix[1] = {idx};
     double s[1];
     exact_f32_warp<1>(metric, rows32, ix, q, d_pad, nch, qn, lane, s);
+    return s[0];
+  } else if constexpr (ST == SB_STORAGE_U8) {
+    const uint32_t ix[1] = {idx};
+    double s[1];
+    exact_u8_warp<1>(metric, rows8, ix, q, d_pad, nch, qn, lane, s);
     return s[0];
   } else {
     return exact_key_warp(metric, rows, cfac, idx, q, d_pad, nch, qn, lane);
@@ -307,9 +378,9 @@ __device__ __forceinline__ void exact_cosine_warp2(const __half* rows, uint32_t 
 // Exact fp64 re-score of the window members sel[0..nsel) (composite keys) against the STORED fp16 rows and the fp32
 // query, final order (score desc, row asc), emit k results.  Whole-CTA cooperative; ek/ei are P-entry shared-memory
 // arrays (P = power of two >= nsel), qq_s a shared double, q_s a shared-memory staging area for the query (d_pad floats;
-// the L2 round trip of the query per re-scored row was a third of the stage's latency).  F32: float32 storage, the
-// window is re-scored against the caller's fp32 rows (exact_f32_warp).
-template <bool F32>
+// the L2 round trip of the query per re-scored row was a third of the stage's latency).  ST = SB_STORAGE_F32 / _U8: the
+// window is re-scored against the caller's rows (exact_f32_warp / exact_u8_warp).
+template <int ST>
 __device__ __forceinline__ void rescore_and_emit(const unsigned long long* sel, int nsel, int P, unsigned long long* ek,
                                                  uint32_t* ei, double* qq_s_ptr, float* q_s, const RescoreArgs p) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nt = blockDim.x, nw = nt >> 5;
@@ -326,10 +397,16 @@ __device__ __forceinline__ void rescore_and_emit(const unsigned long long* sel, 
       i0 = key32_idx(key0);
       i1 = key32_idx(key1);
       double s0, s1;
-      if constexpr (F32) {
+      if constexpr (ST == SB_STORAGE_F32) {
         const uint32_t ix[2] = {i0, i1};
         double s[2];
         exact_f32_warp<2>(p.metric, p.rows32, ix, q_s, p.d_pad, p.ch, qn, lane, s);
+        s0 = s[0];
+        s1 = s[1];
+      } else if constexpr (ST == SB_STORAGE_U8) {
+        const uint32_t ix[2] = {i0, i1};
+        double s[2];
+        exact_u8_warp<2>(p.metric, p.rows8, ix, q_s, p.d_pad, p.ch, qn, lane, s);
         s0 = s[0];
         s1 = s[1];
       } else if (p.metric == SB_METRIC_COSINE) {
@@ -345,10 +422,10 @@ __device__ __forceinline__ void rescore_and_emit(const unsigned long long* sel, 
       o1 = f64_orderable(s1);
     } else if (key0 != 0ull) {
       i0 = key32_idx(key0);
-      o0 = f64_orderable(exact_key_row<F32>(p.metric, p.rows, p.cfac, p.rows32, i0, q_s, p.d_pad, p.ch, qn, lane));
+      o0 = f64_orderable(exact_key_row<ST>(p.metric, p.rows, p.cfac, p.rows32, p.rows8, i0, q_s, p.d_pad, p.ch, qn, lane));
     } else if (key1 != 0ull) {
       i1 = key32_idx(key1);
-      o1 = f64_orderable(exact_key_row<F32>(p.metric, p.rows, p.cfac, p.rows32, i1, q_s, p.d_pad, p.ch, qn, lane));
+      o1 = f64_orderable(exact_key_row<ST>(p.metric, p.rows, p.cfac, p.rows32, p.rows8, i1, q_s, p.d_pad, p.ch, qn, lane));
     }
     if (key0 != 0ull && o0 == 0ull) o0 = 1ull;  // keep 0 reserved for "empty"
     if (key1 != 0ull && o1 == 0ull) o1 = 1ull;

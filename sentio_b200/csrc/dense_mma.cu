@@ -27,6 +27,11 @@
 //
 // Warp roles (288 threads, 1 CTA / SM, persistent): warps 0..7 = two consumer warpgroups (MMA + epilogue; a thread holds
 // two corpus rows x QBN / 4 query columns of the accumulator), warp 8 = TMA producer.
+//
+// Uint8 storage (ST = SB_STORAGE_U8, DESIGN.md K1i): the corpus box is 64 bytes x 128 rows (8 KB, no swizzle) of the
+// integer rows x.  Each consumer thread reads 16 bytes of its two accumulator rows per box, turns them into f16x2 A
+// fragments in registers (exact: 0..255 are fp16 integers) and issues the register-A form of the same MMAs.  The query
+// block's columns are permuted inside each 64-column block to match (u8_query_column).  Every other step is the same.
 #include <cuda.h>
 
 #include <math.h>
@@ -43,6 +48,7 @@ namespace {
 constexpr int kTileRows = 128;
 constexpr int kBK = 64;                       // fp16 elements per 128-byte swizzle row
 constexpr uint32_t kATileBytes = kTileRows * kBK * 2;   // 16 KB
+constexpr uint32_t kATileBytesU8 = kTileRows * kBK;     // 8 KB: a uint8 corpus box
 constexpr int kConsumerWarps = 8;
 constexpr int kMmaThreads = 32 * kConsumerWarps + 32;
 constexpr int kQbnMax = 256;                  // queries per group (m64n256k16)
@@ -60,6 +66,15 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
       "l"(map), "r"(c0), "r"(c1), "r"(bar), "l"(policy)
       : "memory");
 }
+// 4 bytes b0..b3 -> the f16x2 pair (b0, b1) (sel 0x5140) or (b2, b3) (sel 0x7362): 1024 + b has the bit pattern
+// 0x6400 | b, and subtracting 1024 is exact
+__device__ __forceinline__ uint32_t u8_f16x2(uint32_t w, uint32_t sel) {
+  const uint32_t h = __byte_perm(w, 0x64646464u, sel);
+  uint32_t r;
+  asm("sub.rn.f16x2 %0, %1, %2;" : "=r"(r) : "r"(h), "r"(0x64006400u));
+  return r;
+}
+
 // L2 prefetch of a tensor-map box (no shared-memory destination): keeps more HBM requests in flight than the ring holds
 __device__ __forceinline__ void tma_prefetch_l2_2d(const CUtensorMap* map, int c0, int c1) {
   asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global [%0, {%1, %2}];" ::"l"(map), "r"(c0), "r"(c1) : "memory");
@@ -100,7 +115,7 @@ struct MmaScanParams {
 };
 
 // Key of a row (dense.cu dense_scan_kernel): acc * scale[row], EUCLID r * (acc * scale[row]) - h[row].
-template <int QBN, bool FILTER, bool EUCLID>
+template <int QBN, bool FILTER, bool EUCLID, int ST>
 __global__ void __launch_bounds__(kMmaThreads, 1)
 dense_scan_mma_kernel(const __grid_constant__ CUtensorMap tm_rows, const __grid_constant__ CUtensorMap tm_q,
                       const MmaScanParams p) {
@@ -108,8 +123,10 @@ dense_scan_mma_kernel(const __grid_constant__ CUtensorMap tm_rows, const __grid_
   const uint32_t raw = smem_u32(msm_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;  // SWIZZLE_128B operands need 1024-byte alignment
   uint8_t* sm = msm_raw + (base - raw);
+  constexpr bool U8 = ST == SB_STORAGE_U8;
+  constexpr uint32_t kABytes = U8 ? kATileBytesU8 : kATileBytes;   // one corpus box
   constexpr uint32_t kQBoxBytes = QBN * kBK * 2;              // one 64-column box of the query block
-  constexpr uint32_t kStageBytes = kATileBytes + kQBoxBytes;  // corpus box, then query box
+  constexpr uint32_t kStageBytes = kABytes + kQBoxBytes;      // corpus box, then query box
   uint64_t* bars = reinterpret_cast<uint64_t*>(sm + (size_t)p.stages * kStageBytes);
   const uint32_t bar_full = smem_u32(bars), bar_empty = smem_u32(bars + p.stages);
   float* thr = reinterpret_cast<float*>(bars + 2 * p.stages);   // [QBN], 8-byte aligned
@@ -159,7 +176,7 @@ dense_scan_mma_kernel(const __grid_constant__ CUtensorMap tm_rows, const __grid_
           const uint32_t stage = base + (uint32_t)s * kStageBytes;
           mbar_expect_tx(bar_full + 8 * s, kStageBytes);   // both boxes complete on the stage's one barrier
           tma_load_2d(stage, &tm_rows, kb * kBK, row, bar_full + 8 * s, pol_corpus);
-          tma_load_2d(stage + kATileBytes, &tm_q, kb * kBK, 0, bar_full + 8 * s, pol_query);
+          tma_load_2d(stage + kABytes, &tm_q, kb * kBK, 0, bar_full + 8 * s, pol_query);
         }
       }
     }
@@ -181,21 +198,63 @@ dense_scan_mma_kernel(const __grid_constant__ CUtensorMap tm_rows, const __grid_
         h1 = ldg_early(p.hh + row0 + 8, live1);
       }
       float acc[QBN / 2];
-      for (int kb = 0; kb < p.kb_count; ++kb, ++it) {
-        const int s = it % p.stages;
-        mbar_wait(bar_full + 8 * s, (uint32_t)(it / p.stages) & 1u);
-        const uint32_t stage = base + (uint32_t)s * kStageBytes;
-        const uint64_t da = wgmma_desc_sw128(stage + (uint32_t)wg * (kATileBytes / 2));
-        const uint64_t db = wgmma_desc_sw128(stage + kATileBytes);
-        wgmma_fence();
+      if constexpr (U8) {
+        // this thread's 16 bytes of rows row0 and row0 + 8 in a box (64-byte rows): one warp reads 8 rows x 64
+        // contiguous bytes per load.  A fragments of box kb stay live until its MMAs retire, one box after they are
+        // issued, so the boxes alternate between two register sets.
+        const uint32_t a_off = (uint32_t)(wg * 64 + (warp & 3) * 16 + (lane >> 2)) * (uint32_t)kBK + 16u * (lane & 3);
+        uint32_t fa[16], fb[16];
+        auto box = [&](int kb, uint32_t(&a)[16]) {
+          const int s = it % p.stages;
+          mbar_wait(bar_full + 8 * s, (uint32_t)(it / p.stages) & 1u);
+          const uint32_t stage = base + (uint32_t)s * kStageBytes;
+          uint32_t w0[4], w1[4];
+          asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];"
+                       : "=r"(w0[0]), "=r"(w0[1]), "=r"(w0[2]), "=r"(w0[3])
+                       : "r"(stage + a_off));
+          asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];"
+                       : "=r"(w1[0]), "=r"(w1[1]), "=r"(w1[2]), "=r"(w1[3])
+                       : "r"(stage + a_off + 8u * kBK));
 #pragma unroll
-        for (int k = 0; k < kBK / 16; ++k)
-          Wgmma<QBN>::mma(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb | k) ? 1u : 0u);
-        wgmma_commit();
-        // this box's MMAs stay in flight; the previous box has been read once they are the only ones left
-        wgmma_wait<1>();
-        __syncwarp();
-        if (kb > 0 && lane == 0) mbar_arrive(bar_empty + 8 * ((it - 1) % p.stages));
+          for (int k = 0; k < kBK / 16; ++k) {   // word k holds bytes 16 t + 4 k .. + 3: k16 step k
+            a[4 * k + 0] = u8_f16x2(w0[k], 0x5140u);
+            a[4 * k + 1] = u8_f16x2(w1[k], 0x5140u);
+            a[4 * k + 2] = u8_f16x2(w0[k], 0x7362u);
+            a[4 * k + 3] = u8_f16x2(w1[k], 0x7362u);
+          }
+          const uint64_t db = wgmma_desc_sw128(stage + kABytes);
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < kBK / 16; ++k)
+            WgmmaRA<QBN>::mma(acc, a[4 * k], a[4 * k + 1], a[4 * k + 2], a[4 * k + 3], db + (uint64_t)(2 * k),
+                              (kb | k) ? 1u : 0u);
+          wgmma_commit();
+          wgmma_wait<1>();
+          __syncwarp();
+          if (kb > 0 && lane == 0) mbar_arrive(bar_empty + 8 * ((it - 1) % p.stages));
+          ++it;
+        };
+        for (int kb = 0; kb < p.kb_count; kb += 2) {
+          box(kb, fa);
+          if (kb + 1 < p.kb_count) box(kb + 1, fb);
+        }
+      } else {
+        for (int kb = 0; kb < p.kb_count; ++kb, ++it) {
+          const int s = it % p.stages;
+          mbar_wait(bar_full + 8 * s, (uint32_t)(it / p.stages) & 1u);
+          const uint32_t stage = base + (uint32_t)s * kStageBytes;
+          const uint64_t da = wgmma_desc_sw128(stage + (uint32_t)wg * (kATileBytes / 2));
+          const uint64_t db = wgmma_desc_sw128(stage + kATileBytes);
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < kBK / 16; ++k)
+            Wgmma<QBN>::mma(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb | k) ? 1u : 0u);
+          wgmma_commit();
+          // this box's MMAs stay in flight; the previous box has been read once they are the only ones left
+          wgmma_wait<1>();
+          __syncwarp();
+          if (kb > 0 && lane == 0) mbar_arrive(bar_empty + 8 * ((it - 1) % p.stages));
+        }
       }
       wgmma_wait<0>();
       __syncwarp();
@@ -299,7 +358,8 @@ struct SelectParams {
   const int32_t* state;             // FILTER only: [nq] 1 = answered by the gather path (threshold +inf, no emit)
   int32_t metric;
   const double* cfac;
-  const float* rows32;              // F32 only
+  const float* rows32;              // float32 storage only
+  const uint8_t* rows8;             // uint8 storage only
 };
 
 // One CTA per query.  A lower bound of the k-th best approximate key among the survivors of all CTAs by an MSB-first
@@ -308,8 +368,8 @@ struct SelectParams {
 //   mode 0 (sampling pass): threshold = that score - 2 eps.
 //   mode 1: gather every survivor inside the window below it, exact fp64 re-score of all of them, emit k.
 // Survivors are staged in shared memory when they fit (the normal case: ~0.3 % of the corpus); otherwise every pass
-// streams them from HBM/L2 -- slower, still exact.  F32: float32 storage, the exact stage scores the caller's rows.
-template <bool FILTER, bool F32>
+// streams them from HBM/L2 -- slower, still exact.  ST = SB_STORAGE_F32 / _U8: the exact stage scores the caller's rows.
+template <bool FILTER, int ST>
 __global__ void __launch_bounds__(kSelectThreads, 2) dense_select_kernel(const SelectParams p) {
   extern __shared__ __align__(16) uint8_t ssm[];
   unsigned long long* keys = reinterpret_cast<unsigned long long*>(ssm);  // [kSelStage] staged survivors
@@ -451,15 +511,17 @@ __global__ void __launch_bounds__(kSelectThreads, 2) dense_select_kernel(const S
   ra.metric = p.metric;
   ra.cfac = p.cfac;
   ra.rows32 = p.rows32;
+  ra.rows8 = p.rows8;
   // the staged survivors are dead (the window lives in `top`): their shared memory becomes the query staging area
-  rescore_and_emit<F32>(top, ntop, P, ek, ei, &qq_s, reinterpret_cast<float*>(keys), ra);
+  rescore_and_emit<ST>(top, ntop, P, ek, ei, &qq_s, reinterpret_cast<float*>(keys), ra);
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
-int encode_map(CUtensorMap* map, const void* ptr, int64_t rows, int64_t cols, int box_rows) {
+// fp16 K-major operand (SWIZZLE_128B, 64-column boxes), or with u8 the uint8 corpus (64-byte boxes, no swizzle)
+int encode_map(CUtensorMap* map, const void* ptr, int64_t rows, int64_t cols, int box_rows, bool u8 = false) {
   static EncodeTiledFn fn = nullptr;
   if (!fn) {
     void* pfn = nullptr;
@@ -470,47 +532,50 @@ int encode_map(CUtensorMap* map, const void* ptr, int64_t rows, int64_t cols, in
   }
   SB_REQUIRE(fn != nullptr, SB_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
   cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)cols * 2};
+  cuuint64_t strides[1] = {(cuuint64_t)cols * (u8 ? 1 : 2)};
   cuuint32_t box[2] = {(cuuint32_t)kBK, (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+  CUresult r = fn(map, u8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(ptr),
+                  dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                  u8 ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   SB_REQUIRE(r == CUDA_SUCCESS, SB_ERR_CUDA, "cuTensorMapEncodeTiled failed with CUresult %d", (int)r);
   return SB_OK;
 }
 
 // ring stages of a QBN-query group: corpus box + query box each, capped by SB_DENSE_STAGES.  Per query: threshold and
-// count, and for Euclid the query norm r.
+// count, and for Euclid the query norm r.  A uint8 corpus box is half the size (at QBN = 256: 40 KB stages, five fit).
 size_t mma_per_query(bool euclid) { return euclid ? 12 : 8; }
-int mma_stages(const sb_ctx* ctx, int qbn, bool euclid = false) {
-  const size_t stage = kATileBytes + (size_t)qbn * kBK * 2 + 16;   // + its full / empty barriers
+int mma_stages(const sb_ctx* ctx, int qbn, bool euclid = false, bool u8 = false) {
+  const size_t stage = (u8 ? kATileBytesU8 : kATileBytes) + (size_t)qbn * kBK * 2 + 16;   // + its full / empty barriers
   const size_t fixed = 1024 + (size_t)qbn * mma_per_query(euclid); // alignment slack + per-query values
   return std::min((int)((ctx->smem_optin - fixed) / stage), ctx->dense_max_stages);
 }
-size_t mma_smem(int qbn, int stages, bool euclid) {
-  return 1024 + (size_t)stages * (kATileBytes + (size_t)qbn * kBK * 2 + 16) + (size_t)qbn * mma_per_query(euclid);
+size_t mma_smem(int qbn, int stages, bool euclid, bool u8 = false) {
+  return 1024 + (size_t)stages * ((u8 ? kATileBytesU8 : kATileBytes) + (size_t)qbn * kBK * 2 + 16) +
+         (size_t)qbn * mma_per_query(euclid);
 }
 
-template <int QBN, bool FILTER, bool EUCLID>
+template <int QBN, bool FILTER, bool EUCLID, int ST>
 int launch_mma(const CUtensorMap& tm_rows, const CUtensorMap& tm_q, const MmaScanParams& mp, int grid, size_t smem,
                cudaStream_t st) {
-  auto kern = dense_scan_mma_kernel<QBN, FILTER, EUCLID>;
+  auto kern = dense_scan_mma_kernel<QBN, FILTER, EUCLID, ST>;
   SB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   kern<<<grid, kMmaThreads, smem, st>>>(tm_rows, tm_q, mp);
   SB_CUDA(cudaGetLastError());
   return SB_OK;
 }
 
-template <bool FILTER, bool EUCLID>
+// ST: SB_STORAGE_U8 for a uint8 corpus; float16 and float32 slots scan the same fp16 rows (SB_STORAGE_F16)
+template <bool FILTER, bool EUCLID, int ST>
 int dispatch_mma(int qbn, const CUtensorMap& tm_rows, const CUtensorMap& tm_q, const MmaScanParams& mp, int grid,
                  size_t smem, cudaStream_t st) {
   switch (qbn) {
-    case 16: return launch_mma<16, FILTER, EUCLID>(tm_rows, tm_q, mp, grid, smem, st);
-    case 32: return launch_mma<32, FILTER, EUCLID>(tm_rows, tm_q, mp, grid, smem, st);
-    case 64: return launch_mma<64, FILTER, EUCLID>(tm_rows, tm_q, mp, grid, smem, st);
-    case 128: return launch_mma<128, FILTER, EUCLID>(tm_rows, tm_q, mp, grid, smem, st);
-    case 256: return launch_mma<256, FILTER, EUCLID>(tm_rows, tm_q, mp, grid, smem, st);
+    case 16: return launch_mma<16, FILTER, EUCLID, ST>(tm_rows, tm_q, mp, grid, smem, st);
+    case 32: return launch_mma<32, FILTER, EUCLID, ST>(tm_rows, tm_q, mp, grid, smem, st);
+    case 64: return launch_mma<64, FILTER, EUCLID, ST>(tm_rows, tm_q, mp, grid, smem, st);
+    case 128: return launch_mma<128, FILTER, EUCLID, ST>(tm_rows, tm_q, mp, grid, smem, st);
+    case 256: return launch_mma<256, FILTER, EUCLID, ST>(tm_rows, tm_q, mp, grid, smem, st);
   }
   sb_set_error("dense_mma: unsupported query block %d", qbn);
   return SB_ERR_UNSUPPORTED;
@@ -571,27 +636,40 @@ int dense_mma_topk_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int 
   float* thr = ctx->misc3_dev.as<float>();
   int32_t* counts = reinterpret_cast<int32_t*>(thr + (size_t)gsz * gmax);
   unsigned long long* cand = ctx->cand_dev.as<unsigned long long>();
-  if (ix.tm_rows_ptr != ix.rows || ix.tm_n_pad != ix.n_pad) {  // (re)build the corpus map when rows or n_pad change
-    if ((rc = encode_map(reinterpret_cast<CUtensorMap*>(ix.tm_rows), ix.rows, ix.n_pad, ix.d_pad, kTileRows))) return rc;
-    ix.tm_rows_ptr = ix.rows;
+  const bool u8 = ix.storage == SB_STORAGE_U8;
+  const void* corpus = u8 ? (const void*)ix.rows8 : (const void*)ix.rows;
+  if (ix.tm_rows_ptr != corpus || ix.tm_n_pad != ix.n_pad) {  // (re)build the corpus map when rows or n_pad change
+    if ((rc = encode_map(reinterpret_cast<CUtensorMap*>(ix.tm_rows), corpus, ix.n_pad, ix.d_pad, kTileRows, u8)))
+      return rc;
+    ix.tm_rows_ptr = corpus;
     ix.tm_n_pad = ix.n_pad;
   }
   const CUtensorMap& tm_rows = *reinterpret_cast<const CUtensorMap*>(ix.tm_rows);
   const size_t sel_smem = (size_t)kSelStage * 8 + (size_t)kSelTop * 20 + 64;
-  const bool f32 = ix.rows32 != nullptr;
-  auto sel_kern = flt ? (f32 ? dense_select_kernel<true, true> : dense_select_kernel<true, false>)
-                      : (f32 ? dense_select_kernel<false, true> : dense_select_kernel<false, false>);
+  auto sel_kern = flt ? dense_select_kernel<true, SB_STORAGE_F16> : dense_select_kernel<false, SB_STORAGE_F16>;
+  if (ix.storage == SB_STORAGE_F32)
+    sel_kern = flt ? dense_select_kernel<true, SB_STORAGE_F32> : dense_select_kernel<false, SB_STORAGE_F32>;
+  else if (u8)
+    sel_kern = flt ? dense_select_kernel<true, SB_STORAGE_U8> : dense_select_kernel<false, SB_STORAGE_U8>;
   SB_CUDA(cudaFuncSetAttribute(sel_kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sel_smem));
   auto launch_select = [&](int nblocks, const SelectParams& s) {
     sel_kern<<<nblocks, kSelectThreads, sel_smem, st>>>(s);
   };
   const bool euclid = ix.metric == SB_METRIC_EUCLID;   // Cosine and Dot run the same (acc * scale) kernels
   auto run_mma = [&](int qbn, const CUtensorMap& tm_q, const MmaScanParams& m, int g, size_t smem) {
+    constexpr int F16 = SB_STORAGE_F16, U8 = SB_STORAGE_U8;
+    if (u8) {
+      if (euclid)
+        return flt ? dispatch_mma<true, true, U8>(qbn, tm_rows, tm_q, m, g, smem, st)
+                   : dispatch_mma<false, true, U8>(qbn, tm_rows, tm_q, m, g, smem, st);
+      return flt ? dispatch_mma<true, false, U8>(qbn, tm_rows, tm_q, m, g, smem, st)
+                 : dispatch_mma<false, false, U8>(qbn, tm_rows, tm_q, m, g, smem, st);
+    }
     if (euclid)
-      return flt ? dispatch_mma<true, true>(qbn, tm_rows, tm_q, m, g, smem, st)
-                 : dispatch_mma<false, true>(qbn, tm_rows, tm_q, m, g, smem, st);
-    return flt ? dispatch_mma<true, false>(qbn, tm_rows, tm_q, m, g, smem, st)
-               : dispatch_mma<false, false>(qbn, tm_rows, tm_q, m, g, smem, st);
+      return flt ? dispatch_mma<true, true, F16>(qbn, tm_rows, tm_q, m, g, smem, st)
+                 : dispatch_mma<false, true, F16>(qbn, tm_rows, tm_q, m, g, smem, st);
+    return flt ? dispatch_mma<true, false, F16>(qbn, tm_rows, tm_q, m, g, smem, st)
+               : dispatch_mma<false, false, F16>(qbn, tm_rows, tm_q, m, g, smem, st);
   };
   // normalised fp16 operand rows of the whole batch (rows beyond B are zero), eps, cleared fallback flags (and r)
   float *eps = nullptr, *rq = nullptr;
@@ -613,8 +691,8 @@ int dense_mma_topk_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int 
       while (G.qbn > 16 && G.qbn / 2 >= left) G.qbn >>= 1;
       G.nq = std::min(G.qbn, left);
       if ((rc = encode_map(&G.tm_q, q16g, G.qbn, ix.d_pad, G.qbn))) return rc;
-      G.stages = mma_stages(ctx, G.qbn, euclid);
-      G.smem = mma_smem(G.qbn, G.stages, euclid);
+      G.stages = mma_stages(ctx, G.qbn, euclid, u8);
+      G.smem = mma_smem(G.qbn, G.stages, euclid, u8);
       rows_total = g * gsz + G.qbn;
     }
     MmaScanParams mp;
@@ -629,6 +707,7 @@ int dense_mma_topk_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int 
     sp.metric = ix.metric;
     sp.cfac = ix.cfac;
     sp.rows32 = ix.rows32;
+    sp.rows8 = ix.rows8;
     sp.cand = cand;
     sp.counts = counts;
     sp.capg = capg;

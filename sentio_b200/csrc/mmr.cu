@@ -13,7 +13,8 @@ namespace {
 
 constexpr int kGreedyThreads = 1024;
 
-// candidates by id from the stored corpus -> fp32 matrix: the fp16 rows, or a float32 slot's x (what its search scores)
+// candidates by id from the stored corpus -> fp32 matrix: the fp16 rows, or a float32 / uint8 slot's x (what its search
+// scores)
 template <typename T>
 __global__ void mmr_gather_kernel(const T* rows, int d, int d_pad, int64_t n_rows, int64_t id_base,
                                   const int64_t* ids, int n, float* out) {
@@ -222,7 +223,10 @@ int sb_semantic_mmr(sb_ctx* ctx, int slot, const float* q, int32_t d, const floa
                "sb_semantic_mmr: dense slot %d is empty or has dimension %d != %d", slot, ix.d, d);
     if ((rc = ctx->misc3_dev.reserve(nd * 8))) return rc;
     SB_CUDA(cudaMemcpyAsync(ctx->misc3_dev.p, cand_ids, nd * 8, cudaMemcpyHostToDevice, st));
-    if (ix.rows32)
+    if (ix.rows8)
+      mmr_gather_kernel<uint8_t><<<n, 128, 0, st>>>(ix.rows8, ix.d, ix.d_pad, ix.n, ix.id_base,
+                                                    ctx->misc3_dev.as<int64_t>(), n, Cd);
+    else if (ix.rows32)
       mmr_gather_kernel<float><<<n, 128, 0, st>>>(ix.rows32, ix.d, ix.d_pad, ix.n, ix.id_base,
                                                   ctx->misc3_dev.as<int64_t>(), n, Cd);
     else

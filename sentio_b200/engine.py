@@ -88,28 +88,26 @@ class B200Engine:
 
     # ------------------------------------------------------------------ K1 dense
     METRICS = {"cosine": 0, "dot": 1, "euclid": 2}   # SB_METRIC_* (include/sentio_b200.h)
-    DATATYPES = {"float16": 0, "float32": 1}         # SB_STORAGE_*
+    DATATYPES = {"float16": 0, "float32": 1, "uint8": 2}   # SB_STORAGE_*
 
     def load_dense(self, vecs: np.ndarray, id_base: int = 0, slot: int = 0, metric: str = "cosine",
                    storage: str = "float16") -> None:
         """``metric``: "cosine" (default), "dot" or "euclid" -- the slot's distance (DESIGN.md K1e); every search,
         upsert and delete on the slot follows it.  Dot scores are <q, v>, Euclid scores the distance ||q - v||
-        (ascending).  ``storage``: "float16" (default; scores are exact on the stored fp16 representation) or
-        "float32" (the slot also keeps the input rows x, and every score is exact on x; DESIGN.md K1g)."""
+        (ascending).  ``storage``: "float16" (default; scores are exact on the stored fp16 representation), "float32"
+        (the slot also keeps the input rows x, and every score is exact on x; DESIGN.md K1g) or "uint8" (the slot keeps
+        only x, one byte per dimension; every value must be an integer in [0, 255], and every score is exact on x;
+        DESIGN.md K1i).  A ``uint8`` array crosses to the GPU at one byte per dimension."""
         m = self.METRICS.get(str(metric).lower())
         if m is None:
             raise ValueError(f"metric {metric!r} is not supported (cosine, dot or euclid)")
         st = self.DATATYPES.get(str(storage).lower())
         if st is None:
-            raise ValueError(f"storage {storage!r} is not supported (float16 or float32)")
+            raise ValueError(f"storage {storage!r} is not supported ({', '.join(self.DATATYPES)})")
         v = np.ascontiguousarray(vecs)
         if v.ndim != 2:
             raise ValueError("vecs must be [n, d]")
-        if v.dtype == np.float16:
-            dt = 1
-        else:
-            v = np.ascontiguousarray(v, dtype=np.float32)
-            dt = 0
+        v, dt = self._dense_rows(v, st)
         n, d = v.shape
         if st != 0:
             check(self._lib.sb_dense_load_storage(self._h, slot, _ptr(v), n, d, dt, int(id_base), m, st),
@@ -122,6 +120,16 @@ class B200Engine:
         self.dense_dim[slot] = d
         self.dense_count[slot] = n
 
+    @staticmethod
+    def _dense_rows(v: np.ndarray, storage: int):
+        """Rows as the ABI takes them: (array, SB_F32 / SB_F16 / SB_U8).  uint8 arrays stay one byte per dimension on a
+        uint8 slot (storage 2); everything else crosses as float16 or float32."""
+        if v.dtype == np.uint8 and storage == 2:
+            return v, 2
+        if v.dtype == np.float16:
+            return v, 1
+        return np.ascontiguousarray(v, dtype=np.float32), 0
+
     def dense_metric(self, slot: int = 0) -> str:
         """The slot's metric: "cosine", "dot" or "euclid"."""
         m = int(self._lib.sb_dense_metric(self._h, slot))
@@ -131,7 +139,7 @@ class B200Engine:
         return names[m]
 
     def dense_storage(self, slot: int = 0) -> str:
-        """The slot's storage datatype: "float16" or "float32"."""
+        """The slot's storage datatype: "float16", "float32" or "uint8"."""
         s = int(self._lib.sb_dense_storage(self._h, slot))
         names = {v: k for k, v in self.DATATYPES.items()}
         if s not in names:
@@ -175,10 +183,7 @@ class B200Engine:
         """Store ``vecs[i]`` at row ``rows[i]``: rows below the count overwrite, the others must be exactly count ..
         count + m - 1 (appends, any order).  Loaded tag columns read -1 on the written rows until ``dense_tags_write``."""
         r = np.ascontiguousarray(rows, dtype=np.int64).reshape(-1)
-        v = np.ascontiguousarray(vecs)
-        dt = 1 if v.dtype == np.float16 else 0
-        if dt == 0:
-            v = np.ascontiguousarray(v, dtype=np.float32)
+        v, dt = self._dense_rows(np.ascontiguousarray(vecs), self.DATATYPES[self.dense_storage(slot)])
         if v.ndim != 2 or v.shape[0] != len(r) or v.shape[1] != self.dense_dim.get(slot):
             raise ValueError(f"vecs must be [{len(r)}, {self.dense_dim.get(slot)}]")
         check(self._lib.sb_dense_upsert(self._h, slot, _ptr(r), _ptr(v), len(r), dt), "sb_dense_upsert")

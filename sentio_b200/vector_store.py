@@ -79,7 +79,8 @@ class Distance(enum.Enum):
 
 class Datatype(enum.Enum):
     """Qdrant's ``VectorParams.datatype``.  FLOAT16 keeps fp16 rows (scores exact on them); FLOAT32 also keeps the
-    vectors as given, and every score is exact on them (DESIGN.md K1g).  UINT8 is parsed so it can be refused by name."""
+    vectors as given, and every score is exact on them (DESIGN.md K1g); UINT8 keeps integer vectors in [0, 255] at one
+    byte per dimension, and every score is exact on them (DESIGN.md K1i)."""
     FLOAT32 = "float32"
     FLOAT16 = "float16"
     UINT8 = "uint8"
@@ -142,16 +143,28 @@ _ENGINE_METRIC = {Distance.COSINE: "cosine", Distance.DOT: "dot", Distance.EUCLI
 def parse_datatype(dt) -> Datatype:
     """A Qdrant vector datatype given as this module's ``Datatype``, ``qdrant_client``'s ``Datatype`` enum (read by
     ``.name``), its value or a plain string, case-insensitive ("float32", "FLOAT16", ...); ``None`` is FLOAT16, this
-    store's default.  UINT8 (quantised storage) raises ``ValueError``."""
+    store's default.  Any other datatype (int8, bfloat16, ...) raises ``ValueError``."""
     if dt is None:
         return Datatype.FLOAT16
     name = _distance_name(dt).strip().lower()
     for t in Datatype:
         if name in (t.name.lower(), t.value):
-            if t is Datatype.UINT8:
-                raise ValueError("datatype uint8 is not supported (supported: float32, float16)")
             return t
-    raise ValueError(f"datatype {_distance_name(dt)!r} is not supported (supported: float32, float16)")
+    raise ValueError(f"datatype {_distance_name(dt)!r} is not supported (supported: float32, float16, uint8)")
+
+
+def _uint8_rows(v: np.ndarray, where: str) -> np.ndarray:
+    """The vectors of a UINT8 collection as a uint8 array: every value must be an integer in [0, 255] (NaN, inf,
+    fractional and out-of-range values raise ``ValueError``; nothing is rounded)."""
+    if v.dtype == np.uint8:
+        return v
+    f = np.asarray(v, dtype=np.float64)
+    ok = np.isfinite(f) & (f >= 0.0) & (f <= 255.0)
+    ok &= np.floor(np.where(ok, f, 0.0)) == np.where(ok, f, 0.0)
+    if not ok.all():
+        bad = tuple(int(i) for i in np.argwhere(~ok)[0])
+        raise ValueError(f"{where}: a uint8 collection takes integers in [0, 255]; value {f[bad]!r} at {bad} is not one")
+    return f.astype(np.uint8)
 
 
 class _Collection:
@@ -245,8 +258,9 @@ class B200VectorStore:
         The distance is Cosine (the default without ``vectors_config``), Dot or Euclid (Qdrant's semantics: Dot scores
         <q, v>, Euclid scores the distance ||q - v|| and ranks it ascending); Manhattan raises ``ValueError``.
         ``vectors_config.datatype``: None or FLOAT16 (this store's default: fp16 rows) or FLOAT32 (the vectors are kept
-        as given and every score is exact on them, at 6 bytes per dimension per point in HBM); UINT8 raises
-        ``ValueError``."""
+        as given and every score is exact on them, at 6 bytes per dimension per point in HBM) or UINT8 (integer vectors
+        in [0, 255], 1 byte per dimension per point, every score exact on them; other values raise ``ValueError``).  A
+        datatype the engine class does not list in ``DATATYPES`` raises ``ValueError``."""
         dist = Distance.COSINE
         dtype = Datatype.FLOAT16
         if vectors_config is not None:
@@ -262,19 +276,23 @@ class B200VectorStore:
         # likewise DATATYPES: an engine without the table stores float16 only
         if dtype.value not in getattr(B200Engine, "DATATYPES", {"float16": 0}):
             raise ValueError(f"create_collection: datatype {dtype.value} is not supported by {B200Engine.__name__} "
-                             "(it stores float16 only)")
+                             f"(it stores {', '.join(getattr(B200Engine, 'DATATYPES', {'float16': 0}))})")
         if vectors is None:
             if vectors_config is None:
                 raise ValueError("create_collection: give vectors or vectors_config")
             vectors = np.zeros((0, int(vectors_config.size)), dtype=np.float32)
         vecs = np.asarray(vectors)
+        if dtype is Datatype.UINT8:
+            if vecs.ndim != 2:
+                raise ValueError("create_collection: vectors must be [n, d]")
+            vecs = _uint8_rows(vecs, "create_collection")
         n = vecs.shape[0]
         col = _Collection(collection_name, self._device)
         col.distance = dist
         col.datatype = dtype
         try:
-            if dtype is Datatype.FLOAT32:
-                col.engine.load_dense(vecs, id_base=0, slot=0, metric=_ENGINE_METRIC[dist], storage="float32")
+            if dtype in (Datatype.FLOAT32, Datatype.UINT8):
+                col.engine.load_dense(vecs, id_base=0, slot=0, metric=_ENGINE_METRIC[dist], storage=dtype.value)
             elif dist is Distance.COSINE:
                 col.engine.load_dense(vecs, id_base=0, slot=0)
             else:
@@ -354,6 +372,8 @@ class B200VectorStore:
             raise ValueError(f"upsert: vectors must have dimension {col.dim}, got shape {v.shape}")
         if not np.isfinite(v).all():
             raise ValueError("upsert: vectors contain NaN or infinite values")
+        if col.datatype is Datatype.UINT8:
+            v = _uint8_rows(v, "upsert")
         new_payloads = []
         for i in pick:
             p = pls[i]
@@ -413,7 +433,8 @@ class B200VectorStore:
                  **_ignored) -> list[Record]:
         """Points by id (unknown ids are skipped, as in Qdrant); vectors are the stored fp16 values, widened (Dot /
         Euclid: c * y, the input to the fp16 precision of its direction).  A FLOAT32 collection returns the vectors as
-        given (Cosine: normalised, x / ||x||), as Qdrant does."""
+        given (Cosine: normalised, x / ||x||), as Qdrant does.  A UINT8 collection returns its integer vectors as
+        given, for every distance (a normalised uint8 vector does not exist)."""
         col = self._get(collection_name)
         with col.lock:
             rows = [col.row_of[i] for i in ids if i in col.row_of]
