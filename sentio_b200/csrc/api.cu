@@ -16,6 +16,7 @@ void sb_set_error(const char* fmt, ...) {
 void ce_model_free(CeModel* m);        // cross_encoder.cu
 void ce_tokens_free(CeDocTokens* t);   // cross_encoder.cu
 void bm25_build_free(Bm25Build* b);    // bm25_build.cu
+void dense_free(DenseIndex& ix);       // dense.cu
 
 extern "C" {
 
@@ -62,18 +63,7 @@ void sb_destroy(sb_ctx* ctx) {
   if (!ctx) return;
   DeviceGuard g(ctx->device);
   cudaStreamSynchronize(ctx->stream);
-  for (int s = 0; s < SB_MAX_DENSE_SLOTS; ++s) {
-    if (ctx->dense[s].rows) cudaFree(ctx->dense[s].rows);
-    if (ctx->dense[s].inv_norm) cudaFree(ctx->dense[s].inv_norm);
-    if (ctx->dense[s].cfac) cudaFree(ctx->dense[s].cfac);
-    if (ctx->dense[s].hh) cudaFree(ctx->dense[s].hh);
-    if (ctx->dense[s].rows32) cudaFree(ctx->dense[s].rows32);
-    if (ctx->dense[s].rows8) cudaFree(ctx->dense[s].rows8);
-    for (int f = 0; f < SB_MAX_TAG_FIELDS; ++f)
-      if (ctx->dense[s].tags[f]) cudaFree(ctx->dense[s].tags[f]);
-    for (int f = 0; f < SB_MAX_VALUE_FIELDS; ++f)
-      if (ctx->dense[s].vals[f]) cudaFree(ctx->dense[s].vals[f]);
-  }
+  for (int s = 0; s < SB_MAX_DENSE_SLOTS; ++s) dense_free(ctx->dense[s]);
   Bm25Index& b = ctx->bm25;
   if (b.indptr) cudaFree(b.indptr);
   if (b.post_doc) cudaFree(b.post_doc);

@@ -157,54 +157,37 @@ __global__ void dense_store_rows8_kernel(const TIn* __restrict__ in, int64_t n_r
 
 // ------------------------------------------------------------------------------------------------ mutation kernels
 // sb_dense_delete's compaction: one warp per move from[m] -> to[m] (sources >= n - |D| > destinations, so one launch
-// has no read/write hazard): the fp16 row in 16-byte copies, its inverse norm, its code in every loaded tag column and
-// its value in every loaded value column.
+// has no read/write hazard) copies the row in every column of the slot (dense_columns): a row that is a multiple of
+// 16 bytes (the vectors) in 16-byte copies spread over the lanes, a 4- or 8-byte row by one lane.
+constexpr int kMaxDenseColumns = 5 + SB_MAX_TAG_FIELDS + SB_MAX_VALUE_FIELDS;
+
 struct MoveParams {
-  __half* rows;
-  float* inv_norm;
-  double* cfac;                       // Dot / Euclid, else nullptr
-  float* hh;                          // Euclid, else nullptr
-  float* rows32;                      // float32 storage, else nullptr
-  uint8_t* rows8;                     // uint8 storage (then rows is nullptr), else nullptr
-  int32_t* tags[SB_MAX_TAG_FIELDS];   // nullptr = field not loaded
-  double* vals[SB_MAX_VALUE_FIELDS];  // likewise
+  uint8_t* col[kMaxDenseColumns];
+  int32_t row_bytes[kMaxDenseColumns];
+  int32_t n_cols;
   const int64_t* from;
   const int64_t* to;
   int64_t n_moves;
-  int32_t ch;                         // 16-byte chunks per row = d_pad / 8
 };
 
-__global__ void __launch_bounds__(256) dense_move_rows_kernel(const MoveParams p) {
+__global__ void __launch_bounds__(256, 8) dense_move_rows_kernel(const __grid_constant__ MoveParams p) {
   const int64_t m = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (m >= p.n_moves) return;
   const int64_t s = p.from[m], t = p.to[m];
-  if (p.rows) {
-    const uint4* src = reinterpret_cast<const uint4*>(p.rows) + s * p.ch;
-    uint4* dst = reinterpret_cast<uint4*>(p.rows) + t * p.ch;
-    for (int c = lane; c < p.ch; c += 32) dst[c] = src[c];
+  for (int c = 0; c < p.n_cols; ++c) {
+    const int rb = p.row_bytes[c];
+    if (rb % 16) continue;
+    const uint4* src = reinterpret_cast<const uint4*>(p.col[c] + s * rb);
+    uint4* dst = reinterpret_cast<uint4*>(p.col[c] + t * rb);
+#pragma unroll 4   // the default unroll spills
+    for (int i = lane; i < rb / 16; i += 32) dst[i] = src[i];
   }
-  if (p.rows8) {   // the uint8 row: d_pad / 16 = ch / 2 16-byte chunks
-    const uint4* src8 = reinterpret_cast<const uint4*>(p.rows8) + s * (p.ch / 2);
-    uint4* dst8 = reinterpret_cast<uint4*>(p.rows8) + t * (p.ch / 2);
-    for (int c = lane; c < p.ch / 2; c += 32) dst8[c] = src8[c];
+  for (int c = lane; c < p.n_cols; c += 32) {
+    const int rb = p.row_bytes[c];
+    if (rb == 8) reinterpret_cast<uint64_t*>(p.col[c])[t] = reinterpret_cast<const uint64_t*>(p.col[c])[s];
+    else if (rb == 4) reinterpret_cast<uint32_t*>(p.col[c])[t] = reinterpret_cast<const uint32_t*>(p.col[c])[s];
   }
-  if (p.rows32) {   // the fp32 row: 2 * ch 16-byte chunks
-    const uint4* src32 = reinterpret_cast<const uint4*>(p.rows32) + s * 2 * p.ch;
-    uint4* dst32 = reinterpret_cast<uint4*>(p.rows32) + t * 2 * p.ch;
-    for (int c = lane; c < 2 * p.ch; c += 32) dst32[c] = src32[c];
-  }
-  if (lane == 0) {
-    p.inv_norm[t] = p.inv_norm[s];
-    if (p.cfac) p.cfac[t] = p.cfac[s];
-    if (p.hh) p.hh[t] = p.hh[s];
-  }
-#pragma unroll
-  for (int f = 0; f < SB_MAX_TAG_FIELDS; ++f)
-    if (lane == f + 1 && p.tags[f] != nullptr) p.tags[f][t] = p.tags[f][s];
-#pragma unroll
-  for (int f = 0; f < SB_MAX_VALUE_FIELDS; ++f)
-    if (lane == f + 16 && p.vals[f] != nullptr) p.vals[f][t] = p.vals[f][s];
 }
 
 // codes[i] -> col[rows[i]]; codes == nullptr writes -1 (an upserted row's payload is unknown until its codes arrive)
@@ -629,21 +612,15 @@ struct MergeParams {
   int32_t kprime;
   int32_t heads_per_list;    // R = ceil(kprime / G)
   int32_t heads_pow2;        // power of two >= G * R  (<= kSelCap)
-  const __half* rows;
+  SlotView slot;
   const float* q;            // [nq][d_pad] the caller's fp32 queries (exact stage)
   const float* eps;          // [nq] error bound of the approximate scores (0 for an all-zero query)
   int32_t* fallback;         // [nq] raised when the lists cannot serve the window
-  int32_t d_pad;
-  int32_t ch;
-  int64_t id_base;
   int32_t k;
   int64_t* out_ids;          // [nq][k]
   double* out_scores;        // [nq][k]
   int32_t* out_counts;       // [nq]
   const int32_t* state;      // FILTER only: [nq] 1 = answered by the gather path (nothing to merge)
-  int32_t metric;
-  const double* cfac;
-  const float* rows32;       // F32 only
 };
 
 __device__ __forceinline__ void block_sort_desc_u64(unsigned long long* a, int len, int tid, int nt) {
@@ -729,20 +706,8 @@ __global__ void __launch_bounds__(kMergeThreads, 1) dense_merge_kernel(const Mer
   int P = 32;
   while (P < nsel) P <<= 1;
 
-  RescoreArgs ra;
-  ra.rows = p.rows;
-  ra.q = p.q + (size_t)qi * p.d_pad;
-  ra.d_pad = p.d_pad;
-  ra.ch = p.ch;
-  ra.id_base = p.id_base;
-  ra.k = p.k;
-  ra.out_ids = p.out_ids + (size_t)qi * p.k;
-  ra.out_scores = p.out_scores + (size_t)qi * p.k;
-  ra.out_count = p.out_counts + qi;
-  ra.metric = p.metric;
-  ra.cfac = p.cfac;
-  ra.rows32 = p.rows32;
-  ra.rows8 = nullptr;
+  const RescoreArgs ra{p.slot, p.q + (size_t)qi * p.slot.d_pad, p.k, p.out_ids + (size_t)qi * p.k,
+                       p.out_scores + (size_t)qi * p.k, p.out_counts + qi};
   rescore_and_emit<F32 ? SB_STORAGE_F32 : SB_STORAGE_F16>(sel, nsel, P, ek, ei, &qq_s, q_s, ra);
 }
 
@@ -850,11 +815,9 @@ constexpr int kFbBest = 1024;  // >= the largest supported k
 
 struct FallbackParams {
   const int32_t* flag;   // [nq]
-  const __half* rows;
+  SlotView slot;
   const float* q;        // [nq][d_pad]
   int64_t n;
-  int32_t d_pad, ch;
-  int64_t id_base;
   int32_t k;
   int64_t* out_ids;
   double* out_scores;
@@ -862,10 +825,6 @@ struct FallbackParams {
   unsigned long long* counter;   // [1] queries answered here since the context was created
   const uint32_t* mask;          // FILTER only: match bits, mask[(row / 32) * mask_qs + query]
   int32_t mask_qs;
-  int32_t metric;
-  const double* cfac;
-  const float* rows32;           // float32 storage only
-  const uint8_t* rows8;          // uint8 storage only
 };
 
 template <bool FILTER, int ST>
@@ -878,10 +837,10 @@ __global__ void __launch_bounds__(kFbThreads, 1) dense_exact_fallback_kernel(con
   __shared__ int s_beats;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nt = blockDim.x, nw = nt >> 5;
   if (tid == 0) atomicAdd(p.counter, 1ull);
-  const float* q = p.q + (size_t)qi * p.d_pad;
-  const double qn = query_norm_cta(q, p.d_pad, &qq_s);
+  const float* q = p.q + (size_t)qi * p.slot.d_pad;
+  const double qn = query_norm_cta(q, p.slot.d_pad, &qq_s);
   // Cosine / Dot: the all-zero query scores 0 on every row.  Euclid: it does not (the nearest rows are the smallest).
-  const bool zero_shortcut = !(qn > 0.0) && p.metric != SB_METRIC_EUCLID;
+  const bool zero_shortcut = !(qn > 0.0) && p.slot.metric != SB_METRIC_EUCLID;
   if (FILTER && zero_shortcut) {
     // all-zero query: every cosine is 0 -> the first k MATCHING rows in index order (one warp walks the mask words)
     if (warp != 0) return;
@@ -899,7 +858,7 @@ __global__ void __launch_bounds__(kFbThreads, 1) dense_exact_fallback_kernel(con
       for (int pos = got + incl - c; bits != 0u && pos < p.k; ++pos) {
         const int b = __ffs(bits) - 1;
         bits &= bits - 1u;
-        p.out_ids[(size_t)qi * p.k + pos] = p.id_base + w * 32 + b;
+        p.out_ids[(size_t)qi * p.k + pos] = p.slot.id_base + w * 32 + b;
         p.out_scores[(size_t)qi * p.k + pos] = 0.0;
       }
       got += __shfl_sync(0xffffffffu, incl, 31);
@@ -916,7 +875,7 @@ __global__ void __launch_bounds__(kFbThreads, 1) dense_exact_fallback_kernel(con
     // all-zero query: every cosine is exactly 0 -> the first k rows in index order, no scan needed
     const int m = (int)min((int64_t)p.k, p.n);
     for (int i = tid; i < p.k; i += nt) {
-      p.out_ids[(size_t)qi * p.k + i] = i < m ? p.id_base + i : -1;
+      p.out_ids[(size_t)qi * p.k + i] = i < m ? p.slot.id_base + i : -1;
       p.out_scores[(size_t)qi * p.k + i] = 0.0;
     }
     if (tid == 0) p.out_counts[qi] = m;
@@ -939,8 +898,7 @@ __global__ void __launch_bounds__(kFbThreads, 1) dense_exact_fallback_kernel(con
       if constexpr (FILTER)
         if (row < p.n) match = (p.mask[(size_t)(row >> 5) * p.mask_qs + qi] >> (row & 31)) & 1u;
       if (row < p.n && match) {
-        okey = f64_orderable(
-            exact_key_row<ST>(p.metric, p.rows, p.cfac, p.rows32, p.rows8, (uint32_t)row, q, p.d_pad, p.ch, qn, lane));
+        okey = f64_orderable(exact_key_row<ST>(p.slot, (uint32_t)row, q, qn, lane));
         if (okey == 0ull) okey = 1ull;
       }
       if (lane == 0) {
@@ -954,18 +912,7 @@ __global__ void __launch_bounds__(kFbThreads, 1) dense_exact_fallback_kernel(con
     if (s_beats) sort_exact_pairs(ek, ei, 2 * kFbBest, tid, nt);
     __syncthreads();
   }
-  RescoreArgs ra;
-  ra.rows = p.rows;
-  ra.q = q;
-  ra.d_pad = p.d_pad;
-  ra.ch = p.ch;
-  ra.id_base = p.id_base;
-  ra.k = p.k;
-  ra.out_ids = p.out_ids + (size_t)qi * p.k;
-  ra.out_scores = p.out_scores + (size_t)qi * p.k;
-  ra.out_count = p.out_counts + qi;
-  ra.metric = p.metric;
-  ra.cfac = p.cfac;
+  const RescoreArgs ra{p.slot, q, p.k, p.out_ids + (size_t)qi * p.k, p.out_scores + (size_t)qi * p.k, p.out_counts + qi};
   emit_exact_pairs(ek, ei, kFbBest, ra);
 }
 
@@ -1111,18 +1058,12 @@ struct GatherParams {
   int32_t qs;
   int64_t n_words;
   const int32_t* qlist;      // [grid] chunk-local query index of each CTA
-  const __half* rows;
+  SlotView slot;
   const float* q;            // [nq][d_pad] the caller's fp32 queries
-  int32_t d_pad, ch;
-  int64_t id_base;
   int32_t k;
   int64_t* out_ids;
   double* out_scores;
   int32_t* out_counts;
-  int32_t metric;
-  const double* cfac;
-  const float* rows32;       // float32 storage only
-  const uint8_t* rows8;      // uint8 storage only
 };
 
 template <int ST>
@@ -1148,20 +1089,8 @@ __global__ void __launch_bounds__(kMergeThreads, 1) dense_filter_gather_kernel(c
   const int nsel = min(s_n, kGatherMax);   // the host routes only queries with <= kGatherMax matches here
   int P = 32;
   while (P < nsel) P <<= 1;
-  RescoreArgs ra;
-  ra.rows = p.rows;
-  ra.q = p.q + (size_t)qi * p.d_pad;
-  ra.d_pad = p.d_pad;
-  ra.ch = p.ch;
-  ra.id_base = p.id_base;
-  ra.k = p.k;
-  ra.out_ids = p.out_ids + (size_t)qi * p.k;
-  ra.out_scores = p.out_scores + (size_t)qi * p.k;
-  ra.out_count = p.out_counts + qi;
-  ra.metric = p.metric;
-  ra.cfac = p.cfac;
-  ra.rows32 = p.rows32;
-  ra.rows8 = p.rows8;
+  const RescoreArgs ra{p.slot, p.q + (size_t)qi * p.slot.d_pad, p.k, p.out_ids + (size_t)qi * p.k,
+                       p.out_scores + (size_t)qi * p.k, p.out_counts + qi};
   rescore_and_emit<ST>(sel, nsel, P, ek, ei, &qq_s, q_s, ra);
 }
 
@@ -1426,7 +1355,7 @@ int dense_topk_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int B, i
   float *qn = nullptr, *eps = nullptr, *rq = nullptr;
   int32_t* fb = nullptr;
   if ((rc = dense_prep_queries(ctx, ix, q_pad, B, B, /*mma=*/false, &qn, nullptr, &eps, &fb, &rq, st))) return rc;
-  const bool f32 = ix.rows32 != nullptr;
+  const bool f32 = ix.storage == SB_STORAGE_F32;
   auto merge_kern = flt ? (f32 ? dense_merge_kernel<true, true> : dense_merge_kernel<true, false>)
                         : (f32 ? dense_merge_kernel<false, true> : dense_merge_kernel<false, false>);
   SB_CUDA(cudaFuncSetAttribute(merge_kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.merge_smem));
@@ -1475,21 +1404,15 @@ int dense_topk_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int B, i
     mp.kprime = pl.kprime;
     mp.heads_per_list = pl.heads_per_list;
     mp.heads_pow2 = pl.heads_pow2;
-    mp.rows = ix.rows;
+    mp.slot = slot_view(ix);
     mp.q = q_pad + (size_t)c0 * ix.d_pad;
     mp.eps = eps + c0;
     mp.fallback = fb + c0;
-    mp.d_pad = ix.d_pad;
-    mp.ch = ix.d_pad / 8;
-    mp.id_base = ix.id_base;
     mp.k = k;
     mp.out_ids = out_ids + (size_t)c0 * k;
     mp.out_scores = out_scores + (size_t)c0 * k;
     mp.out_counts = out_counts + c0;
     mp.state = flt ? flt->state + c0 : nullptr;
-    mp.metric = ix.metric;
-    mp.cfac = ix.cfac;
-    mp.rows32 = ix.rows32;
     {
       ProfScope ps(ctx, SB_PROF_DENSE_MERGE, st);
       merge_kern<<<nq, kMergeThreads, pl.merge_smem, st>>>(mp);
@@ -1590,7 +1513,7 @@ int dense_prep_queries(sb_ctx* ctx, const DenseIndex& ix, const float* q_pad, in
   ctx->launches += 1;
   if (ix.storage == SB_STORAGE_U8)
     dense_prep_queries_kernel<SB_STORAGE_U8><<<rows, 256, 0, st>>>(q_pad, B, ix.d_pad, qn, q16, eps, mma ? 1 : 0, pm);
-  else if (ix.rows32)
+  else if (ix.storage == SB_STORAGE_F32)
     dense_prep_queries_kernel<SB_STORAGE_F32><<<rows, 256, 0, st>>>(q_pad, B, ix.d_pad, qn, q16, eps, mma ? 1 : 0, pm);
   else
     dense_prep_queries_kernel<SB_STORAGE_F16><<<rows, 256, 0, st>>>(q_pad, B, ix.d_pad, qn, q16, eps, mma ? 1 : 0, pm);
@@ -1613,20 +1536,13 @@ int dense_fallback_enqueue(sb_ctx* ctx, const DenseIndex& ix, const float* q_pad
   fp.mask = flt ? flt->mask : nullptr;
   fp.mask_qs = flt ? flt->qs : 0;
   fp.flag = fb;
-  fp.rows = ix.rows;
+  fp.slot = slot_view(ix);
   fp.q = q_pad;
   fp.n = ix.n;
-  fp.d_pad = ix.d_pad;
-  fp.ch = ix.d_pad / 8;
-  fp.id_base = ix.id_base;
   fp.k = k;
   fp.out_ids = out_ids;
   fp.out_scores = out_scores;
   fp.out_counts = out_counts;
-  fp.metric = ix.metric;
-  fp.cfac = ix.cfac;
-  fp.rows32 = ix.rows32;
-  fp.rows8 = ix.rows8;
   ctx->launches += 1;
   auto kern = flt ? dense_exact_fallback_kernel<true, SB_STORAGE_F16> : dense_exact_fallback_kernel<false, SB_STORAGE_F16>;
   if (ix.storage == SB_STORAGE_F32)
@@ -1906,19 +1822,12 @@ int dense_topk_where_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, in
       gp.qs = qs;
       gp.n_words = n_words;
       gp.qlist = qlist_d;
-      gp.rows = ix.rows;
+      gp.slot = slot_view(ix);
       gp.q = qc;
-      gp.d_pad = ix.d_pad;
-      gp.ch = ix.d_pad / 8;
-      gp.id_base = ix.id_base;
       gp.k = k;
       gp.out_ids = oi;
       gp.out_scores = os;
       gp.out_counts = oc;
-      gp.metric = ix.metric;
-      gp.cfac = ix.cfac;
-      gp.rows32 = ix.rows32;
-      gp.rows8 = ix.rows8;
       ProfScope ps(ctx, SB_PROF_DENSE_GATHER, st);
       gather_kern<<<n_gather, kMergeThreads, gather_smem, st>>>(gp);
     }
@@ -2190,12 +2099,12 @@ int dense_store_staged(sb_ctx* ctx, DenseIndex& ix, const void* vecs, int64_t n,
                        int64_t row0, double* sigma) {
   const int d = ix.d;
   const size_t esz = dtype == SB_F32 ? 4 : dtype == SB_U8 ? 1 : 2;
-  const bool u8 = ix.storage == SB_STORAGE_U8;
+  const bool u8 = ix.storage == SB_STORAGE_U8, f32 = ix.storage == SB_STORAGE_F32;
   const int64_t chunk_rows = std::max<int64_t>(1, (int64_t)((256ull << 20) / ((size_t)d * esz)));
   int rc = ctx->misc_dev.reserve((size_t)std::min<int64_t>(chunk_rows, n) * d * esz);
   if (rc) return rc;
   unsigned long long* sigma_bits = nullptr;
-  if (ix.rows32 || u8) {
+  if (f32 || u8) {
     if ((rc = ctx->sigma_dev.reserve(8))) return rc;
     sigma_bits = ctx->sigma_dev.as<unsigned long long>();
     SB_CUDA(cudaMemsetAsync(sigma_bits, 0, 8, ctx->stream));
@@ -2227,7 +2136,7 @@ int dense_store_staged(sb_ctx* ctx, DenseIndex& ix, const void* vecs, int64_t n,
                                                                             ix.rows, ix.inv_norm, row0 + r0, dst,
                                                                             ix.cfac != nullptr, ix.cfac, ix.hh);
     SB_CUDA(cudaGetLastError());
-    if (ix.rows32) {
+    if (f32) {
       if (dtype == SB_F32)
         dense_store_rows32_kernel<float><<<blocks, wpb * 32, 0, ctx->stream>>>(
             ctx->misc_dev.as<float>(), nr, d, ix.d_pad, ix.rows, ix.rows32, row0 + r0, dst, ix.cfac, sigma_bits);
@@ -2248,98 +2157,84 @@ int dense_store_staged(sb_ctx* ctx, DenseIndex& ix, const void* vecs, int64_t n,
   return SB_OK;
 }
 
-// Reallocate rows / inv_norm / cfac / hh / every loaded tag and value column to n_cap rows (> ix.n_cap): the [0, n_pad)
-// prefix is copied device to device, the rest is zero (tags -1, values NaN).  Old and new buffers coexist during the copy.
+// One per-row device column of a slot: the address of its pointer field in DenseIndex, its bytes per row and the byte
+// its unused capacity [n, n_cap) holds.
+struct DenseColumn {
+  void** ptr;
+  int32_t row_bytes;
+  int fill;
+};
+
+template <typename T>
+DenseColumn column(T*& field, int32_t row_bytes, int fill) {
+  return {reinterpret_cast<void**>(&field), row_bytes, fill};
+}
+DenseColumn tag_column(DenseIndex& ix, int f) { return column(ix.tags[f], 4, 0xff); }     // code -1
+DenseColumn value_column(DenseIndex& ix, int f) { return column(ix.vals[f], 8, 0xff); }   // NaN
+
+// The columns a slot has, from its storage, metric and loaded payload fields.  Every one spans n_cap rows (a payload
+// column loaded on an empty slot: 1 row).  Returns their count (<= kMaxDenseColumns).
+int dense_columns(DenseIndex& ix, DenseColumn* out) {
+  int n = 0;
+  if (ix.storage == SB_STORAGE_U8) out[n++] = column(ix.rows8, ix.d_pad, 0);
+  else out[n++] = column(ix.rows, 2 * ix.d_pad, 0);
+  if (ix.storage == SB_STORAGE_F32) out[n++] = column(ix.rows32, 4 * ix.d_pad, 0);
+  out[n++] = column(ix.inv_norm, 4, 0);
+  if (ix.metric != SB_METRIC_COSINE && ix.storage != SB_STORAGE_U8) out[n++] = column(ix.cfac, 8, 0);
+  if (ix.metric == SB_METRIC_EUCLID) out[n++] = column(ix.hh, 4, 0);
+  for (int f = 0; f < SB_MAX_TAG_FIELDS; ++f)
+    if (ix.tags[f]) out[n++] = tag_column(ix, f);
+  for (int f = 0; f < SB_MAX_VALUE_FIELDS; ++f)
+    if (ix.vals[f]) out[n++] = value_column(ix, f);
+  return n;
+}
+
+// *p = `rows` rows of column c, rows [from, rows) filled (stream-ordered on st)
+cudaError_t column_alloc(const DenseColumn& c, void** p, int64_t rows, int64_t from, cudaStream_t st) {
+  cudaError_t e = cudaMalloc(p, (size_t)rows * c.row_bytes);
+  if (e != cudaSuccess) return e;
+  return cudaMemsetAsync(static_cast<uint8_t*>(*p) + (size_t)from * c.row_bytes, c.fill,
+                         (size_t)(rows - from) * c.row_bytes, st);
+}
+
+// Reallocate every column to n_cap rows (> ix.n_cap): the [0, n_pad) prefix is copied device to device, the rest is
+// filled.  The old buffers stay valid until every new one is complete; on failure the slot is unchanged.
 int dense_grow(sb_ctx* ctx, DenseIndex& ix, int64_t n_cap) {
-  const bool u8 = ix.storage == SB_STORAGE_U8;   // rows8 instead of rows
-  const size_t rb = (size_t)ix.d_pad * (u8 ? 1 : sizeof(__half));
-  __half* rows = nullptr;
-  uint8_t* rows8 = nullptr;
-  float* inv = nullptr;
-  double* cfac = nullptr;
-  float* hh = nullptr;
-  float* rows32 = nullptr;
-  const size_t rb32 = (size_t)ix.d_pad * sizeof(float);
-  int32_t* tags[SB_MAX_TAG_FIELDS] = {};
-  double* vals[SB_MAX_VALUE_FIELDS] = {};
-  cudaError_t e = u8 ? cudaMalloc(&rows8, (size_t)n_cap * rb) : cudaMalloc(&rows, (size_t)n_cap * rb);
-  if (e == cudaSuccess) e = cudaMalloc(&inv, (size_t)n_cap * sizeof(float));
-  if (e == cudaSuccess && ix.metric != SB_METRIC_COSINE && !u8) e = cudaMalloc(&cfac, (size_t)n_cap * sizeof(double));
-  if (e == cudaSuccess && ix.metric == SB_METRIC_EUCLID) e = cudaMalloc(&hh, (size_t)n_cap * sizeof(float));
-  if (e == cudaSuccess && ix.storage == SB_STORAGE_F32) e = cudaMalloc(&rows32, (size_t)n_cap * rb32);
-  for (int f = 0; f < SB_MAX_TAG_FIELDS && e == cudaSuccess; ++f)
-    if (ix.tags[f]) e = cudaMalloc(&tags[f], (size_t)n_cap * 4);
-  for (int f = 0; f < SB_MAX_VALUE_FIELDS && e == cudaSuccess; ++f)
-    if (ix.vals[f]) e = cudaMalloc(&vals[f], (size_t)n_cap * 8);
+  DenseColumn col[kMaxDenseColumns];
+  const int nc = dense_columns(ix, col);
+  void* fresh[kMaxDenseColumns] = {};
   const int64_t keep = ix.n_pad;
   cudaStream_t st = ctx->stream;
-  uint8_t* rows_b = u8 ? rows8 : reinterpret_cast<uint8_t*>(rows);   // the row buffer, as bytes
-  const void* old_b = u8 ? (const void*)ix.rows8 : (const void*)ix.rows;
-  if (e == cudaSuccess && keep) e = cudaMemcpyAsync(rows_b, old_b, (size_t)keep * rb, cudaMemcpyDeviceToDevice, st);
-  if (e == cudaSuccess && keep)
-    e = cudaMemcpyAsync(inv, ix.inv_norm, (size_t)keep * sizeof(float), cudaMemcpyDeviceToDevice, st);
-  if (e == cudaSuccess) e = cudaMemsetAsync(rows_b + (size_t)keep * rb, 0, (size_t)(n_cap - keep) * rb, st);
-  if (e == cudaSuccess) e = cudaMemsetAsync(inv + keep, 0, (size_t)(n_cap - keep) * sizeof(float), st);
-  if (cfac) {
+  cudaError_t e = cudaSuccess;
+  for (int i = 0; i < nc && e == cudaSuccess; ++i) {
+    e = column_alloc(col[i], &fresh[i], n_cap, keep, st);
     if (e == cudaSuccess && keep)
-      e = cudaMemcpyAsync(cfac, ix.cfac, (size_t)keep * sizeof(double), cudaMemcpyDeviceToDevice, st);
-    if (e == cudaSuccess) e = cudaMemsetAsync(cfac + keep, 0, (size_t)(n_cap - keep) * sizeof(double), st);
-  }
-  if (hh) {
-    if (e == cudaSuccess && keep) e = cudaMemcpyAsync(hh, ix.hh, (size_t)keep * sizeof(float), cudaMemcpyDeviceToDevice, st);
-    if (e == cudaSuccess) e = cudaMemsetAsync(hh + keep, 0, (size_t)(n_cap - keep) * sizeof(float), st);
-  }
-  if (rows32) {
-    if (e == cudaSuccess && keep) e = cudaMemcpyAsync(rows32, ix.rows32, (size_t)keep * rb32, cudaMemcpyDeviceToDevice, st);
-    if (e == cudaSuccess) e = cudaMemsetAsync(rows32 + (size_t)keep * ix.d_pad, 0, (size_t)(n_cap - keep) * rb32, st);
-  }
-  for (int f = 0; f < SB_MAX_TAG_FIELDS && e == cudaSuccess; ++f) {
-    if (!tags[f]) continue;
-    if (keep) e = cudaMemcpyAsync(tags[f], ix.tags[f], (size_t)keep * 4, cudaMemcpyDeviceToDevice, st);
-    if (e == cudaSuccess) e = cudaMemsetAsync(tags[f] + keep, 0xff, (size_t)(n_cap - keep) * 4, st);
-  }
-  for (int f = 0; f < SB_MAX_VALUE_FIELDS && e == cudaSuccess; ++f) {
-    if (!vals[f]) continue;
-    if (keep) e = cudaMemcpyAsync(vals[f], ix.vals[f], (size_t)keep * 8, cudaMemcpyDeviceToDevice, st);
-    if (e == cudaSuccess) e = cudaMemsetAsync(vals[f] + keep, 0xff, (size_t)(n_cap - keep) * 8, st);
+      e = cudaMemcpyAsync(fresh[i], *col[i].ptr, (size_t)keep * col[i].row_bytes, cudaMemcpyDeviceToDevice, st);
   }
   if (e == cudaSuccess) e = cudaStreamSynchronize(st);
   if (e != cudaSuccess) {   // the slot keeps its old buffers; the new ones are released on every failure
     cudaStreamSynchronize(st);
-    cudaFree(rows);
-    cudaFree(rows8);
-    cudaFree(inv);
-    cudaFree(cfac);
-    cudaFree(hh);
-    cudaFree(rows32);
-    for (int f = 0; f < SB_MAX_TAG_FIELDS; ++f) cudaFree(tags[f]);
-    for (int f = 0; f < SB_MAX_VALUE_FIELDS; ++f) cudaFree(vals[f]);
+    for (int i = 0; i < nc; ++i) cudaFree(fresh[i]);
     sb_set_error("dense: growing slot to %lld rows failed: %s", (long long)n_cap, cudaGetErrorString(e));
     return SB_ERR_CUDA;
   }
-  cudaFree(ix.rows);
-  cudaFree(ix.rows8);
-  cudaFree(ix.inv_norm);
-  cudaFree(ix.cfac);
-  cudaFree(ix.hh);
-  cudaFree(ix.rows32);
-  ix.rows = rows;
-  ix.rows8 = rows8;
-  ix.inv_norm = inv;
-  ix.cfac = cfac;
-  ix.hh = hh;
-  ix.rows32 = rows32;
-  for (int f = 0; f < SB_MAX_TAG_FIELDS; ++f)
-    if (ix.tags[f]) {
-      cudaFree(ix.tags[f]);
-      ix.tags[f] = tags[f];
-    }
-  for (int f = 0; f < SB_MAX_VALUE_FIELDS; ++f)
-    if (ix.vals[f]) {
-      cudaFree(ix.vals[f]);
-      ix.vals[f] = vals[f];
-    }
+  for (int i = 0; i < nc; ++i) {
+    cudaFree(*col[i].ptr);
+    *col[i].ptr = fresh[i];
+  }
   ix.n_cap = n_cap;
+  return SB_OK;
+}
+
+// (Re)load payload column c with rows[0, n) (n = the slot's row count).  It spans the slot's capacity, at least one
+// row, so upserts and deletes never reallocate it alone.
+int dense_payload_load(sb_ctx* ctx, DenseIndex& ix, const DenseColumn& c, const void* rows, int64_t n) {
+  SB_CUDA(cudaStreamSynchronize(ctx->stream));
+  cudaFree(*c.ptr);
+  *c.ptr = nullptr;
+  SB_CUDA(column_alloc(c, c.ptr, std::max<int64_t>(ix.n_cap, 1), n, ctx->stream));
+  if (n) SB_CUDA(cudaMemcpyAsync(*c.ptr, rows, (size_t)n * c.row_bytes, cudaMemcpyHostToDevice, ctx->stream));
+  SB_CUDA(cudaStreamSynchronize(ctx->stream));
   return SB_OK;
 }
 
@@ -2413,6 +2308,13 @@ void u8_norm_bounds(int metric, double xx, double* rho, double* hmax) {
 
 }  // namespace
 
+// Frees every column of the slot (sb_dense_load, sb_destroy).
+void dense_free(DenseIndex& ix) {
+  DenseColumn col[kMaxDenseColumns];
+  const int nc = dense_columns(ix, col);
+  for (int i = 0; i < nc; ++i) cudaFree(*col[i].ptr);
+}
+
 // Shared with other translation units (hybrid batch path, scorers).
 int sb_dense_pad_queries(sb_ctx* ctx, const DenseIndex& ix, const float* q, int B, bool q_on_device, float** q_pad_out,
                          cudaStream_t st) {
@@ -2456,16 +2358,7 @@ int sb_dense_load_storage(sb_ctx* ctx, int slot, const void* vecs, int64_t n, in
   DeviceGuard g(ctx->device);
   DenseIndex& ix = ctx->dense[slot];
   SB_CUDA(cudaStreamSynchronize(ctx->stream));
-  if (ix.rows) cudaFree(ix.rows);
-  if (ix.inv_norm) cudaFree(ix.inv_norm);
-  if (ix.cfac) cudaFree(ix.cfac);
-  if (ix.hh) cudaFree(ix.hh);
-  if (ix.rows32) cudaFree(ix.rows32);
-  if (ix.rows8) cudaFree(ix.rows8);
-  for (int f = 0; f < SB_MAX_TAG_FIELDS; ++f)
-    if (ix.tags[f]) cudaFree(ix.tags[f]);
-  for (int f = 0; f < SB_MAX_VALUE_FIELDS; ++f)
-    if (ix.vals[f]) cudaFree(ix.vals[f]);
+  dense_free(ix);   // payload columns included: a load drops them
   ix = DenseIndex();
   ix.n = n;
   ix.d = d;
@@ -2476,29 +2369,11 @@ int sb_dense_load_storage(sb_ctx* ctx, int slot, const void* vecs, int64_t n, in
   ix.storage = storage;
   ix.rho_max = rho;
   ix.h_max = hmax;
-  if (n == 0) return SB_OK;   // an empty float32 / uint8 slot gets rows32 / rows8 with its first growth
+  if (n == 0) return SB_OK;   // an empty slot allocates nothing: its first growth allocates every column
   ix.n_cap = ix.n_pad;
-  if (u8) {
-    SB_CUDA(cudaMalloc(&ix.rows8, (size_t)ix.n_cap * ix.d_pad));
-    SB_CUDA(cudaMemsetAsync(ix.rows8, 0, (size_t)ix.n_cap * ix.d_pad, ctx->stream));
-  } else {
-    SB_CUDA(cudaMalloc(&ix.rows, (size_t)ix.n_cap * ix.d_pad * sizeof(__half)));
-    SB_CUDA(cudaMemsetAsync(ix.rows, 0, (size_t)ix.n_cap * ix.d_pad * sizeof(__half), ctx->stream));
-  }
-  SB_CUDA(cudaMalloc(&ix.inv_norm, (size_t)ix.n_cap * sizeof(float)));
-  SB_CUDA(cudaMemsetAsync(ix.inv_norm, 0, (size_t)ix.n_cap * sizeof(float), ctx->stream));
-  if (metric != SB_METRIC_COSINE && !u8) {
-    SB_CUDA(cudaMalloc(&ix.cfac, (size_t)ix.n_cap * sizeof(double)));
-    SB_CUDA(cudaMemsetAsync(ix.cfac, 0, (size_t)ix.n_cap * sizeof(double), ctx->stream));
-  }
-  if (metric == SB_METRIC_EUCLID) {
-    SB_CUDA(cudaMalloc(&ix.hh, (size_t)ix.n_cap * sizeof(float)));
-    SB_CUDA(cudaMemsetAsync(ix.hh, 0, (size_t)ix.n_cap * sizeof(float), ctx->stream));
-  }
-  if (storage == SB_STORAGE_F32) {
-    SB_CUDA(cudaMalloc(&ix.rows32, (size_t)ix.n_cap * ix.d_pad * sizeof(float)));
-    SB_CUDA(cudaMemsetAsync(ix.rows32, 0, (size_t)ix.n_cap * ix.d_pad * sizeof(float), ctx->stream));
-  }
+  DenseColumn col[kMaxDenseColumns];
+  const int nc = dense_columns(ix, col);
+  for (int i = 0; i < nc; ++i) SB_CUDA(column_alloc(col[i], col[i].ptr, ix.n_cap, 0, ctx->stream));
   if (u8) {
     double xx = 0.0;
     int rc = dense_store_staged(ctx, ix, vecs, n, dtype, nullptr, 0, &xx);
@@ -2660,40 +2535,29 @@ int sb_dense_delete(sb_ctx* ctx, int slot, const int64_t* rows, int64_t n, int64
   }
   *n_moved = mv;
   SB_CUDA(cudaDeviceSynchronize());   // searches enqueued on other streams may still read the rows that move
+  DenseColumn col[kMaxDenseColumns];
+  const int nc = dense_columns(ix, col);
   if (mv) {
     if ((rc = ctx->misc2_dev.reserve((size_t)mv * 16))) return rc;
     int64_t* f_dev = ctx->misc2_dev.as<int64_t>();
     SB_CUDA(cudaMemcpyAsync(f_dev, moved_from, (size_t)mv * 8, cudaMemcpyHostToDevice, ctx->stream));
     SB_CUDA(cudaMemcpyAsync(f_dev + mv, moved_to, (size_t)mv * 8, cudaMemcpyHostToDevice, ctx->stream));
     MoveParams mp;
-    mp.rows = ix.rows;
-    mp.inv_norm = ix.inv_norm;
-    mp.cfac = ix.cfac;
-    mp.hh = ix.hh;
-    mp.rows32 = ix.rows32;
-    mp.rows8 = ix.rows8;
-    memcpy(mp.tags, ix.tags, sizeof(mp.tags));
-    memcpy(mp.vals, ix.vals, sizeof(mp.vals));
+    for (int i = 0; i < nc; ++i) {
+      mp.col[i] = static_cast<uint8_t*>(*col[i].ptr);
+      mp.row_bytes[i] = col[i].row_bytes;
+    }
+    mp.n_cols = nc;
     mp.from = f_dev;
     mp.to = f_dev + mv;
     mp.n_moves = mv;
-    mp.ch = ix.d_pad / 8;
     dense_move_rows_kernel<<<(unsigned)((mv + 7) / 8), 256, 0, ctx->stream>>>(mp);
     SB_CUDA(cudaGetLastError());
   }
-  // the vacated tail [keep, n) returns to the zero state of unused capacity
-  if (ix.rows)
-    SB_CUDA(cudaMemsetAsync(ix.rows + (size_t)keep * ix.d_pad, 0, (size_t)n * ix.d_pad * sizeof(__half), ctx->stream));
-  if (ix.rows8) SB_CUDA(cudaMemsetAsync(ix.rows8 + (size_t)keep * ix.d_pad, 0, (size_t)n * ix.d_pad, ctx->stream));
-  SB_CUDA(cudaMemsetAsync(ix.inv_norm + keep, 0, (size_t)n * sizeof(float), ctx->stream));
-  if (ix.cfac) SB_CUDA(cudaMemsetAsync(ix.cfac + keep, 0, (size_t)n * sizeof(double), ctx->stream));
-  if (ix.hh) SB_CUDA(cudaMemsetAsync(ix.hh + keep, 0, (size_t)n * sizeof(float), ctx->stream));
-  if (ix.rows32)
-    SB_CUDA(cudaMemsetAsync(ix.rows32 + (size_t)keep * ix.d_pad, 0, (size_t)n * ix.d_pad * sizeof(float), ctx->stream));
-  for (int f = 0; f < SB_MAX_TAG_FIELDS; ++f)
-    if (ix.tags[f]) SB_CUDA(cudaMemsetAsync(ix.tags[f] + keep, 0xff, (size_t)n * 4, ctx->stream));
-  for (int f = 0; f < SB_MAX_VALUE_FIELDS; ++f)
-    if (ix.vals[f]) SB_CUDA(cudaMemsetAsync(ix.vals[f] + keep, 0xff, (size_t)n * 8, ctx->stream));
+  // the vacated tail [keep, n) returns to the fill of unused capacity
+  for (int i = 0; i < nc; ++i)
+    SB_CUDA(cudaMemsetAsync(static_cast<uint8_t*>(*col[i].ptr) + (size_t)keep * col[i].row_bytes, col[i].fill,
+                            (size_t)n * col[i].row_bytes, ctx->stream));
   SB_CUDA(cudaStreamSynchronize(ctx->stream));
   ix.n = keep;
   ix.n_pad = round_rows(keep);
@@ -2808,10 +2672,10 @@ int sb_dense_fetch(sb_ctx* ctx, int slot, const int64_t* ids, int32_t n_ids, flo
   if ((rc = ctx->misc2_dev.reserve((size_t)n_ids * 8))) return rc;
   if ((rc = ctx->misc3_dev.reserve((size_t)n_ids * ix.d * 4))) return rc;
   SB_CUDA(cudaMemcpyAsync(ctx->misc2_dev.p, ids, (size_t)n_ids * 8, cudaMemcpyHostToDevice, ctx->stream));
-  if (ix.rows8)
+  if (ix.storage == SB_STORAGE_U8)
     dense_fetch_u8_kernel<<<n_ids, 128, 0, ctx->stream>>>(ix.rows8, ix.d, ix.d_pad, ix.n, ix.id_base,
                                                           ctx->misc2_dev.as<int64_t>(), n_ids, ctx->misc3_dev.as<float>());
-  else if (ix.rows32)
+  else if (ix.storage == SB_STORAGE_F32)
     dense_fetch_f32_kernel<<<n_ids, 128, 0, ctx->stream>>>(ix.rows32, ix.metric == SB_METRIC_COSINE, ix.d, ix.d_pad, ix.n,
                                                            ix.id_base, ctx->misc2_dev.as<int64_t>(), n_ids,
                                                            ctx->misc3_dev.as<float>());
@@ -2838,15 +2702,7 @@ int sb_dense_tags_load(sb_ctx* ctx, int slot, int32_t field, const int32_t* code
   for (int64_t i = 0; i < n; ++i)
     SB_REQUIRE(codes[i] >= -1, SB_ERR_ARG, "sb_dense_tags_load: code %d at row %lld (must be >= -1)", codes[i],
                (long long)i);
-  SB_CUDA(cudaStreamSynchronize(ctx->stream));
-  if (ix.tags[field]) cudaFree(ix.tags[field]);
-  ix.tags[field] = nullptr;
-  // a column spans the slot's capacity: -1 on the rows past n, so upserts and deletes never reallocate it alone
-  const int64_t cap = std::max<int64_t>(ix.n_cap, 1);
-  SB_CUDA(cudaMalloc(&ix.tags[field], (size_t)cap * 4));
-  SB_CUDA(cudaMemset(ix.tags[field], 0xff, (size_t)cap * 4));
-  if (n) SB_CUDA(cudaMemcpy(ix.tags[field], codes, (size_t)n * 4, cudaMemcpyHostToDevice));
-  return SB_OK;
+  return dense_payload_load(ctx, ix, tag_column(ix, field), codes, n);
 }
 
 int sb_dense_topk_filtered_dev(sb_ctx* ctx, int slot, const float* q_dev, int32_t B, int32_t k,
@@ -2938,15 +2794,7 @@ int sb_dense_values_load(sb_ctx* ctx, int slot, int32_t field, const double* val
   SB_REQUIRE(ix.d > 0, SB_ERR_STATE, "sb_dense_values_load: dense slot %d has no index loaded", slot);
   SB_REQUIRE(n == ix.n, SB_ERR_ARG, "sb_dense_values_load: %lld values for %lld rows", (long long)n, (long long)ix.n);
   SB_REQUIRE(n == 0 || vals != nullptr, SB_ERR_ARG, "sb_dense_values_load: vals is NULL");
-  SB_CUDA(cudaStreamSynchronize(ctx->stream));
-  if (ix.vals[field]) cudaFree(ix.vals[field]);
-  ix.vals[field] = nullptr;
-  // a column spans the slot's capacity: NaN on the rows past n, so upserts and deletes never reallocate it alone
-  const int64_t cap = std::max<int64_t>(ix.n_cap, 1);
-  SB_CUDA(cudaMalloc(&ix.vals[field], (size_t)cap * 8));
-  SB_CUDA(cudaMemset(ix.vals[field], 0xff, (size_t)cap * 8));
-  if (n) SB_CUDA(cudaMemcpy(ix.vals[field], vals, (size_t)n * 8, cudaMemcpyHostToDevice));
-  return SB_OK;
+  return dense_payload_load(ctx, ix, value_column(ix, field), vals, n);
 }
 
 int sb_dense_values_write(sb_ctx* ctx, int slot, int32_t field, const int64_t* rows, const double* vals, int64_t n) {

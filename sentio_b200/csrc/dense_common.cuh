@@ -2,20 +2,29 @@
 #pragma once
 #include "common.cuh"
 
-struct RescoreArgs {
-  const __half* rows;
-  const float* q;     // this query's fp32 vector [d_pad]
+// What the exact stage (window re-score, brute-force fallback, filtered gather) reads of a slot.
+struct SlotView {
+  const __half* rows;   // [rows][d_pad] fp16 (float16 and float32 storage)
+  const float* rows32;  // float32 storage: [rows][d_pad] the caller's x (read by the F32 instantiations only)
+  const uint8_t* rows8; // uint8 storage: [rows][d_pad] the caller's x (read by the U8 instantiations only)
+  const double* cfac;   // [rows] c of v = c * y (Dot / Euclid)
+  int32_t metric;       // SB_METRIC_*
   int32_t d_pad;
-  int32_t ch;         // 16-byte chunks per row
+  int32_t ch;           // d_pad / 8: eight-element chunks per row
   int64_t id_base;
+};
+
+inline SlotView slot_view(const DenseIndex& ix) {
+  return {ix.rows, ix.rows32, ix.rows8, ix.cfac, ix.metric, ix.d_pad, ix.d_pad / 8, ix.id_base};
+}
+
+struct RescoreArgs {
+  SlotView s;
+  const float* q;       // this query's fp32 vector [d_pad]
   int32_t k;
   int64_t* out_ids;     // [k] of this query
   double* out_scores;   // [k]
   int32_t* out_count;   // [1]
-  int32_t metric;       // SB_METRIC_*
-  const double* cfac;   // [rows] c of v = c * y (Dot / Euclid)
-  const float* rows32;  // float32 storage: [rows][d_pad] the caller's x (read by the F32 instantiations only)
-  const uint8_t* rows8; // uint8 storage: [rows][d_pad] the caller's x (read by the U8 instantiations only)
 };
 
 // ---- approximate -> exact hand-off (DESIGN.md "K1: exactness") --------------------------------------------------------
@@ -297,21 +306,19 @@ __device__ __forceinline__ double exact_key_warp(int metric, const __half* rows,
 // exact ordering key of one row under the slot's storage ST (SB_STORAGE_*): float32 and uint8 score the caller's x,
 // float16 the stored fp16 representation
 template <int ST>
-__device__ __forceinline__ double exact_key_row(int metric, const __half* rows, const double* cfac, const float* rows32,
-                                                const uint8_t* rows8, uint32_t idx, const float* q, int d_pad, int nch,
-                                                double qn, int lane) {
+__device__ __forceinline__ double exact_key_row(const SlotView& v, uint32_t idx, const float* q, double qn, int lane) {
   if constexpr (ST == SB_STORAGE_F32) {
     const uint32_t ix[1] = {idx};
     double s[1];
-    exact_f32_warp<1>(metric, rows32, ix, q, d_pad, nch, qn, lane, s);
+    exact_f32_warp<1>(v.metric, v.rows32, ix, q, v.d_pad, v.ch, qn, lane, s);
     return s[0];
   } else if constexpr (ST == SB_STORAGE_U8) {
     const uint32_t ix[1] = {idx};
     double s[1];
-    exact_u8_warp<1>(metric, rows8, ix, q, d_pad, nch, qn, lane, s);
+    exact_u8_warp<1>(v.metric, v.rows8, ix, q, v.d_pad, v.ch, qn, lane, s);
     return s[0];
   } else {
-    return exact_key_warp(metric, rows, cfac, idx, q, d_pad, nch, qn, lane);
+    return exact_key_warp(v.metric, v.rows, v.cfac, idx, q, v.d_pad, v.ch, qn, lane);
   }
 }
 
@@ -319,10 +326,10 @@ __device__ __forceinline__ double exact_key_row(int metric, const __half* rows, 
 __device__ __forceinline__ void emit_exact_pairs(const unsigned long long* ek, const uint32_t* ei, int P,
                                                  const RescoreArgs& p) {
   const int tid = threadIdx.x, nt = blockDim.x;
-  const bool euclid = p.metric == SB_METRIC_EUCLID;
+  const bool euclid = p.s.metric == SB_METRIC_EUCLID;
   for (int i = tid; i < p.k; i += nt) {
     const bool valid = (i < P) && ek[i] != 0ull;
-    p.out_ids[i] = valid ? p.id_base + (int64_t)ei[i] : -1;
+    p.out_ids[i] = valid ? p.s.id_base + (int64_t)ei[i] : -1;
     double s = 0.0;
     if (valid) s = euclid ? -orderable_f64(ek[i]) : orderable_f64(ek[i]);
     p.out_scores[i] = s;
@@ -384,9 +391,10 @@ template <int ST>
 __device__ __forceinline__ void rescore_and_emit(const unsigned long long* sel, int nsel, int P, unsigned long long* ek,
                                                  uint32_t* ei, double* qq_s_ptr, float* q_s, const RescoreArgs p) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nt = blockDim.x, nw = nt >> 5;
-  for (int i = tid; i < p.d_pad; i += nt) q_s[i] = p.q[i];
+  const SlotView& v = p.s;
+  for (int i = tid; i < v.d_pad; i += nt) q_s[i] = p.q[i];
   __syncthreads();
-  const double qn = query_norm_cta(q_s, p.d_pad, qq_s_ptr);
+  const double qn = query_norm_cta(q_s, v.d_pad, qq_s_ptr);
   for (int c = warp; c < P; c += 2 * nw) {
     const int c1 = c + nw;
     const unsigned long long key0 = c < nsel ? sel[c] : 0ull;
@@ -400,21 +408,21 @@ __device__ __forceinline__ void rescore_and_emit(const unsigned long long* sel, 
       if constexpr (ST == SB_STORAGE_F32) {
         const uint32_t ix[2] = {i0, i1};
         double s[2];
-        exact_f32_warp<2>(p.metric, p.rows32, ix, q_s, p.d_pad, p.ch, qn, lane, s);
+        exact_f32_warp<2>(v.metric, v.rows32, ix, q_s, v.d_pad, v.ch, qn, lane, s);
         s0 = s[0];
         s1 = s[1];
       } else if constexpr (ST == SB_STORAGE_U8) {
         const uint32_t ix[2] = {i0, i1};
         double s[2];
-        exact_u8_warp<2>(p.metric, p.rows8, ix, q_s, p.d_pad, p.ch, qn, lane, s);
+        exact_u8_warp<2>(v.metric, v.rows8, ix, q_s, v.d_pad, v.ch, qn, lane, s);
         s0 = s[0];
         s1 = s[1];
-      } else if (p.metric == SB_METRIC_COSINE) {
-        exact_cosine_warp2(p.rows, i0, i1, q_s, p.d_pad, p.ch, qn, lane, &s0, &s1);
+      } else if (v.metric == SB_METRIC_COSINE) {
+        exact_cosine_warp2(v.rows, i0, i1, q_s, v.d_pad, v.ch, qn, lane, &s0, &s1);
       } else {
         const uint32_t ix[2] = {i0, i1};
         double s[2];
-        exact_metric_warp<2>(p.metric, p.rows, p.cfac, ix, q_s, p.d_pad, p.ch, lane, s);
+        exact_metric_warp<2>(v.metric, v.rows, v.cfac, ix, q_s, v.d_pad, v.ch, lane, s);
         s0 = s[0];
         s1 = s[1];
       }
@@ -422,10 +430,10 @@ __device__ __forceinline__ void rescore_and_emit(const unsigned long long* sel, 
       o1 = f64_orderable(s1);
     } else if (key0 != 0ull) {
       i0 = key32_idx(key0);
-      o0 = f64_orderable(exact_key_row<ST>(p.metric, p.rows, p.cfac, p.rows32, p.rows8, i0, q_s, p.d_pad, p.ch, qn, lane));
+      o0 = f64_orderable(exact_key_row<ST>(v, i0, q_s, qn, lane));
     } else if (key1 != 0ull) {
       i1 = key32_idx(key1);
-      o1 = f64_orderable(exact_key_row<ST>(p.metric, p.rows, p.cfac, p.rows32, p.rows8, i1, q_s, p.d_pad, p.ch, qn, lane));
+      o1 = f64_orderable(exact_key_row<ST>(v, i1, q_s, qn, lane));
     }
     if (key0 != 0ull && o0 == 0ull) o0 = 1ull;  // keep 0 reserved for "empty"
     if (key1 != 0ull && o1 == 0ull) o1 = 1ull;

@@ -347,19 +347,13 @@ struct SelectParams {
   float* thr_out;                   // [rows] (mode 0)
   const float* eps;                 // [nq] error bound of the approximate scores (0 = all-zero query)
   int32_t* fallback;                // [nq] (mode 1)
-  const __half* rows;               // mode 1
+  SlotView slot;                    // mode 1
   const float* q;                   // [nq][d_pad] the caller's fp32 queries
-  int32_t d_pad, ch;
-  int64_t id_base;
   int32_t k;
   int64_t* out_ids;
   double* out_scores;
   int32_t* out_counts;
   const int32_t* state;             // FILTER only: [nq] 1 = answered by the gather path (threshold +inf, no emit)
-  int32_t metric;
-  const double* cfac;
-  const float* rows32;              // float32 storage only
-  const uint8_t* rows8;             // uint8 storage only
 };
 
 // One CTA per query.  A lower bound of the k-th best approximate key among the survivors of all CTAs by an MSB-first
@@ -498,20 +492,8 @@ __global__ void __launch_bounds__(kSelectThreads, 2) dense_select_kernel(const S
   }
   int P = 32;
   while (P < ntop) P <<= 1;
-  RescoreArgs ra;
-  ra.rows = p.rows;
-  ra.q = p.q + (size_t)qi * p.d_pad;
-  ra.d_pad = p.d_pad;
-  ra.ch = p.ch;
-  ra.id_base = p.id_base;
-  ra.k = p.k;
-  ra.out_ids = p.out_ids + (size_t)qi * p.k;
-  ra.out_scores = p.out_scores + (size_t)qi * p.k;
-  ra.out_count = p.out_counts + qi;
-  ra.metric = p.metric;
-  ra.cfac = p.cfac;
-  ra.rows32 = p.rows32;
-  ra.rows8 = p.rows8;
+  const RescoreArgs ra{p.slot, p.q + (size_t)qi * p.slot.d_pad, p.k, p.out_ids + (size_t)qi * p.k,
+                       p.out_scores + (size_t)qi * p.k, p.out_counts + qi};
   // the staged survivors are dead (the window lives in `top`): their shared memory becomes the query staging area
   rescore_and_emit<ST>(top, ntop, P, ek, ei, &qq_s, reinterpret_cast<float*>(keys), ra);
 }
@@ -704,10 +686,6 @@ int dense_mma_topk_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int 
     mp.mask_qs = flt ? flt->qs : 0;
     mp.hh = ix.hh;
     SelectParams sp;
-    sp.metric = ix.metric;
-    sp.cfac = ix.cfac;
-    sp.rows32 = ix.rows32;
-    sp.rows8 = ix.rows8;
     sp.cand = cand;
     sp.counts = counts;
     sp.capg = capg;
@@ -715,11 +693,8 @@ int dense_mma_topk_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int 
     sp.thr_out = thr;
     sp.eps = eps + c0;
     sp.fallback = fb + c0;
-    sp.rows = ix.rows;
+    sp.slot = slot_view(ix);
     sp.q = q_pad + (size_t)c0 * ix.d_pad;
-    sp.d_pad = ix.d_pad;
-    sp.ch = ix.d_pad / 8;
-    sp.id_base = ix.id_base;
     sp.k = k;
     sp.out_ids = out_ids + (size_t)c0 * k;
     sp.out_scores = out_scores + (size_t)c0 * k;

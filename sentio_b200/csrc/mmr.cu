@@ -223,10 +223,10 @@ int sb_semantic_mmr(sb_ctx* ctx, int slot, const float* q, int32_t d, const floa
                "sb_semantic_mmr: dense slot %d is empty or has dimension %d != %d", slot, ix.d, d);
     if ((rc = ctx->misc3_dev.reserve(nd * 8))) return rc;
     SB_CUDA(cudaMemcpyAsync(ctx->misc3_dev.p, cand_ids, nd * 8, cudaMemcpyHostToDevice, st));
-    if (ix.rows8)
+    if (ix.storage == SB_STORAGE_U8)
       mmr_gather_kernel<uint8_t><<<n, 128, 0, st>>>(ix.rows8, ix.d, ix.d_pad, ix.n, ix.id_base,
                                                     ctx->misc3_dev.as<int64_t>(), n, Cd);
-    else if (ix.rows32)
+    else if (ix.storage == SB_STORAGE_F32)
       mmr_gather_kernel<float><<<n, 128, 0, st>>>(ix.rows32, ix.d, ix.d_pad, ix.n, ix.id_base,
                                                   ctx->misc3_dev.as<int64_t>(), n, Cd);
     else
