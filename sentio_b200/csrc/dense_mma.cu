@@ -12,7 +12,8 @@
 // Every CTA loads the query boxes itself (512 KB per tile from L2 at d = 1024).  Those L2 reads do not bound the pass,
 // and sharing them across a 2-CTA cluster by TMA multicast measured no faster on the H100.  The serial epilogue does
 // bound it: skipping it takes a 256-query pass from 1.07 to 0.79 ms (DESIGN.md K1b).  So the epilogue keeps global loads
-// off its critical path: a tile's row scales are loaded before its MMAs, and the thresholds once per column pair.
+// off its critical path: a tile's row scales are loaded before its MMAs, and the thresholds once per column pair.  It
+// also tests every score without a branch, into one pass bit per accumulator register, and walks only the set bits.
 //
 // Exactness (dense_common.cuh, DESIGN.md "K1: exactness"):
 //   * queries are L2-normalised before the fp16 rounding (cosine is scale invariant; the caller's scale never reaches
@@ -93,6 +94,22 @@ __device__ __forceinline__ float ldg_early(const float* ptr, bool live) {
       : "+f"(v)
       : "l"(ptr), "r"((uint32_t)live));
   return v;
+}
+
+// acc[32 w + b] for a bit index b known only at run time: a tree of selects on the bits of b over the word's values.
+// Indexing the register array with b would move the accumulator to local memory, and a switch would branch apart the
+// lanes of a warp.  w must be a constant once the caller's loop is unrolled.
+template <int N>
+__device__ __forceinline__ float acc_word_at(const float (&acc)[N], int w, int b) {
+  constexpr int kN = N < 32 ? N : 32;   // accumulator values behind one mask word
+  float v[kN];
+#pragma unroll
+  for (int i = 0; i < kN; ++i) v[i] = acc[32 * w + i];
+#pragma unroll
+  for (int s = 1; s < kN; s <<= 1)
+#pragma unroll
+    for (int i = 0; i < kN; i += 2 * s) v[i] = (b & s) ? v[i + s] : v[i];
+  return v[0];
 }
 
 struct MmaScanParams {
@@ -298,6 +315,14 @@ dense_scan_mma_kernel(const __grid_constant__ CUtensorMap tm_rows, const __grid_
           }
         }
       } else {
+        // Full pass.  About 0.3 % of the scores pass, so the test of every score is kept free of branches: one bit per
+        // accumulator register, set when the row is live, score >= thr[col] (IEEE: -0 >= +0 holds, NaN fails) and,
+        // FILTER, its match bit holds.  Bit a of the mask is acc[a]: row row0 + 8 ((a >> 1) & 1), column
+        // 8 (a >> 2) + 2 (lane % 4) + (a & 1).  Only the set bits are then walked and appended, in the order of a.
+        constexpr int kWords = (QBN / 2 + 31) / 32;
+        uint32_t pass[kWords];
+#pragma unroll
+        for (int w = 0; w < kWords; ++w) pass[w] = 0u;
 #pragma unroll
         for (int j = 0; j < QBN / 4; j += 2) {   // acc[2 j .. 2 j + 3]: columns 4 j .. 4 j + 7
           uint2 mw = make_uint2(0u, 0u);
@@ -309,21 +334,30 @@ dense_scan_mma_kernel(const __grid_constant__ CUtensorMap tm_rows, const __grid_
                        : "r"(thr_s + 4u * (4 * j + 2 * (lane & 3))));
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
-            if (!(h ? live1 : live0)) continue;
-            const int64_t row = row0 + 8 * h;
-            const float invn = h ? invn1 : invn0;
-            const float hrow = h ? h1 : h0;
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
+              const int a = 2 * j + 2 * h + e;
               const int col = 4 * j + 2 * (lane & 3) + e;
-              const float score = key(acc[2 * j + 2 * h + e], invn, hrow, col);
-              bool match = true;
-              if constexpr (FILTER) match = ((e ? mw.y : mw.x) >> (h ? sh1 : sh0)) & 1u;
-              if (score >= (e ? tc.y : tc.x) && match) {
-                const int pos = atomicAdd(&cnt[col], 1);
-                if (pos < p.capg) my_cand[(size_t)col * q_stride + pos] = make_key32(score, (uint32_t)row);
-              }
+              bool b = key(acc[a], h ? invn1 : invn0, h ? h1 : h0, col) >= (e ? tc.y : tc.x);
+              if constexpr (FILTER) b = b && (((e ? mw.y : mw.x) >> (h ? sh1 : sh0)) & 1u);
+              pass[a >> 5] |= (uint32_t)b << (a & 31);
             }
+          }
+        }
+        // bits of row0 are a = 0, 1 mod 4, bits of row0 + 8 are a = 2, 3 mod 4
+        const uint32_t live_bits = (live0 ? 0x33333333u : 0u) | (live1 ? 0xccccccccu : 0u);
+#pragma unroll
+        for (int w = 0; w < kWords; ++w) {
+          uint32_t m = pass[w] & live_bits;
+          while (m != 0u) {
+            const int bit = __ffs(m) - 1;
+            m &= m - 1u;
+            const int a = 32 * w + bit;
+            const int h = (a >> 1) & 1;
+            const int col = 8 * (a >> 2) + 2 * (lane & 3) + (a & 1);
+            const float score = key(acc_word_at(acc, w, bit), h ? invn1 : invn0, h ? h1 : h0, col);
+            const int pos = atomicAdd(&cnt[col], 1);
+            if (pos < p.capg) my_cand[(size_t)col * q_stride + pos] = make_key32(score, (uint32_t)(row0 + 8 * h));
           }
         }
       }
