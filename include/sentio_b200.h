@@ -253,6 +253,30 @@ int sb_dense_topk_where(sb_ctx* ctx, int slot, const float* q, int32_t B, int32_
                         const sb_pred* prog, const int32_t* pool, int32_t n_pool, int64_t* out_ids, double* out_scores,
                         int32_t* out_counts);
 /*
+ * Recommendation by example -- Qdrant's `recommend(positive=, negative=, strategy=)` with the `best_score` and
+ * `sum_scores` strategies (DESIGN.md K1j).  `average_vector` is one nearest query and goes through sb_dense_topk /
+ * sb_dense_topk_where.
+ *
+ * sb_dense_recommend: R requests over m examples ex (row-major m x d fp32, host), ordered request by request, positives
+ * first: request r owns examples [r_off[r], r_off[r+1]) (1 to SB_RECO_MAX_EXAMPLES of them), the first n_pos[r] positive,
+ * the rest negative, merged by strategy[r] (SB_RECO_*).  With s_j = the similarity of a row to example j (Cosine: the
+ * cosine, 0 for a zero example; Dot: <e_j, v>), in fp64 on the exact similarities:
+ *   SB_RECO_BEST_SCORE  p = max over positives, n = max over negatives (-inf for an empty side);
+ *                       score = g(p) if p > n else -g(n),  g(x) = 0.5 (x / (1 + |x|) + 1)
+ *   SB_RECO_SUM_SCORES  score = (sum over positives, in order) - (sum over negatives, in order)
+ * Results: per request the EXACT top-k rows by (score descending, row ascending) among the rows on which its program
+ * (p_off / prog / pool as sb_dense_topk_where; p_off == NULL: unfiltered) leaves a 1: out_ids [R][k] (id_base + row,
+ * -1 past out_counts[r]), out_scores [R][k].  Cosine and Dot slots only (Euclid: SB_ERR_UNSUPPORTED); k <= 1024; finite
+ * examples; everything is validated before the first launch (SB_ERR_ARG).  A request whose candidate window does not
+ * fit is answered by a brute force and counted by sb_dense_fallback_count.
+ */
+#define SB_RECO_BEST_SCORE 1
+#define SB_RECO_SUM_SCORES 2
+#define SB_RECO_MAX_EXAMPLES 256
+int sb_dense_recommend(sb_ctx* ctx, int slot, const float* ex, int32_t m, const int32_t* r_off, const int32_t* n_pos,
+                       const int32_t* strategy, int32_t R, int32_t k, const int32_t* p_off, const sb_pred* prog,
+                       const int32_t* pool, int32_t n_pool, int64_t* out_ids, double* out_scores, int32_t* out_counts);
+/*
  * Grouped dense search -- Qdrant's `search_groups(group_by=, limit=L, group_size=G, query_filter=)`: one answer per
  * document, not per chunk (the reference stamps every chunk with metadata.parent_id, text_splitter.py:143).
  *

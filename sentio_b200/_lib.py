@@ -65,6 +65,9 @@ SIGNATURES = {
     "sb_dense_values_write": (C.c_int, [C.c_void_p, C.c_int, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64]),
     "sb_dense_topk_where": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                                       C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "sb_dense_recommend": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                     C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
+                                     C.c_void_p, C.c_void_p]),
     "sb_dense_groups": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "sb_dense_group_rounds": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32]),

@@ -88,6 +88,7 @@ void sb_destroy(sb_ctx* ctx) {
   ctx->misc3_dev.release();
   ctx->acc_dev.release();
   ctx->qn_dev.release();
+  ctx->reco_dev.release();
   ctx->qaux_dev.release();
   ctx->fb_count_dev.release();
   ctx->sigma_dev.release();

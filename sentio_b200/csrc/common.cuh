@@ -174,6 +174,7 @@ struct sb_ctx {
   // scratch
   DevBuf q_dev, cand_dev, out_ids_dev, out_sc_dev, out_cnt_dev, misc_dev, misc2_dev, misc3_dev, acc_dev;
   DevBuf qn_dev;     // dense: normalised fp32 queries [B][d_pad] fed to the scans
+  DevBuf reco_dev;   // dense recommendation (DESIGN.md K1j): operand rows, per-example bounds, keys and intervals
   DevBuf qaux_dev;   // dense: per-query eps [B] fp32 | fallback flags [B] i32
   DevBuf fb_count_dev;   // dense: [1] u64, queries answered by the exact fallback kernel (sb_dense_fallback_count)
   DevBuf sigma_dev;      // dense float32 storage: [1] u64, bits of the largest sigma of the rows one load / upsert stores

@@ -1714,6 +1714,78 @@ void where_plan_chunk(const int32_t* p_off, const sb_pred* prog, const int32_t* 
   }
 }
 
+// The mask launches of one planned chunk whose programs are staged on the device at sd (kernel attribute already set)
+int where_mask_launches(sb_ctx* ctx, const DenseIndex& ix, const WhereChunk& ch, const uint8_t* sd, uint32_t* mask,
+                        int32_t* cnt_d, int qs, cudaStream_t st) {
+  const int64_t n_words = ix.n_pad / 32;
+  WhereParams wp;
+  for (int c = 0; c < ch.n_tag; ++c) wp.tag[c] = ix.tags[ch.tag_f[c]];
+  for (int c = 0; c < ch.n_val; ++c) wp.val[c] = ix.vals[ch.val_f[c]];
+  wp.n_tag = ch.n_tag;
+  wp.n_val = ch.n_val;
+  wp.n = ix.n;
+  wp.n_words = n_words;
+  wp.qs = qs;
+  wp.mask = mask;
+  wp.counts = cnt_d;
+  for (const WhereLaunch& L : ch.launches) {
+    wp.prog = reinterpret_cast<const sb_pred*>(sd + L.o_prog);
+    wp.u_off = reinterpret_cast<const int32_t*>(sd + L.o_uoff);
+    wp.q_u = reinterpret_cast<const int32_t*>(sd + L.o_qu);
+    wp.pool = reinterpret_cast<const int32_t*>(sd + L.o_pool);
+    wp.n_preds = L.n_preds;
+    wp.n_u = L.n_u;
+    wp.n_pool = L.n_pool;
+    wp.pool_staged = L.n_pool <= kWhereMaxPoolStaged ? 1 : 0;
+    const size_t smem = where_smem_bytes(ch.n_val, L.n_preds, ch.n_tag, L.n_u, wp.pool_staged ? L.n_pool : 0);
+    const int64_t blocks = std::min<int64_t>((n_words + kWhereWarps - 1) / kWhereWarps, (int64_t)ctx->num_sms * 8);
+    ProfScope ps(ctx, SB_PROF_DENSE_FILTER, st);
+    dense_where_mask_kernel<<<(unsigned)blocks, kWhereThreads, smem, st>>>(wp);
+  }
+  SB_CUDA(cudaGetLastError());
+  return SB_OK;
+}
+
+// largest dynamic shared memory of a planned chunk's mask launches
+size_t where_chunk_smem(const WhereChunk& ch) {
+  size_t m = 0;
+  for (const WhereLaunch& L : ch.launches) {
+    const int staged = L.n_pool <= kWhereMaxPoolStaged ? L.n_pool : 0;
+    m = std::max(m, where_smem_bytes(ch.n_val, L.n_preds, ch.n_tag, L.n_u, staged));
+  }
+  return m;
+}
+
+}  // namespace
+
+int dense_where_mask(sb_ctx* ctx, DenseIndex& ix, const int32_t* p_off, const sb_pred* prog, const int32_t* pool, int c0,
+                     int nq, const uint32_t** mask_out, int* qs_out, cudaStream_t st) {
+  const int qs = std::max(32, next_pow2(nq));
+  WhereChunk ch;
+  where_plan_chunk(p_off, prog, pool, c0, nq, qs, ch);
+  const size_t smem = where_chunk_smem(ch);
+  SB_REQUIRE(smem <= ctx->smem_optin, SB_ERR_UNSUPPORTED, "dense: filter programs need %zu bytes of shared memory", smem);
+  // device: counts [qs] | the chunk's programs | mask
+  const size_t o_stage = align16((size_t)qs * 4);
+  const size_t o_mask = (o_stage + ch.bytes.size() + 255) / 256 * 256;
+  int rc;
+  if ((rc = ctx->filt_dev.reserve(o_mask + (size_t)(ix.n_pad / 32) * qs * 4))) return rc;
+  if ((rc = ctx->filt_pin.reserve(ch.bytes.size() + 16))) return rc;
+  uint8_t* dv = ctx->filt_dev.as<uint8_t>();
+  SB_CUDA(cudaStreamSynchronize(st));   // the pinned staging may still feed an earlier call's copies
+  memcpy(ctx->filt_pin.p, ch.bytes.data(), ch.bytes.size());
+  SB_CUDA(cudaMemcpyAsync(dv + o_stage, ctx->filt_pin.p, ch.bytes.size(), cudaMemcpyHostToDevice, st));
+  SB_CUDA(cudaMemsetAsync(dv, 0, (size_t)qs * 4, st));
+  SB_CUDA(cudaFuncSetAttribute(dense_where_mask_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  uint32_t* mask = reinterpret_cast<uint32_t*>(dv + o_mask);
+  if ((rc = where_mask_launches(ctx, ix, ch, dv + o_stage, mask, reinterpret_cast<int32_t*>(dv), qs, st))) return rc;
+  *mask_out = mask;
+  *qs_out = qs;
+  return SB_OK;
+}
+
+namespace {
+
 // Filtered top-k of B queries (q_pad on the device; one validated program per query, host arrays) in chunks of <= 256
 // queries: per chunk the match mask + match counts, one wait for the counts, then the gather path for low-cardinality
 // queries and the masked scans for the rest.  A batch of empty programs is the unfiltered search.
@@ -1734,10 +1806,7 @@ int dense_topk_where_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, in
     WhereChunk& ch = chunks[c];
     where_plan_chunk(p_off, prog, pool, c0, nq, std::max(32, next_pow2(nq)), ch);
     stage_bytes = std::max(stage_bytes, ch.bytes.size());
-    for (const WhereLaunch& L : ch.launches) {
-      const int staged = L.n_pool <= kWhereMaxPoolStaged ? L.n_pool : 0;
-      smem_max = std::max(smem_max, where_smem_bytes(ch.n_val, L.n_preds, ch.n_tag, L.n_u, staged));
-    }
+    smem_max = std::max(smem_max, where_chunk_smem(ch));
   }
   // device: counts [qchunk] | state [qchunk] | qlist [qchunk] | one chunk's programs | mask
   const size_t o_cnt = 0, o_state = (size_t)qchunk * 4, o_qlist = o_state + (size_t)qchunk * 4;
@@ -1772,32 +1841,7 @@ int dense_topk_where_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, in
     memcpy(hp + o_stage, ch.bytes.data(), ch.bytes.size());
     SB_CUDA(cudaMemcpyAsync(dv + o_stage, hp + o_stage, ch.bytes.size(), cudaMemcpyHostToDevice, st));
     SB_CUDA(cudaMemsetAsync(cnt_d, 0, (size_t)qs * 4, st));
-    WhereParams wp;
-    for (int c = 0; c < ch.n_tag; ++c) wp.tag[c] = ix.tags[ch.tag_f[c]];
-    for (int c = 0; c < ch.n_val; ++c) wp.val[c] = ix.vals[ch.val_f[c]];
-    wp.n_tag = ch.n_tag;
-    wp.n_val = ch.n_val;
-    wp.n = ix.n;
-    wp.n_words = n_words;
-    wp.qs = qs;
-    wp.mask = mask;
-    wp.counts = cnt_d;
-    const uint8_t* sd = dv + o_stage;
-    for (const WhereLaunch& L : ch.launches) {
-      wp.prog = reinterpret_cast<const sb_pred*>(sd + L.o_prog);
-      wp.u_off = reinterpret_cast<const int32_t*>(sd + L.o_uoff);
-      wp.q_u = reinterpret_cast<const int32_t*>(sd + L.o_qu);
-      wp.pool = reinterpret_cast<const int32_t*>(sd + L.o_pool);
-      wp.n_preds = L.n_preds;
-      wp.n_u = L.n_u;
-      wp.n_pool = L.n_pool;
-      wp.pool_staged = L.n_pool <= kWhereMaxPoolStaged ? 1 : 0;
-      const size_t smem = where_smem_bytes(ch.n_val, L.n_preds, ch.n_tag, L.n_u, wp.pool_staged ? L.n_pool : 0);
-      const int64_t blocks = std::min<int64_t>((n_words + kWhereWarps - 1) / kWhereWarps, (int64_t)ctx->num_sms * 8);
-      ProfScope ps(ctx, SB_PROF_DENSE_FILTER, st);
-      dense_where_mask_kernel<<<(unsigned)blocks, kWhereThreads, smem, st>>>(wp);
-    }
-    SB_CUDA(cudaGetLastError());
+    if ((rc = where_mask_launches(ctx, ix, ch, dv + o_stage, mask, cnt_d, qs, st))) return rc;
     SB_CUDA(cudaMemcpyAsync(cnt_h, cnt_d, (size_t)nq * 4, cudaMemcpyDeviceToHost, st));
     SB_CUDA(cudaStreamSynchronize(st));
     // route: a filtered query with <= kGatherMax matching rows is answered exactly from its matches; the others are
@@ -2864,6 +2908,65 @@ int sb_dense_topk_where(sb_ctx* ctx, int slot, const float* q, int32_t B, int32_
   SB_CUDA(cudaMemcpyAsync(out_ids, ctx->out_ids_dev.p, nid * 8, cudaMemcpyDeviceToHost, st));
   SB_CUDA(cudaMemcpyAsync(out_scores, ctx->out_sc_dev.p, nid * 8, cudaMemcpyDeviceToHost, st));
   SB_CUDA(cudaMemcpyAsync(out_counts, ctx->out_cnt_dev.p, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
+  SB_CUDA(cudaStreamSynchronize(st));
+  return SB_OK;
+}
+
+int sb_dense_recommend(sb_ctx* ctx, int slot, const float* ex, int32_t m, const int32_t* r_off, const int32_t* n_pos,
+                       const int32_t* strategy, int32_t R, int32_t k, const int32_t* p_off, const sb_pred* prog,
+                       const int32_t* pool, int32_t n_pool, int64_t* out_ids, double* out_scores, int32_t* out_counts) {
+  const char* who = "sb_dense_recommend";
+  SB_REQUIRE(ctx != nullptr, SB_ERR_ARG, "%s: ctx is NULL", who);
+  SB_REQUIRE(slot >= 0 && slot < SB_MAX_DENSE_SLOTS, SB_ERR_ARG, "%s: bad slot %d", who, slot);
+  SB_REQUIRE(R >= 0 && m >= 0 && k > 0, SB_ERR_ARG, "%s: bad R=%d m=%d k=%d", who, R, m, k);
+  SB_REQUIRE(k <= kDenseMaxK, SB_ERR_UNSUPPORTED, "%s: top_k %d too large (max %d per call)", who, k, kDenseMaxK);
+  if (R == 0) return SB_OK;
+  SB_REQUIRE(ex && r_off && n_pos && strategy && out_ids && out_scores && out_counts, SB_ERR_ARG, "%s: NULL buffer", who);
+  SB_REQUIRE(r_off[0] == 0 && r_off[R] == m, SB_ERR_ARG, "%s: r_off must run from 0 to m = %d", who, m);
+  std::vector<RecoReq> req((size_t)R);
+  for (int r = 0; r < R; ++r) {
+    const int32_t mr = r_off[r + 1] - r_off[r];
+    SB_REQUIRE(mr >= 1 && mr <= SB_RECO_MAX_EXAMPLES, SB_ERR_ARG, "%s: request %d has %d examples (1 to %d)", who, r, mr,
+               SB_RECO_MAX_EXAMPLES);
+    SB_REQUIRE(n_pos[r] >= 0 && n_pos[r] <= mr, SB_ERR_ARG, "%s: request %d: n_pos %d outside [0, %d]", who, r, n_pos[r],
+               mr);
+    SB_REQUIRE(strategy[r] == SB_RECO_BEST_SCORE || strategy[r] == SB_RECO_SUM_SCORES, SB_ERR_ARG,
+               "%s: request %d: strategy %d", who, r, strategy[r]);
+    req[(size_t)r] = {r_off[r], mr, n_pos[r], strategy[r]};
+  }
+  SB_REQUIRE(p_off == nullptr || p_off[R] == 0 || prog != nullptr, SB_ERR_ARG, "%s: NULL program", who);
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  DeviceGuard g(ctx->device);
+  cudaStream_t st = ctx->stream;
+  DenseIndex& ix = ctx->dense[slot];
+  SB_REQUIRE(ix.d > 0, SB_ERR_STATE, "%s: dense slot %d has no index loaded", who, slot);
+  SB_REQUIRE(ix.metric != SB_METRIC_EUCLID, SB_ERR_UNSUPPORTED, "%s: best_score / sum_scores on a Euclid slot", who);
+  for (int64_t i = 0; i < (int64_t)m * ix.d; ++i)
+    SB_REQUIRE(std::isfinite(ex[i]), SB_ERR_ARG, "%s: example %lld has a NaN or infinite value", who,
+               (long long)(i / ix.d));
+  int rc;
+  if (p_off && (rc = where_validate(who, ix, R, p_off, prog, pool, n_pool))) return rc;
+  if (ix.n == 0) {
+    for (int64_t i = 0; i < (int64_t)R * k; ++i) { out_ids[i] = -1; out_scores[i] = 0.0; }
+    for (int i = 0; i < R; ++i) out_counts[i] = 0;
+    return SB_OK;
+  }
+  const size_t nid = (size_t)R * k;
+  if ((rc = ctx->pin_in.reserve((size_t)m * ix.d * sizeof(float)))) return rc;
+  SB_CUDA(cudaStreamSynchronize(st));
+  memcpy(ctx->pin_in.p, ex, (size_t)m * ix.d * sizeof(float));
+  float* ex_pad = nullptr;
+  if ((rc = sb_dense_pad_queries(ctx, ix, ctx->pin_in.as<float>(), m, false, &ex_pad, st))) return rc;
+  if ((rc = ctx->out_ids_dev.reserve(nid * 8))) return rc;
+  if ((rc = ctx->out_sc_dev.reserve(nid * 8))) return rc;
+  if ((rc = ctx->out_cnt_dev.reserve((size_t)R * 4))) return rc;
+  if ((rc = dense_reco_enqueue(ctx, ix, ex_pad, m, req.data(), R, k, p_off && p_off[R] > 0 ? p_off : nullptr, prog, pool,
+                               ctx->out_ids_dev.as<int64_t>(), ctx->out_sc_dev.as<double>(),
+                               ctx->out_cnt_dev.as<int32_t>(), st)))
+    return rc;
+  SB_CUDA(cudaMemcpyAsync(out_ids, ctx->out_ids_dev.p, nid * 8, cudaMemcpyDeviceToHost, st));
+  SB_CUDA(cudaMemcpyAsync(out_scores, ctx->out_sc_dev.p, nid * 8, cudaMemcpyDeviceToHost, st));
+  SB_CUDA(cudaMemcpyAsync(out_counts, ctx->out_cnt_dev.p, (size_t)R * 4, cudaMemcpyDeviceToHost, st));
   SB_CUDA(cudaStreamSynchronize(st));
   return SB_OK;
 }

@@ -130,9 +130,13 @@ struct MmaScanParams {
   const float* hh;              // EUCLID only: per-row h (>= ||v||^2 / 2)
   const float* rq;              // EUCLID only: [QBN] (float)||q|| of the group's queries
 };
+// STORE mode reads the same parameters (keeping every other instantiation's code unchanged): cand is the float key
+// buffer, keys[col * capg + row], and mask_qs the number of columns stored.
 
 // Key of a row (dense.cu dense_scan_kernel): acc * scale[row], EUCLID r * (acc * scale[row]) - h[row].
-template <int QBN, bool FILTER, bool EUCLID, int ST>
+// STORE (recommendation, DESIGN.md K1j): no threshold and no lists; every live row's key of every column < mask_qs is
+// written to the key buffer (MmaScanParams).
+template <int QBN, bool FILTER, bool EUCLID, int ST, bool STORE = false>
 __global__ void __launch_bounds__(kMmaThreads, 1)
 dense_scan_mma_kernel(const __grid_constant__ CUtensorMap tm_rows, const __grid_constant__ CUtensorMap tm_q,
                       const MmaScanParams p) {
@@ -285,7 +289,15 @@ dense_scan_mma_kernel(const __grid_constant__ CUtensorMap tm_rows, const __grid_
       const uint32_t* mrow = nullptr;
       if constexpr (FILTER) mrow = p.mask + (size_t)(row0 >> 5) * p.mask_qs + 2 * (lane & 3);
       const int sh0 = (int)(row0 & 31), sh1 = sh0 + 8;
-      if (p.thr_init == nullptr) {
+      if constexpr (STORE) {
+#pragma unroll
+        for (int a = 0; a < QBN / 2; ++a) {   // acc[a]: row row0 + 8 ((a >> 1) & 1), column 8 (a >> 2) + 2 (lane % 4) + (a & 1)
+          const int h = (a >> 1) & 1;
+          const int col = 8 * (a >> 2) + 2 * (lane & 3) + (a & 1);
+          if ((h ? live1 : live0) && col < p.mask_qs)
+            reinterpret_cast<float*>(p.cand)[(size_t)col * p.capg + row0 + 8 * h] = key(acc[a], h ? invn1 : invn0, 0.f, col);
+        }
+      } else if (p.thr_init == nullptr) {
         // Sampling pass.  The threshold only needs a LOWER bound of the k-th best score, and the k-th largest of ANY set
         // of distinct rows' scores is one: each warp contributes the best score among its 16 rows per query (two
         // registers, then a max over the 8 lanes that share a column), one 8-byte store per (warp, query) at slot
@@ -363,6 +375,7 @@ dense_scan_mma_kernel(const __grid_constant__ CUtensorMap tm_rows, const __grid_
       }
     }
   }
+  if constexpr (STORE) return;
   __syncthreads();
   for (int i = threadIdx.x; i < QBN; i += blockDim.x) {
     const int c = p.thr_init == nullptr ? my_tiles * kSampleKeys : cnt[i];   // sampling pass: one key per warp and tile
@@ -559,6 +572,20 @@ int encode_map(CUtensorMap* map, const void* ptr, int64_t rows, int64_t cols, in
   return SB_OK;
 }
 
+// the slot's cached corpus map (ix.tm_rows), (re)built when rows or n_pad change
+int corpus_map(DenseIndex& ix) {
+  const bool u8 = ix.storage == SB_STORAGE_U8;
+  const void* corpus = u8 ? (const void*)ix.rows8 : (const void*)ix.rows;
+  if (ix.tm_rows_ptr != corpus || ix.tm_n_pad != ix.n_pad) {
+    int rc;
+    if ((rc = encode_map(reinterpret_cast<CUtensorMap*>(ix.tm_rows), corpus, ix.n_pad, ix.d_pad, kTileRows, u8)))
+      return rc;
+    ix.tm_rows_ptr = corpus;
+    ix.tm_n_pad = ix.n_pad;
+  }
+  return SB_OK;
+}
+
 // ring stages of a QBN-query group: corpus box + query box each, capped by SB_DENSE_STAGES.  Per query: threshold and
 // count, and for Euclid the query norm r.  A uint8 corpus box is half the size (at QBN = 256: 40 KB stages, five fit).
 size_t mma_per_query(bool euclid) { return euclid ? 12 : 8; }
@@ -572,10 +599,10 @@ size_t mma_smem(int qbn, int stages, bool euclid, bool u8 = false) {
          (size_t)qbn * mma_per_query(euclid);
 }
 
-template <int QBN, bool FILTER, bool EUCLID, int ST>
+template <int QBN, bool FILTER, bool EUCLID, int ST, bool STORE = false>
 int launch_mma(const CUtensorMap& tm_rows, const CUtensorMap& tm_q, const MmaScanParams& mp, int grid, size_t smem,
                cudaStream_t st) {
-  auto kern = dense_scan_mma_kernel<QBN, FILTER, EUCLID, ST>;
+  auto kern = dense_scan_mma_kernel<QBN, FILTER, EUCLID, ST, STORE>;
   SB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   kern<<<grid, kMmaThreads, smem, st>>>(tm_rows, tm_q, mp);
   SB_CUDA(cudaGetLastError());
@@ -583,18 +610,288 @@ int launch_mma(const CUtensorMap& tm_rows, const CUtensorMap& tm_q, const MmaSca
 }
 
 // ST: SB_STORAGE_U8 for a uint8 corpus; float16 and float32 slots scan the same fp16 rows (SB_STORAGE_F16)
-template <bool FILTER, bool EUCLID, int ST>
+template <bool FILTER, bool EUCLID, int ST, bool STORE = false>
 int dispatch_mma(int qbn, const CUtensorMap& tm_rows, const CUtensorMap& tm_q, const MmaScanParams& mp, int grid,
                  size_t smem, cudaStream_t st) {
   switch (qbn) {
-    case 16: return launch_mma<16, FILTER, EUCLID, ST>(tm_rows, tm_q, mp, grid, smem, st);
-    case 32: return launch_mma<32, FILTER, EUCLID, ST>(tm_rows, tm_q, mp, grid, smem, st);
-    case 64: return launch_mma<64, FILTER, EUCLID, ST>(tm_rows, tm_q, mp, grid, smem, st);
-    case 128: return launch_mma<128, FILTER, EUCLID, ST>(tm_rows, tm_q, mp, grid, smem, st);
-    case 256: return launch_mma<256, FILTER, EUCLID, ST>(tm_rows, tm_q, mp, grid, smem, st);
+    case 16: return launch_mma<16, FILTER, EUCLID, ST, STORE>(tm_rows, tm_q, mp, grid, smem, st);
+    case 32: return launch_mma<32, FILTER, EUCLID, ST, STORE>(tm_rows, tm_q, mp, grid, smem, st);
+    case 64: return launch_mma<64, FILTER, EUCLID, ST, STORE>(tm_rows, tm_q, mp, grid, smem, st);
+    case 128: return launch_mma<128, FILTER, EUCLID, ST, STORE>(tm_rows, tm_q, mp, grid, smem, st);
+    case 256: return launch_mma<256, FILTER, EUCLID, ST, STORE>(tm_rows, tm_q, mp, grid, smem, st);
   }
   sb_set_error("dense_mma: unsupported query block %d", qbn);
   return SB_ERR_UNSUPPORTED;
+}
+
+
+// ------------------------------------------------------------------------------------------------ recommendation (K1j)
+// The scan in STORE mode leaves key a_j(x) of every (example j, row x) of a pass.  With |a_j(x) - s_j(x) / c_j| <= eps_j
+// (c_j = ||e_j|| for Dot, 1 for Cosine), s_j(x) lies in [c_j a_j - delta_j, c_j a_j + delta_j], delta_j = c_j eps_j.  The
+// merged score is non-decreasing in every positive and non-increasing in every negative similarity (best_score across
+// its jump at p = n too), so its interval is the merge at the two corners, widened by the fp64 rounding.  The exact top-k lies in W = {x : hi(x) >= the k-th largest lo}; every member is re-scored in fp64.
+constexpr int kRecoThreads = 1024;
+constexpr int kRecoFbBest = 1024;                  // >= k
+constexpr int64_t kRecoKeyBudget = 1ll << 30;      // bytes of keys of one pass (examples x n_pad fp32)
+constexpr int64_t kRecoBoundBudget = 1ll << 29;    // bytes of intervals of one pass (requests x n_pad x 16)
+
+__device__ __forceinline__ double reco_g(double x) { return 0.5 * (x / (1.0 + fabs(x)) + 1.0); }
+// best_score of (p, n); ties p == n take the negative branch
+__device__ __forceinline__ double reco_best(double p, double n) { return p > n ? reco_g(p) : -reco_g(n); }
+
+// ||e_j|| in fp64 as query_norm_cta computes it, and (c_j, delta_j); one warp per example
+__global__ void __launch_bounds__(256) dense_reco_norms_kernel(const float* ex, int M, int d_pad, int metric,
+                                                               const float* eps, double* qn, double* cd) {
+  const int j = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+  if (j >= M) return;
+  double s = 0.0;
+  for (int i = lane; i < d_pad; i += 32) {
+    const double v = (double)ex[(size_t)j * d_pad + i];
+    s += v * v;
+  }
+  for (int o = 16; o; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if (lane == 0) {
+    const double nrm = sqrt(s);
+    const double c = metric == SB_METRIC_DOT ? nrm : 1.0;
+    qn[j] = nrm;
+    cd[2 * j] = c;
+    cd[2 * j + 1] = c * (double)eps[j];
+  }
+}
+
+struct RecoCombineParams {
+  const float* keys;      // [examples of the pass][ld]
+  int64_t ld, n;
+  int32_t e0, r0;         // first example / request of the pass
+  const RecoReq* req;
+  const double* cd;       // [M][2] c_j, delta_j
+  const uint32_t* mask;   // filtered passes: bit (row % 32) of mask[(row / 32) * mask_qs + request - r0]
+  int32_t mask_qs;
+  unsigned long long* lo; // [requests of the pass][ld] orderable fp64 lower bound; 0 = the row does not match
+  double* hi;             // [requests of the pass][ld] upper bound
+};
+
+__global__ void __launch_bounds__(256) dense_reco_combine_kernel(const RecoCombineParams p) {
+  const int rl = blockIdx.y;
+  const int64_t row = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (row >= p.n) return;
+  const RecoReq q = p.req[p.r0 + rl];
+  bool match = true;
+  if (p.mask) match = (p.mask[(size_t)(row >> 5) * p.mask_qs + rl] >> (row & 31)) & 1u;
+  unsigned long long lo_key = 0ull;
+  double hi_d = -INFINITY;
+  if (match) {
+    double plo = -INFINITY, phi = -INFINITY, nlo = -INFINITY, nhi = -INFINITY, slo = 0.0, shi = 0.0, scale = 0.0;
+    const float* kc = p.keys + (size_t)(q.ex0 - p.e0) * p.ld + row;
+    for (int j = 0; j < q.m; ++j) {
+      const double c = p.cd[2 * (q.ex0 + j)], d = p.cd[2 * (q.ex0 + j) + 1];
+      const double s = c * (double)__ldg(kc + (size_t)j * p.ld);
+      const double w = 1e-12 * (fabs(s) + d);   // covers the fp64 rounding of s and s -+ d
+      const double a = s - d - w, b = s + d + w;
+      if (j < q.n_pos) {
+        plo = fmax(plo, a);
+        phi = fmax(phi, b);
+        slo += a;
+        shi += b;
+      } else {
+        nlo = fmax(nlo, a);
+        nhi = fmax(nhi, b);
+        slo -= b;
+        shi -= a;
+      }
+      scale += fabs(s) + d;
+    }
+    // fp64 rounding: of g, inside 1e-15 (g <= 1); of a sum of <= 256 terms, inside 1e-12 (1 + scale).  The intervals
+    // stay fp64: a Dot best_score saturates g near 1, where fp32 would merge every row into a few values.
+    const bool best = q.strategy == SB_RECO_BEST_SCORE;
+    const double slack = best ? 1e-15 : 1e-12 * (1.0 + scale);
+    const double lo = (best ? reco_best(plo, nhi) : slo) - slack;
+    hi_d = (best ? reco_best(phi, nlo) : shi) + slack;
+    lo_key = f64_orderable(lo);
+  }
+  p.lo[(size_t)rl * p.ld + row] = lo_key;
+  p.hi[(size_t)rl * p.ld + row] = hi_d;
+}
+
+struct RecoSelectParams {
+  const unsigned long long* lo;
+  const double* hi;
+  int64_t ld, n;
+  int32_t r0;
+  const RecoReq* req;
+  const float* ex;              // [M][d_pad] the caller's fp32 examples
+  const double* qn;             // [M] ||e_j||
+  const int32_t* ex_fb;         // [M] raised by the query preparation: the keys of e_j are not bounded
+  SlotView slot;
+  int32_t k;
+  int32_t* fallback;            // [R]
+  int64_t* out_ids;             // [R][k]
+  double* out_scores;
+  int32_t* out_counts;          // [R]
+  const uint32_t* mask;         // fallback: as RecoCombineParams
+  int32_t mask_qs;
+  unsigned long long* counter;  // fallback: requests answered by brute force
+};
+
+// exact merged score of one row (one full warp; every lane returns it)
+template <int ST>
+__device__ __forceinline__ double reco_exact_row(const RecoSelectParams& p, const RecoReq& q, uint32_t row, int lane) {
+  double sp = 0.0, sn = 0.0, pm = -INFINITY, nm = -INFINITY;
+  for (int j = 0; j < q.m; ++j) {
+    const int e = q.ex0 + j;
+    const double s = exact_key_row<ST>(p.slot, row, p.ex + (size_t)e * p.slot.d_pad, p.qn[e], lane);
+    if (j < q.n_pos) {
+      sp += s;
+      pm = fmax(pm, s);
+    } else {
+      sn += s;
+      nm = fmax(nm, s);
+    }
+  }
+  return q.strategy == SB_RECO_BEST_SCORE ? reco_best(pm, nm) : sp - sn;
+}
+
+// One CTA per request of the pass: the k-th largest lower bound by an MSB-first radix select over the request's rows,
+// the window {hi >= it}, the exact re-score of the window and the emit.  A window over kSelTop raises the fallback flag.
+template <int ST>
+__global__ void __launch_bounds__(kRecoThreads, 1) dense_reco_select_kernel(const RecoSelectParams p) {
+  __shared__ uint32_t top[kSelTop];
+  __shared__ unsigned long long ek[kSelTop];
+  __shared__ uint32_t ei[kSelTop];
+  __shared__ int s_hist[256];
+  __shared__ int s_scal[4];
+  __shared__ int s_cnt;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nt = blockDim.x, nw = nt >> 5;
+  const int rl = blockIdx.x, r = p.r0 + rl;
+  const RecoReq q = p.req[r];
+  if (tid == 0) {
+    int f = 0;
+    for (int j = 0; j < q.m; ++j) f |= p.ex_fb[q.ex0 + j];
+    s_cnt = f;
+  }
+  __syncthreads();
+  if (s_cnt != 0) {
+    if (tid == 0) p.fallback[r] = 1;
+    return;
+  }
+  __syncthreads();
+  if (tid == 0) s_cnt = 0;
+  __syncthreads();
+  const unsigned long long* lo = p.lo + (size_t)rl * p.ld;
+  const double* hi = p.hi + (size_t)rl * p.ld;
+  {
+    int c = 0;
+    for (int64_t i = tid; i < p.n; i += nt) c += lo[i] != 0ull;
+    for (int o = 16; o; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
+    if (lane == 0 && c) atomicAdd(&s_cnt, c);
+  }
+  __syncthreads();
+  const int total = s_cnt;
+  double thr = -INFINITY;   // at most k candidates: every one is a member
+  if (total > p.k) {
+    unsigned long long prefix = 0ull, msk = 0ull;
+    int need = p.k;
+    for (int shift = 56; shift >= 0; shift -= 8) {
+      for (int i = tid; i < 256; i += nt) s_hist[i] = 0;
+      __syncthreads();
+      for (int64_t i = tid; i < p.n; i += nt) {
+        const unsigned long long key = lo[i];
+        if (key != 0ull && (key & msk) == prefix) {
+          const int dgt = (int)((key >> shift) & 0xffull);
+          const unsigned grp = __match_any_sync(__activemask(), dgt);
+          if (lane == __ffs(grp) - 1) atomicAdd(&s_hist[dgt], __popc(grp));
+        }
+      }
+      __syncthreads();
+      if (warp == 0) warp_select_bin<true>(s_hist, need, lane, s_scal);
+      __syncthreads();
+      prefix |= (unsigned long long)s_scal[0] << shift;
+      msk |= 0xffull << shift;
+      need = s_scal[1];
+      __syncthreads();
+    }
+    thr = orderable_f64(prefix);   // the k-th largest lower bound
+  }
+  if (tid == 0) s_cnt = 0;
+  __syncthreads();
+  for (int64_t i = tid; i < p.n; i += nt)
+    if (lo[i] != 0ull && hi[i] >= thr) {
+      const int at = atomicAdd(&s_cnt, 1);
+      if (at < kSelTop) top[at] = (uint32_t)i;
+    }
+  __syncthreads();
+  const int ntop = s_cnt;
+  if (ntop > kSelTop) {
+    if (tid == 0) p.fallback[r] = 1;
+    return;
+  }
+  int P = 32;
+  while (P < ntop) P <<= 1;
+  for (int c = warp; c < P; c += nw) {
+    unsigned long long okey = 0ull;
+    uint32_t row = 0xffffffffu;
+    if (c < ntop) {
+      row = top[c];
+      okey = f64_orderable(reco_exact_row<ST>(p, q, row, lane));
+      if (okey == 0ull) okey = 1ull;   // 0 is reserved for "empty"
+    }
+    if (lane == 0) {
+      ek[c] = okey;
+      ei[c] = row;
+    }
+  }
+  __syncthreads();
+  sort_exact_pairs(ek, ei, P, tid, nt);
+  const RescoreArgs ra{p.slot, nullptr, p.k, p.out_ids + (size_t)r * p.k, p.out_scores + (size_t)r * p.k,
+                       p.out_counts + r};
+  emit_exact_pairs(ek, ei, P, ra);
+}
+
+// One CTA per FLAGGED request of the pass: the merged score of every matching row in fp64, 1024 rows per round folded
+// into the running best list (as dense_exact_fallback_kernel).
+template <int ST>
+__global__ void __launch_bounds__(kRecoThreads, 1) dense_reco_fallback_kernel(const RecoSelectParams p) {
+  const int rl = blockIdx.x, r = p.r0 + rl;
+  if (p.fallback[r] == 0) return;
+  __shared__ unsigned long long ek[2 * kRecoFbBest];
+  __shared__ uint32_t ei[2 * kRecoFbBest];
+  __shared__ int s_beats;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nt = blockDim.x, nw = nt >> 5;
+  if (tid == 0) atomicAdd(p.counter, 1ull);
+  const RecoReq q = p.req[r];
+  for (int i = tid; i < 2 * kRecoFbBest; i += nt) {
+    ek[i] = 0ull;
+    ei[i] = 0xffffffffu;
+  }
+  __syncthreads();
+  for (int64_t r0 = 0; r0 < p.n; r0 += kRecoFbBest) {
+    if (tid == 0) s_beats = 0;
+    __syncthreads();
+    const unsigned long long kth = ek[p.k - 1];
+    bool beat = false;
+    for (int c = warp; c < kRecoFbBest; c += nw) {
+      const int64_t row = r0 + c;
+      bool match = row < p.n;
+      if (match && p.mask) match = (p.mask[(size_t)(row >> 5) * p.mask_qs + rl] >> (row & 31)) & 1u;
+      unsigned long long okey = 0ull;
+      if (match) {
+        okey = f64_orderable(reco_exact_row<ST>(p, q, (uint32_t)row, lane));
+        if (okey == 0ull) okey = 1ull;
+      }
+      if (lane == 0) {
+        ek[kRecoFbBest + c] = okey;
+        ei[kRecoFbBest + c] = row < p.n ? (uint32_t)row : 0xffffffffu;
+        beat |= okey > kth;
+      }
+    }
+    if (beat) s_beats = 1;
+    __syncthreads();
+    if (s_beats) sort_exact_pairs(ek, ei, 2 * kRecoFbBest, tid, nt);
+    __syncthreads();
+  }
+  const RescoreArgs ra{p.slot, nullptr, p.k, p.out_ids + (size_t)r * p.k, p.out_scores + (size_t)r * p.k,
+                       p.out_counts + r};
+  emit_exact_pairs(ek, ei, kRecoFbBest, ra);
 }
 
 }  // namespace
@@ -653,13 +950,7 @@ int dense_mma_topk_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int 
   int32_t* counts = reinterpret_cast<int32_t*>(thr + (size_t)gsz * gmax);
   unsigned long long* cand = ctx->cand_dev.as<unsigned long long>();
   const bool u8 = ix.storage == SB_STORAGE_U8;
-  const void* corpus = u8 ? (const void*)ix.rows8 : (const void*)ix.rows;
-  if (ix.tm_rows_ptr != corpus || ix.tm_n_pad != ix.n_pad) {  // (re)build the corpus map when rows or n_pad change
-    if ((rc = encode_map(reinterpret_cast<CUtensorMap*>(ix.tm_rows), corpus, ix.n_pad, ix.d_pad, kTileRows, u8)))
-      return rc;
-    ix.tm_rows_ptr = corpus;
-    ix.tm_n_pad = ix.n_pad;
-  }
+  if ((rc = corpus_map(ix))) return rc;
   const CUtensorMap& tm_rows = *reinterpret_cast<const CUtensorMap*>(ix.tm_rows);
   const size_t sel_smem = (size_t)kSelStage * 8 + (size_t)kSelTop * 20 + 64;
   auto sel_kern = flt ? dense_select_kernel<true, SB_STORAGE_F16> : dense_select_kernel<false, SB_STORAGE_F16>;
@@ -782,4 +1073,135 @@ int dense_mma_topk_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int 
     SB_CUDA(cudaGetLastError());
   }
   return dense_fallback_enqueue(ctx, ix, q_pad, B, k, fb, out_ids, out_scores, out_counts, st, flt);
+}
+
+// Recommendation (DESIGN.md K1j): requests packed into passes of <= 256 examples (fewer on slots whose keys would pass
+// kRecoKeyBudget, never fewer than the largest request), one STORE-mode scan per pass, then per pass the intervals, the
+// select + exact stage and the brute force of the flagged requests.
+int dense_reco_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* ex_pad, int M, const RecoReq* req, int R, int k,
+                       const int32_t* p_off, const sb_pred* prog, const int32_t* pool, int64_t* out_ids,
+                       double* out_scores, int32_t* out_counts, cudaStream_t st) {
+  const bool u8 = ix.storage == SB_STORAGE_U8;
+  const int64_t n_pad = ix.n_pad;
+  auto align_up = [](size_t v, size_t a) { return (v + a - 1) / a * a; };
+  int m_max = 1;
+  for (int r = 0; r < R; ++r) m_max = std::max(m_max, req[r].m);
+  const int e_cap = std::max(m_max, (int)std::min<int64_t>(kQbnMax, std::max<int64_t>(16, kRecoKeyBudget / (4 * n_pad))));
+  const int r_cap = (int)std::min<int64_t>(kQbnMax, std::max<int64_t>(1, kRecoBoundBudget / (16 * n_pad)));
+  // scratch: fp16 operand rows | qn [M] | (c, delta) [M] | requests [R] | fallback [R] | keys | lo | hi
+  const size_t o_qn = align_up((size_t)(M + kQbnMax) * ix.d_pad * 2, 256);
+  const size_t o_cd = o_qn + align_up((size_t)M * 8, 256);
+  const size_t o_req = o_cd + align_up((size_t)M * 16, 256);
+  const size_t o_fb = o_req + align_up((size_t)R * sizeof(RecoReq), 256);
+  const size_t o_keys = o_fb + align_up((size_t)R * 4, 256);
+  const size_t o_lo = o_keys + align_up((size_t)e_cap * n_pad * 4, 256);
+  const size_t o_hi = o_lo + (size_t)r_cap * n_pad * 8;
+  int rc;
+  if ((rc = ctx->reco_dev.reserve(o_hi + (size_t)r_cap * n_pad * 8))) return rc;
+  uint8_t* base = ctx->reco_dev.as<uint8_t>();
+  __half* q16 = reinterpret_cast<__half*>(base);
+  double* qn = reinterpret_cast<double*>(base + o_qn);
+  double* cd = reinterpret_cast<double*>(base + o_cd);
+  RecoReq* req_d = reinterpret_cast<RecoReq*>(base + o_req);
+  int32_t* fb = reinterpret_cast<int32_t*>(base + o_fb);
+  float* keys = reinterpret_cast<float*>(base + o_keys);
+  unsigned long long* lo = reinterpret_cast<unsigned long long*>(base + o_lo);
+  double* hi = reinterpret_cast<double*>(base + o_hi);
+  SB_CUDA(cudaMemcpyAsync(req_d, req, (size_t)R * sizeof(RecoReq), cudaMemcpyHostToDevice, st));
+  SB_CUDA(cudaMemsetAsync(fb, 0, (size_t)R * 4, st));
+  if (ctx->fb_count_dev.cap == 0) {
+    if ((rc = ctx->fb_count_dev.reserve(8))) return rc;
+    SB_CUDA(cudaMemsetAsync(ctx->fb_count_dev.p, 0, 8, st));
+  }
+  float *eps = nullptr, *rq = nullptr;
+  int32_t* ex_fb = nullptr;
+  if ((rc = dense_prep_queries(ctx, ix, ex_pad, M, M + kQbnMax, /*mma=*/true, nullptr, q16, &eps, &ex_fb, &rq, st)))
+    return rc;
+  dense_reco_norms_kernel<<<(M + 7) / 8, 256, 0, st>>>(ex_pad, M, ix.d_pad, ix.metric, eps, qn, cd);
+  SB_CUDA(cudaGetLastError());
+  ctx->launches += 1;
+  if ((rc = corpus_map(ix))) return rc;
+  const CUtensorMap& tm_rows = *reinterpret_cast<const CUtensorMap*>(ix.tm_rows);
+  const int total_tiles = (int)(n_pad / kTileRows);
+  const int grid = std::min(ctx->num_sms, total_tiles);
+  auto sel_kern = u8 ? dense_reco_select_kernel<SB_STORAGE_U8>
+                  : ix.storage == SB_STORAGE_F32 ? dense_reco_select_kernel<SB_STORAGE_F32>
+                                                 : dense_reco_select_kernel<SB_STORAGE_F16>;
+  auto fb_kern = u8 ? dense_reco_fallback_kernel<SB_STORAGE_U8>
+                 : ix.storage == SB_STORAGE_F32 ? dense_reco_fallback_kernel<SB_STORAGE_F32>
+                                                : dense_reco_fallback_kernel<SB_STORAGE_F16>;
+  for (int r0 = 0; r0 < R;) {
+    int r1 = r0 + 1, me = req[r0].m;
+    while (r1 < R && r1 - r0 < r_cap && me + req[r1].m <= e_cap) me += req[r1++].m;
+    const int nr = r1 - r0, e0 = req[r0].ex0;
+    const uint32_t* mask = nullptr;
+    int qs = 0;
+    if (p_off && p_off[r1] > p_off[r0] &&
+        (rc = dense_where_mask(ctx, ix, p_off, prog, pool, r0, nr, &mask, &qs, st)))
+      return rc;
+    int qbn = 16;
+    while (qbn < me) qbn <<= 1;
+    CUtensorMap tm_q;
+    if ((rc = encode_map(&tm_q, q16 + (size_t)e0 * ix.d_pad, qbn, ix.d_pad, qbn))) return rc;
+    MmaScanParams mp = {};
+    mp.inv_norm = ix.inv_norm;
+    mp.n = ix.n;
+    mp.kb_count = (ix.d_pad + kBK - 1) / kBK;   // a partial last box is zero-filled by the TMA unit
+    mp.num_tiles = total_tiles;
+    mp.tile_first = 0;
+    mp.tile_step = 1;
+    mp.stages = mma_stages(ctx, qbn, false, u8);
+    mp.prefetch = ctx->dense_prefetch;
+    mp.cand = reinterpret_cast<unsigned long long*>(keys);   // STORE: the key buffer, row stride capg
+    mp.capg = (int32_t)n_pad;
+    mp.mask_qs = me;
+    const size_t smem = mma_smem(qbn, mp.stages, false, u8);
+    {
+      ProfScope ps(ctx, SB_PROF_DENSE_SCAN, st);
+      rc = u8 ? dispatch_mma<false, false, SB_STORAGE_U8, true>(qbn, tm_rows, tm_q, mp, grid, smem, st)
+              : dispatch_mma<false, false, SB_STORAGE_F16, true>(qbn, tm_rows, tm_q, mp, grid, smem, st);
+      if (rc) return rc;
+    }
+    RecoCombineParams cp;
+    cp.keys = keys;
+    cp.ld = n_pad;
+    cp.n = ix.n;
+    cp.e0 = e0;
+    cp.r0 = r0;
+    cp.req = req_d;
+    cp.cd = cd;
+    cp.mask = mask;
+    cp.mask_qs = qs;
+    cp.lo = lo;
+    cp.hi = hi;
+    dense_reco_combine_kernel<<<dim3((unsigned)((ix.n + 255) / 256), (unsigned)nr), 256, 0, st>>>(cp);
+    RecoSelectParams sp;
+    sp.lo = lo;
+    sp.hi = hi;
+    sp.ld = n_pad;
+    sp.n = ix.n;
+    sp.r0 = r0;
+    sp.req = req_d;
+    sp.ex = ex_pad;
+    sp.qn = qn;
+    sp.ex_fb = ex_fb;
+    sp.slot = slot_view(ix);
+    sp.k = k;
+    sp.fallback = fb;
+    sp.out_ids = out_ids;
+    sp.out_scores = out_scores;
+    sp.out_counts = out_counts;
+    sp.mask = mask;
+    sp.mask_qs = qs;
+    sp.counter = ctx->fb_count_dev.as<unsigned long long>();
+    {
+      ProfScope ps(ctx, SB_PROF_DENSE_MERGE, st, 2);
+      sel_kern<<<nr, kRecoThreads, 0, st>>>(sp);
+      fb_kern<<<nr, kRecoThreads, 0, st>>>(sp);
+    }
+    SB_CUDA(cudaGetLastError());
+    ctx->launches += 1;   // the combine
+    r0 = r1;
+  }
+  return SB_OK;
 }

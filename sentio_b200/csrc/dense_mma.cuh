@@ -26,6 +26,20 @@ int dense_mma_topk_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* q_pad, int 
 // keys the scans cannot bound are raised here already (DESIGN.md K1e).
 int dense_prep_queries(sb_ctx* ctx, const DenseIndex& ix, const float* q_pad, int B, int rows, bool mma, float** qn_out,
                        __half* q16, float** eps_out, int32_t** fb_out, float** rq_out, cudaStream_t st);
+// Recommendation (DESIGN.md K1j): request r owns examples [ex0, ex0 + m) of the padded example rows, the first n_pos
+// positive, merged by strategy (SB_RECO_*).
+struct RecoReq {
+  int32_t ex0, m, n_pos, strategy;
+};
+// R validated requests over M examples (ex_pad: [M][d_pad] fp32 device), programs as sb_dense_topk_where (host arrays;
+// p_off == nullptr: unfiltered), k <= 1024, a Cosine or Dot slot with rows: the exact top-k of every request.
+int dense_reco_enqueue(sb_ctx* ctx, DenseIndex& ix, const float* ex_pad, int M, const RecoReq* req, int R, int k,
+                       const int32_t* p_off, const sb_pred* prog, const int32_t* pool, int64_t* out_ids,
+                       double* out_scores, int32_t* out_counts, cudaStream_t st);
+// dense.cu: the match mask of queries [c0, c0 + nq) (nq <= 256) of validated programs; bit (row % 32) of
+// (*mask)[(row / 32) * *qs + q - c0].  The mask lives in the context's filter buffer until the next filtered call.
+int dense_where_mask(sb_ctx* ctx, DenseIndex& ix, const int32_t* p_off, const sb_pred* prog, const int32_t* pool, int c0,
+                     int nq, const uint32_t** mask, int* qs, cudaStream_t st);
 // dense.cu: brute-force fp64 answer for every query whose fallback flag is raised (one CTA per query, idle CTAs exit)
 int dense_fallback_enqueue(sb_ctx* ctx, const DenseIndex& ix, const float* q_pad, int B, int k, const int32_t* fb,
                            int64_t* out_ids, double* out_scores, int32_t* out_counts, cudaStream_t st,

@@ -292,6 +292,55 @@ class B200Engine:
                                             _ptr(ids), _ptr(sc), _ptr(cnt)), "sb_dense_topk_where")
         return ids, sc, cnt
 
+    # recommendation strategies (DESIGN.md K1j); average_vector is one nearest query (dense_topk / dense_topk_where), the
+    # others are SB_RECO_* codes of sb_dense_recommend
+    RECO_STRATEGIES = {"average_vector": 0, "best_score": 1, "sum_scores": 2}
+
+    def dense_recommend(self, examples: np.ndarray, r_off, n_pos, strategies, k: int, programs=None, slot: int = 0):
+        """Exact top-k of R recommendation requests (``sb_dense_recommend``, DESIGN.md K1j).  ``examples`` [m, d] float32,
+        request r owns rows [r_off[r], r_off[r+1]), the first n_pos[r] positive; ``strategies`` [R] names from
+        ``RECO_STRATEGIES`` other than average_vector; ``programs`` as ``dense_topk_where`` (None = unfiltered).  Returns
+        (ids [R,k] int64, scores [R,k] float64, counts [R] int32)."""
+        from .payload_filter import PRED_DTYPE
+
+        ex = np.ascontiguousarray(np.atleast_2d(examples), dtype=np.float32)
+        m, d = ex.shape
+        if slot not in self.dense_dim:
+            raise SentioB200Error(f"dense slot {slot} has no index loaded")
+        if d != self.dense_dim[slot]:
+            raise ValueError(f"example dimension {d} != index dimension {self.dense_dim[slot]}")
+        r_off = np.ascontiguousarray(r_off, dtype=np.int32).reshape(-1)
+        R = len(r_off) - 1
+        n_pos = np.ascontiguousarray(n_pos, dtype=np.int32).reshape(-1)
+        codes = []
+        for s in strategies:
+            c = self.RECO_STRATEGIES.get(str(s).lower(), 0)
+            if c == 0:
+                raise ValueError(f"dense_recommend: strategy {s!r} is not one of best_score, sum_scores")
+            codes.append(c)
+        codes = np.ascontiguousarray(codes, dtype=np.int32)
+        if R < 0 or len(n_pos) != R or len(codes) != R:
+            raise ValueError("dense_recommend: r_off [R+1], n_pos [R] and strategies [R] must agree")
+        off = prog = pool = None
+        n_pool = 0
+        if programs is not None:
+            off, prog, pool = programs
+            off = np.ascontiguousarray(off, dtype=np.int32).reshape(-1)
+            prog = np.ascontiguousarray(prog).reshape(-1)
+            pool = np.ascontiguousarray(pool, dtype=np.int32).reshape(-1)
+            if prog.dtype != PRED_DTYPE:
+                raise ValueError("programs: prog must be a payload_filter.PRED_DTYPE array")
+            if len(off) != R + 1 or int(off[-1]) != len(prog):
+                raise ValueError("programs must be (p_off [R+1], prog [n], pool) with p_off[R] == n")
+            n_pool = len(pool)
+        ids = np.empty((R, k), dtype=np.int64)
+        sc = np.empty((R, k), dtype=np.float64)
+        cnt = np.empty(R, dtype=np.int32)
+        check(self._lib.sb_dense_recommend(self._h, slot, _ptr(ex), m, _ptr(r_off), _ptr(n_pos), _ptr(codes), R, int(k),
+                                           _ptr(off), _ptr(prog), _ptr(pool), n_pool, _ptr(ids), _ptr(sc), _ptr(cnt)),
+              "sb_dense_recommend")
+        return ids, sc, cnt
+
     def dense_groups(self, q: np.ndarray, field: int, limit: int, group_size: int, filters=None, slot: int = 0):
         """Grouped search (``sb_dense_groups``, DESIGN.md K1f): per query the best ``limit`` groups of tag column ``field``
         (groups ranked by their best row, rows with code -1 in no group), each with its best ``group_size`` rows, over

@@ -30,7 +30,7 @@ from .engine import B200Engine
 from .payload_filter import PayloadIndex
 
 __all__ = ["B200VectorStore", "ScoredPoint", "Record", "UpdateResult", "CollectionInfo", "Distance", "Datatype",
-           "PointGroup", "GroupsResult", "QueryResponse"]
+           "PointGroup", "GroupsResult", "QueryResponse", "RecommendStrategy"]
 
 
 @dataclass
@@ -86,6 +86,14 @@ class Datatype(enum.Enum):
     UINT8 = "uint8"
 
 
+class RecommendStrategy(enum.Enum):
+    """Qdrant's ``RecommendStrategy`` (DESIGN.md K1j, INTEGRATION.md).  AVERAGE_VECTOR searches avg(P) + (avg(P) - avg(N));
+    BEST_SCORE and SUM_SCORES merge the similarities of every row to every example (Cosine and Dot only)."""
+    AVERAGE_VECTOR = "average_vector"
+    BEST_SCORE = "best_score"
+    SUM_SCORES = "sum_scores"
+
+
 @dataclass
 class VectorParams:
     size: int
@@ -138,6 +146,20 @@ def parse_distance(dist) -> Distance:
 
 
 _ENGINE_METRIC = {Distance.COSINE: "cosine", Distance.DOT: "dot", Distance.EUCLID: "euclid"}
+
+
+def parse_strategy(strategy) -> RecommendStrategy:
+    """A recommendation strategy given as this module's ``RecommendStrategy``, ``qdrant_client``'s enum (read by
+    ``.name``), its value or a plain string, case-insensitive; ``None`` is AVERAGE_VECTOR, as in Qdrant.  Anything else
+    raises ``ValueError``."""
+    if strategy is None:
+        return RecommendStrategy.AVERAGE_VECTOR
+    name = _distance_name(strategy).strip().lower()
+    for t in RecommendStrategy:
+        if name in (t.name.lower(), t.value):
+            return t
+    raise ValueError(f"strategy {_distance_name(strategy)!r} is not supported "
+                     "(supported: average_vector, best_score, sum_scores)")
 
 
 def parse_datatype(dt) -> Datatype:
@@ -218,6 +240,27 @@ def _query_vector(query, where: str) -> np.ndarray:
     if q.ndim != 1:
         raise ValueError(f"{where}: the query must be one vector, got shape {q.shape}")
     return q
+
+
+MAX_RECO_EXAMPLES = 256   # examples of one recommendation request (one 256-column block of the scan)
+
+
+def _reco_example(e, where: str):
+    """A recommendation example: a point id (str, int or UUID) or one dense vector (float32)."""
+    if isinstance(e, bool):
+        raise ValueError(f"{where}: an example must be a point id or a vector, got {e!r}")
+    if isinstance(e, (str, int)) or hasattr(e, "hex"):
+        return e
+    if isinstance(e, dict) or hasattr(e, "indices"):
+        raise ValueError(f"{where}: named, sparse and multi-vector examples are not supported (one dense vector)")
+    try:
+        v = np.asarray(e, dtype=np.float32)
+    except (TypeError, ValueError) as err:
+        raise ValueError(f"{where}: an example must be a point id or a numeric vector ({err})") from None
+    if v.ndim != 1:
+        raise ValueError(f"{where}: named, sparse and multi-vector examples are not supported (one dense vector, "
+                         f"got shape {v.shape})")
+    return v
 
 
 def _points_columns(points):
@@ -605,6 +648,146 @@ class B200VectorStore:
                                 vector=vecs[j].tolist() if vecs is not None else None)
                     for j, (r, s_) in enumerate(zip(rows, sc))]))
             return out
+
+    def recommend(self, collection_name: str, positive=None, negative=None, query_filter=None, search_params=None,
+                  limit: int = 10, offset: int = 0, with_payload: bool = True, with_vectors: bool = False,
+                  score_threshold: float | None = None, using=None, lookup_from=None, strategy=None,
+                  **_ignored) -> list[ScoredPoint]:
+        """Qdrant ``recommend``: the exact best points "like the positive examples and unlike the negative ones", after
+        skipping ``offset``, at most ``limit`` of them, over the points matching ``query_filter`` (the ``query_points``
+        filter language).  An example is a point id (its stored vector, as ``retrieve(with_vectors=True)`` returns it) or
+        a vector; every id example is left out of the results.  ``strategy`` (None = average_vector):
+        average_vector searches avg(P) + (avg(P) - avg(N)) (avg(P) without negatives) with the scores of
+        ``query_points``; best_score and sum_scores merge the exact similarities to every example (Cosine and Dot;
+        INTEGRATION.md has the formulas).  ``score_threshold`` keeps scores >= it (distances <= it for Euclid
+        average_vector).  ``search_params`` is accepted: every search here is exact.  Unknown ids, NaN, wrong
+        dimensions, ``using``, ``lookup_from``, no examples, more than 256 of them and offset + limit + id examples
+        > 1024 raise ``ValueError`` before anything runs."""
+        req = SimpleNamespace(positive=positive, negative=negative, strategy=strategy, filter=query_filter, limit=limit,
+                              offset=offset, with_payload=with_payload, with_vector=with_vectors,
+                              score_threshold=score_threshold, using=using, lookup_from=lookup_from)
+        return self._recommend(collection_name, [req], "recommend")[0]
+
+    def recommend_batch(self, collection_name: str, requests: Sequence) -> list[list[ScoredPoint]]:
+        """Qdrant ``recommend_batch``: one ``recommend`` per ``RecommendRequest``-shaped request (``.positive``,
+        ``.negative``, ``.strategy``, ``.filter``, ``.limit``, ``.offset``, ``.with_payload``, ``.with_vector``,
+        ``.score_threshold``, ``.using``, ``.lookup_from``), answered by one device call per strategy family.  Each
+        answer is a cut of its request's exact order, so it equals the request run alone."""
+        return self._recommend(collection_name, list(requests), "recommend_batch")
+
+    def _recommend(self, collection_name: str, reqs: list, where: str) -> list[list[ScoredPoint]]:
+        col = self._get(collection_name)
+        if not reqs:
+            return []
+        listed = getattr(B200Engine, "RECO_STRATEGIES", {})
+        parsed = []
+        for r in reqs:
+            for attr in ("using", "lookup_from"):
+                if getattr(r, attr, None) is not None:
+                    raise ValueError(f"{where}: {attr} is not supported")
+            strat = parse_strategy(getattr(r, "strategy", None))
+            if strat.value not in listed:
+                raise ValueError(f"{where}: strategy {strat.value} is not supported by {B200Engine.__name__}")
+            if strat is not RecommendStrategy.AVERAGE_VECTOR and col.distance is Distance.EUCLID:
+                raise ValueError(f"{where}: strategy {strat.value} is not supported on a Euclid collection "
+                                 "(average_vector is)")
+            pos = [_reco_example(e, where) for e in (getattr(r, "positive", None) or [])]
+            neg = [_reco_example(e, where) for e in (getattr(r, "negative", None) or [])]
+            if not pos and not neg:
+                raise ValueError(f"{where}: give at least one positive or negative example")
+            if strat is RecommendStrategy.AVERAGE_VECTOR and not pos:
+                raise ValueError(f"{where}: average_vector needs at least one positive example")
+            if len(pos) + len(neg) > MAX_RECO_EXAMPLES:
+                raise ValueError(f"{where}: {len(pos) + len(neg)} examples exceed {MAX_RECO_EXAMPLES} per request")
+            for v in pos + neg:
+                if isinstance(v, np.ndarray):
+                    if len(v) != col.dim:
+                        raise ValueError(f"{where}: example vectors must have dimension {col.dim}, got {len(v)}")
+                    if not np.isfinite(v).all():
+                        raise ValueError(f"{where}: an example vector contains NaN or infinite values")
+            limit = getattr(r, "limit", None)
+            limit = 10 if limit is None else limit
+            offset = getattr(r, "offset", None) or 0
+            if not all(isinstance(v, int) and not isinstance(v, bool) for v in (limit, offset)) or limit < 1 \
+                    or offset < 0:
+                raise ValueError(f"{where}: limit must be an int >= 1 and offset an int >= 0")
+            flags = [getattr(r, "with_payload", True), getattr(r, "with_vector", getattr(r, "with_vectors", False))]
+            flags = [False if f is None else f for f in flags]
+            if not all(isinstance(f, bool) for f in flags):
+                raise ValueError(f"{where}: with_payload / with_vector must be True or False (selectors are not "
+                                 "supported)")
+            t = getattr(r, "score_threshold", None)
+            if t is not None and (isinstance(t, bool) or not isinstance(t, (int, float))):
+                raise ValueError(f"{where}: score_threshold must be a number")
+            parsed.append((strat, pos, neg, getattr(r, "filter", None), offset, limit, t, *flags))
+        with col.lock:
+            # resolve the id examples and check the depth before anything runs
+            plans = []
+            for strat, pos, neg, flt, offset, limit, t, wp, wv in parsed:
+                excl = set()
+                for e in pos + neg:
+                    if not isinstance(e, np.ndarray):
+                        if e not in col.row_of:
+                            raise ValueError(f"{where}: no point with id {e!r}")
+                        excl.add(col.row_of[e])
+                if offset + limit + len(excl) > MAX_QUERY_DEPTH:
+                    raise ValueError(f"{where}: offset + limit + id examples = {offset + limit + len(excl)} exceeds "
+                                     f"{MAX_QUERY_DEPTH}")
+                plans.append((excl, offset + limit + len(excl)))
+            id_rows = sorted({r for excl, _ in plans for r in excl})
+            stored = dict(zip(id_rows, col.engine.dense_fetch(id_rows, slot=0))) if id_rows else {}
+
+            def vec(e):
+                return e if isinstance(e, np.ndarray) else stored[col.row_of[e]]
+
+            results = [None] * len(parsed)
+            avg = [b for b, p in enumerate(parsed) if p[0] is RecommendStrategy.AVERAGE_VECTOR]
+            merged = [b for b, p in enumerate(parsed) if p[0] is not RecommendStrategy.AVERAGE_VECTOR]
+            for group in (avg, merged):
+                if not group:
+                    continue
+                k = max(1, min(max(plans[b][1] for b in group), max(len(col.ids), 1)))
+                filters = [parsed[b][3] for b in group]
+                programs = col.payload_index().compile_programs(filters) if any(f is not None for f in filters) \
+                    else None
+                if group is avg:
+                    qs = []
+                    for b in group:
+                        P = np.asarray([vec(e) for e in parsed[b][1]], np.float64)
+                        ap = P.sum(0) / len(P)
+                        if parsed[b][2]:
+                            N = np.asarray([vec(e) for e in parsed[b][2]], np.float64)
+                            ap = ap + (ap - N.sum(0) / len(N))
+                        qs.append(ap.astype(np.float32))
+                    q = np.stack(qs)
+                    out = col.engine.dense_topk_where(q, k, programs) if programs is not None \
+                        else col.engine.dense_topk(q, k)
+                else:
+                    ex, r_off, n_pos, strats = [], [0], [], []
+                    for b in group:
+                        strat, pos, neg = parsed[b][:3]
+                        ex.extend(vec(e) for e in pos + neg)
+                        r_off.append(len(ex))
+                        n_pos.append(len(pos))
+                        strats.append(strat.value)
+                    out = col.engine.dense_recommend(np.asarray(ex, np.float32), r_off, n_pos, strats, k,
+                                                     programs=programs)
+                for j, b in enumerate(group):
+                    results[b] = tuple(a[j] for a in out)
+            euclid = col.distance is Distance.EUCLID
+            answers = []
+            for (strat, pos, neg, flt, offset, limit, t, wp, wv), (excl, _), (ids, scores, count) in \
+                    zip(parsed, plans, results):
+                kept = [(int(r), float(s_)) for r, s_ in zip(ids[:int(count)], scores[:int(count)]) if int(r) not in excl]
+                kept = kept[offset:offset + limit]
+                if t is not None:   # the order is best first, so the points kept are a prefix
+                    kept = [(r, s_) for r, s_ in kept if (s_ <= t if euclid else s_ >= t)]
+                rows = [r for r, _ in kept]
+                vecs = col.engine.dense_fetch(rows, slot=0) if wv and rows else None
+                answers.append([ScoredPoint(id=col.ids[r], score=s_, payload=col.payloads[r] if wp else None,
+                                            vector=vecs[j].tolist() if vecs is not None else None)
+                                for j, (r, s_) in enumerate(kept)])
+            return answers
 
     def search_batch_arrays(self, collection_name: str, query_vectors: np.ndarray, limit: int):
         """Batched extension: (rows [B,k] int64, scores [B,k] float64, counts [B]) without Python objects."""
